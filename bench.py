@@ -1,5 +1,10 @@
 #!/usr/bin/env python
-"""Headline benchmark: Llama-3-8B ZeRO-3 bf16 training throughput (tokens/s, whole job).
+"""Headline benchmark: Llama-3.2-3B ZeRO-3 bf16 training throughput (tokens/s, whole job).
+
+The default model is sized for one 80 GB H100: Llama-3.2-3B's shape with an untied LM head (3.6 B parameters) needs ~50 GB
+of bf16 weights, fp32 master weights and Adam moments on a single rank, which leaves room for the activations of
+2 x 4096 tokens.  Larger presets
+(``--model llama3-8b``) need more ranks or ``--offload cpu``.
 
 Contract (see task statement): ``python bench.py --gpus N --steps K --warmup W`` (N>1 is launched
 under ``torch.distributed.run``).  W untimed warm-up steps, then exactly K timed steps bracketed by a
@@ -17,6 +22,10 @@ same config, same timing harness.
 
 Synthetic data (random token ids of the benchmark shape) and random-init weights: there is no network
 for datasets / checkpoints.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last device-timed step returned and produced as float32
+``.npy`` files: ``loss.npy`` (the loss of that step) and ``params_sample.npy`` (a fixed, seeded sample of the updated
+fp32 master weights), so that two builds can be compared output for output on identical inputs.
 """
 import argparse
 import json
@@ -29,7 +38,7 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-# same allocator setting for both arms: avoids fragmentation-induced OOMs near the 180 GB limit
+# same allocator setting for both arms: avoids fragmentation-induced OOMs near the HBM limit
 os.environ.setdefault("PYTORCH_CUDA_ALLOC_CONF", "expandable_segments:True")
 
 
@@ -39,7 +48,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--model", default="llama3-8b")
+    ap.add_argument("--model", default="llama3.2-3b")
     ap.add_argument("--seq", type=int, default=4096)
     ap.add_argument("--micro-batch", type=int, default=2)
     ap.add_argument("--zero-stage", type=int, default=3)
@@ -58,6 +67,8 @@ def parse():
     ap.add_argument("--clip", type=float, default=0.0, help="gradient_clipping (both arms)")
     ap.add_argument("--gas", type=int, default=1, help="gradient_accumulation_steps (both arms); a timed step = one "
                     "optimizer step = GAS micro-batches")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss and a seeded sample of the updated weights as .npy files")
     ap.add_argument("--local_rank", type=int, default=0)
     return ap.parse_args()
 
@@ -181,7 +192,7 @@ def common_config(args, world):
         "gradient_accumulation_steps": args.gas,
         "offload_optimizer": args.offload if args.offload == "none" else f"{args.offload} (ratio {args.offload_ratio})",
         "precision": "bf16 params/activations/grads-in-flight",
-        "l2": "working set (>= 100 GB of parameter/optimizer state streamed per step) >> 126 MB L2",
+        "l2": "working set (tens of GB of parameter/optimizer state streamed per step) >> 50 MB L2",
     }
 
 
@@ -310,11 +321,14 @@ def run_b200(args):
     def fwd(ids):
         return engine(input_ids=ids, labels=ids).loss if hf else engine(ids, labels=ids)
 
+    last_loss = []
+
     def step_dev(i):
         for k in range(gas):
             loss = fwd(dev[(i * gas + k) % n_batches])
             engine.backward(loss)
             engine.step()
+        last_loss[:] = [loss.detach()]
 
     def step_e2e(i):
         for k in range(gas):
@@ -346,6 +360,8 @@ def run_b200(args):
     l0 = native.launch_count
     t_dev = timed_loop(torch, ds.comm, world, args.steps, step_dev)
     launches = native.launch_count - l0
+    if args.dump_outputs and args.steps > 0:
+        dump_outputs(torch, engine, last_loss[0], args.dump_outputs, rank)
     t_e2e = timed_loop(torch, ds.comm, world, args.steps, step_e2e)
     clocks = sampler.stop() if rank == 0 else None
     # exposed (non-overlapped) communication: 2 extra, untimed-for-throughput steps with every compute-stream
@@ -382,8 +398,8 @@ def run_b200(args):
         else:
             flops = cfg.flops_per_token(S) * val / world
         out = {
-            "metric": ("tokens/sec (whole job, device-timed, max over ranks) Llama-3-8B ZeRO-3 bf16 training"
-                       if (args.model == "llama3-8b" and args.zero_stage == 3) else
+            "metric": ("tokens/sec (whole job, device-timed, max over ranks) Llama-3.2-3B ZeRO-3 bf16 training"
+                       if (args.model == "llama3.2-3b" and args.zero_stage == 3) else
                        f"tokens/sec (whole job, device-timed, max over ranks) {args.model} ZeRO-{args.zero_stage} bf16 training"),
             "value": val,
             "unit": "tokens/s",
@@ -399,8 +415,8 @@ def run_b200(args):
             "impl": "b200",
             "config": common_config(args, world),
             "details": {
-                "model_impl": "transformers.LlamaForCausalLM (sdpa)" if hf else "deepspeed_b200.models.llama (fused sm_100a kernels)",
-                "optimizer_impl": "fused sm_100a AdamW kernel",
+                "model_impl": "transformers.LlamaForCausalLM (sdpa)" if hf else "deepspeed_b200.models.llama (fused sm_90a kernels)",
+                "optimizer_impl": "fused sm_90a AdamW kernel",
                 "activation_checkpoint_layers": cfg.checkpoint_layers if not hf else None,
                 "hf_gradient_checkpointing": hf_ckpt if hf else None,
                 "fused_in_backward_optimizer": bool(engine.optimizer.fused_in_backward),
@@ -426,13 +442,35 @@ def run_b200(args):
         print(json.dumps(out), flush=True)
 
 
+DUMP_PER_PARAM = 4096  # fp32 master-weight elements sampled per parameter tensor by --dump-outputs
+
+
+def dump_outputs(torch, engine, loss, out_dir, rank):
+    """Loss of the last timed step and a fixed, seeded sample of the fp32 master weights it produced (rank 0 writes)."""
+    import numpy as np
+    from deepspeed_b200.utils.tensor_fragment import safe_get_full_fp32_param
+    torch.cuda.synchronize()
+    sample = []
+    for i, p in enumerate(q for q in engine.module.parameters() if q.requires_grad):
+        full = safe_get_full_fp32_param(p).detach().reshape(-1)  # collective under ZeRO-3: every rank takes part
+        g = torch.Generator().manual_seed(i)
+        idx = torch.randint(full.numel(), (min(full.numel(), DUMP_PER_PARAM), ), generator=g)
+        sample.append(full[idx.to(full.device)].float().cpu())
+        del full
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss)], dtype=np.float32))
+    np.save(os.path.join(out_dir, "params_sample.npy"), torch.cat(sample).numpy())
+
+
 def _gemm_choice_summary():
     """Which implementation served each distinct GEMM problem of the step (persisted table / first-use measurement)."""
     from deepspeed_b200.ops import gemm
     used = gemm.tuning_table()
     own = sorted(k for k, v in used.items() if v == "own")
     lib = sorted(k for k, v in used.items() if v == "lib")
-    return {"own_tcgen05": len(own), "cublas": len(lib), "cublas_shapes": lib, "measured_online": gemm.tuning_measurements()}
+    return {"own_wgmma": len(own), "cublas": len(lib), "cublas_shapes": lib, "measured_online": gemm.tuning_measurements()}
 
 
 def run_reference(args):
@@ -444,7 +482,7 @@ def run_reference(args):
         return
     sys.path.insert(0, ref_dir)
     os.environ.setdefault("TORCH_EXTENSIONS_DIR", os.path.join(ref_dir, "_torch_extensions"))
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("DS_SKIP_CUDA_CHECK", "1")
     try:
         import torch

@@ -1,4 +1,4 @@
-"""deepspeed_b200 -- a Blackwell-native (sm_100a) distributed training / inference framework with the
+"""deepspeed_b200 -- a Hopper-native (sm_90a) distributed training / inference framework with the
 capabilities and user-facing contract of DeepSpeed.
 
 Public API parity: reference ``deepspeed/__init__.py`` (``initialize :69``, ``init_inference :291``,

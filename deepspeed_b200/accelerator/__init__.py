@@ -2,9 +2,9 @@
 
 Parity target: reference ``accelerator/abstract_accelerator.py`` (the 69-method ABC) and
 ``accelerator/real_accelerator.py:51 get_accelerator``.  The reference dispatches over eight
-vendors; this framework is B200-only, so there are exactly two concrete devices:
+vendors; this framework is H100-only, so there are exactly two concrete devices:
 
-* :class:`B200Accelerator` -- CUDA sm_100a, NCCL over NVLink 5.
+* :class:`B200Accelerator` -- CUDA sm_90a, NCCL over NVLink 5.
 * :class:`HostAccelerator` -- CPU + gloo, used by the no-GPU test tier and by the
   GPT-2/gloo plumbing config in BASELINE.json.
 

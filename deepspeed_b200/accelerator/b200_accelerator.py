@@ -1,7 +1,7 @@
-"""CUDA sm_100a accelerator (the product device).
+"""CUDA sm_90a accelerator (the product device).
 
 Reference counterpart: ``accelerator/cuda_accelerator.py``.  Differences by design: no
-compute-capability sweep (the only supported arch is 10.0a), NCCL is the only collective
+compute-capability sweep (the only supported arch is 9.0a), NCCL is the only collective
 backend, and graph capture / stream / event helpers are exposed because the engines use CUDA
 graphs and side streams as first-class scheduling tools rather than a tracing compiler.
 """
@@ -11,8 +11,7 @@ import torch
 
 from .base import AcceleratorBase
 
-SM_COUNT_B200 = 148
-HBM_BYTES_B200 = 180 * (1 << 30)
+SM_COUNT_H100 = 132  # reported when no device is visible
 
 
 class B200Accelerator(AcceleratorBase):
@@ -47,11 +46,8 @@ class B200Accelerator(AcceleratorBase):
     @functools.lru_cache(None)
     def sm_count(self, device_index=None):
         if not torch.cuda.is_available():
-            return SM_COUNT_B200
+            return SM_COUNT_H100
         return torch.cuda.get_device_properties(device_index or 0).multi_processor_count
-
-    def is_blackwell(self, device_index=None):
-        return torch.cuda.is_available() and self.device_capability(device_index)[0] == 10
 
     # ---- rng ------------------------------------------------------------------------------
     def random(self):

@@ -99,7 +99,7 @@ class AcceleratorBase:
         return [torch.float, torch.half, torch.bfloat16]
 
     def is_triton_supported(self):
-        # No Triton anywhere in this framework: sm_100a CUDA only.
+        # No Triton anywhere in this framework: sm_90a CUDA only.
         return False
 
     # ---- rng ------------------------------------------------------------------------------

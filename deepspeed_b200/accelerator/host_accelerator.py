@@ -37,9 +37,6 @@ class HostAccelerator(AcceleratorBase):
     def sm_count(self, device_index=None):
         return psutil.cpu_count(logical=False) or 1
 
-    def is_blackwell(self, device_index=None):
-        return False
-
     def random(self):
         return torch.random
 

@@ -20,7 +20,7 @@ def get_accelerator():
     import torch
     forced = os.environ.get("DSB200_ACCELERATOR", os.environ.get("DS_ACCELERATOR"))
     if forced is not None and forced not in SUPPORTED:
-        raise ValueError(f"accelerator {forced!r} is not supported; this framework targets B200 (cuda) "
+        raise ValueError(f"accelerator {forced!r} is not supported; this framework targets H100 (cuda) "
                          f"with a cpu/gloo tier for tests. Choose from {SUPPORTED}.")
     name = forced or ("cuda" if torch.cuda.is_available() else "cpu")
     if name == "cuda":

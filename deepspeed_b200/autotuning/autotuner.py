@@ -3,7 +3,7 @@
 Flow parity with reference ``autotuning/autotuner.py`` (``tune :404``): (1) model-info profiling run, (2) for each
 ZeRO stage that fits in memory (estimator below), sweep micro-batch sizes, (3) tune the stage's knob space with
 the chosen tuner around the best micro-batch size, (4) write the optimal config + a results table.  Memory
-arithmetic uses B200's 180 GB HBM via ``torch.cuda.mem_get_info`` when a GPU is visible.
+arithmetic uses H100's 80 GB HBM via ``torch.cuda.mem_get_info`` when a GPU is visible.
 """
 import copy
 import json
@@ -74,7 +74,7 @@ class Autotuner:
                 return torch.cuda.get_device_properties(0).total_memory
         except Exception:
             pass
-        return 180 * (1 << 30)
+        return 80 * (1 << 30)
 
     def get_model_num_params(self):
         return (self.model_info or {}).get(K.MODEL_INFO_NUM_PARAMS)

@@ -1,7 +1,7 @@
 """``deepspeed_b200.comm`` -- a torch.distributed-shaped facade.
 
 Parity target: reference ``deepspeed/comm/comm.py`` + ``comm/torch.py`` (``TorchBackend``).
-Design notes (B200-first):
+Design notes (H100-first):
 
 * Rendezvous, scalar reductions, barriers and the multi-node / CPU tiers ride on
   ``torch.distributed`` (NCCL on device, gloo on host).  Bulk ZeRO traffic has a second path --
@@ -148,7 +148,7 @@ def init_distributed(dist_backend: Optional[str] = None,
                      world_size: int = -1):
     """Initialise the process group (reference: comm/comm.py:625).
 
-    ``dist_backend`` defaults to the accelerator's backend (``nccl`` on B200, ``gloo`` on host).
+    ``dist_backend`` defaults to the accelerator's backend (``nccl`` on H100, ``gloo`` on host).
     """
     global _initialized_here, cdb
     if config is not None:
@@ -323,7 +323,7 @@ def all_reduce(tensor, op=ReduceOp.SUM, group=None, async_op=False):
 def inference_all_reduce(tensor, op=ReduceOp.SUM, group=None):
     """Latency-optimised all-reduce used by TP inference (reference: comm/torch.py:171).
 
-    On B200 the fast path is the one-shot NVLS ``multimem`` kernel in :mod:`comm.symm`; fall back
+    On H100 the fast path is the one-shot NVLS ``multimem`` kernel in :mod:`comm.symm`; fall back
     to NCCL when the tensor is not in a symmetric arena or on host.
     """
     from . import symm

@@ -1,6 +1,6 @@
 """Symmetric (peer-mapped) memory + in-kernel NVLink collectives.
 
-This is the B200-native replacement for "NCCL call on a side stream" on the two ZeRO hot paths
+This is the H100-native replacement for "NCCL call on a side stream" on the two ZeRO hot paths
 (SURVEY.md 5.8): buffers are allocated with the CUDA VMM API, exported as POSIX file descriptors,
 exchanged between the ranks of one node over a unix-domain socket (``SCM_RIGHTS``) and mapped into
 every rank's address space, so a kernel can ``ld``/``st`` a peer's buffer over NVLink.  A

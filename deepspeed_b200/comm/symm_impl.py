@@ -247,7 +247,7 @@ class SymmContext:
     def all_gather_matmul(self, a, full, shard, shard_numel, w_offset, n_rows, k, chunk_bytes=1 << 20, comm_ctas=32):
         """``a [M,K] @ W^T`` where ``W [n_rows, K]`` lives ``w_offset`` elements into the gathered unit buffer
         ``full`` — ONE kernel that pulls every rank's shard over NVLink (trailing ``comm_ctas`` CTAs, chunk flags
-        with release/acquire) while the tcgen05 tiles of rows that already arrived are being multiplied.
+        with release/acquire) while the wgmma tiles of rows that already arrived are being multiplied.
         Returns ``(out [M, n_rows])``; on return-to-stream the whole unit is resident in ``full``."""
         from deepspeed_b200.ops.kernels import gemm_sm100
         shards, _ = self._peers(shard)

@@ -1,4 +1,4 @@
-// Paged-KV attention for ragged (continuous-batching) inference on sm_100a.
+// Paged-KV attention for ragged (continuous-batching) inference on sm_90a.
 //
 // One CTA per (query token, query head).  K/V live in a blocked cache laid out by `kv_rotary_append`
 // (moe_ragged.cu): cache[block][slot][k|v][kv_head][d].  Each warp walks a strided subset of the visible
@@ -97,7 +97,7 @@ paged_attention_kernel(const T* __restrict__ q, const T* __restrict__ cache, T* 
 //     fetched once per KV head instead of once per query head.
 //   * memory-level parallelism: every lane keeps U=4 independent 16-byte K loads and 4 V loads in flight; a warp
 //     load instruction covers 32/LPK whole keys (LPK = D/8 lanes per key), i.e. 512 contiguous-row bytes.
-//   * split-KV: long contexts are cut into `nsplit` ranges so small decode batches still fill 148 SMs; partial
+//   * split-KV: long contexts are cut into `nsplit` ranges so small decode batches still fill 132 SMs; partial
 //     (m, l, acc) triples go to a workspace and a tiny merge kernel combines them.
 // The per-key dot product is reduced over only LPK lanes; the running max is shared by the whole warp so all lanes
 // rescale identically.
@@ -249,7 +249,7 @@ paged_decode_kernel(const T* __restrict__ q, const T* __restrict__ cache, T* __r
 //   * O = P V: the S accumulators of two 8-key tiles ARE the A fragment (keys 2t,2t+1 | 2t+8,2t+9); lane (g, t) loads
 //     16 bytes at d = 64 G + 8 g of those four keys' V rows and packs (V[2t][d], V[2t+1][d]) with one byte-permute, i.e.
 //     output column g of n-tile j is d = 64 G + 8 g + j (undone when the result is written).
-// (mma.sync on purpose: M is 1..8 useful rows - a tcgen05 tile would be > 90 % padding - and the kernel is bound by the
+// (mma.sync on purpose: M is 1..8 useful rows - a wgmma tile would be > 90 % padding - and the kernel is bound by the
 // KV stream.)
 // ---------------------------------------------------------------------------------------------------------------------
 template <typename T>

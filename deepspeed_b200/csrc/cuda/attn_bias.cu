@@ -7,8 +7,8 @@
 //   * Block-sparse attention (reference Triton SDD / DSD / softmax in ops/sparse_attention/{matmul.py, softmax.py}): a
 //     [H, L/bs, L/bs] 0/1 layout decides which score blocks exist; key-padding / attention masks ride the two bias slots.
 //
-// Why mma.sync and not tcgen05 here: with D <= 64 the two GEMMs of a score tile are 4*D <= 256 FLOP per score while every
-// score still costs one exp2 and (backward) one TMEM read each for S and dP.  At TMEM's ~16 fp32 / clk / SM the tcgen05
+// Why mma.sync and not wgmma here: with D <= 64 the two GEMMs of a score tile are 4*D <= 256 FLOP per score while every
+// score still costs one exp2 and (backward) one registers read each for S and dP.  At registers's ~16 fp32 / clk / SM the wgmma
 // formulation is capped at the SFU rate before the tensor core matters, and the fixed 128-row tile wastes most of an MSA
 // row of 100-300 residues.  Register accumulators (m16n8k16, 16 query rows per warp) have no such read port: S, P, dP, dS
 // never leave the register file, P / dS are re-used in place as the A operand of the second GEMM.

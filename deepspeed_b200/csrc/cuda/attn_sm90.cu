@@ -1,0 +1,613 @@
+// Training attention for sm_90a: causal / full softmax(Q K^T / sqrt(d)) V with grouped-query heads, head dim 128, bf16.
+//
+// Forward -- one CTA per (128 query rows, query head, batch):
+//   warp 8      TMA producer: Q once, then a 3-stage ring of K and V tiles (64 keys x 128 dims = 16 KiB each)
+//   warps 0-7   two consumer warpgroups, 64 query rows each: S = Q K_j^T with wgmma (both operands in shared memory,
+//               accumulators in registers), online softmax in the log2 domain (ex2.approx) on the accumulator fragments,
+//               then O += P V_j with P taken straight from registers as the A operand (the m64n64 accumulator layout is the
+//               m64k16 A-fragment layout) and V_j read MN-major from shared memory; at the end O / l -> bf16 -> global and
+//               the log-sum-exp for backward.
+//   S, P never touch shared or global memory; K/V tiles are shared by the query heads of a GQA group through L2.
+// Backward recomputes S / P per (query block, key block) pair from Q, K and the saved LSE with the same tile machinery
+// and produces dQ, dK, dV.
+//
+// Reference role: the reference has no training attention kernel of its own for HF-style models (it calls flash-attn,
+// sequence/fpdt_layer.py:235); its BERT-era fused layer is csrc/transformer/softmax_kernels.cu + cuBLAS strided batched GEMMs.
+#include "dsb_tc.cuh"
+
+namespace dsb {
+namespace attn {
+using namespace dsb::tc;
+
+constexpr int BQ = 128, BS = 64, D = 128;
+constexpr int kThreads = 288;                            // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int kProducer = 256;                           // thread index of the producer
+constexpr uint32_t TILE = BS * D * 2;                    // 16 KiB: [64 x 128] bf16 = 2 TMA boxes of [64 x 64]
+constexpr uint32_t HALF = TILE / 2;                      // 8 KiB box (one 128-byte swizzle span of 64 bf16 per row)
+constexpr float kNegInf = -__builtin_huge_valf();
+
+// Operand descriptors of a [64 x 128] tile at `t`:
+//   K-major over the 128 columns (S = Q K^T: Q as A, K as B): 16-column step kk in 0..7
+__device__ __forceinline__ uint64_t desc_k(uint32_t t, int kk) { return desc_kmajor_sw128(t + (kk >> 2) * HALF + (kk & 3) * 32); }
+//   MN-major, rows as the reduction dimension, the 128 columns as N (O = P V: V as B): 16-row step kk in 0..3
+__device__ __forceinline__ uint64_t desc_mn(uint32_t t, int kk) { return desc_mnmajor_sw128(t + kk * 2048, HALF); }
+
+__device__ __forceinline__ void load_tile(uint32_t dst, const CUtensorMap* map, uint32_t bar, int col, int row)
+{
+    tma_load_2d(dst, map, bar, col, row);
+    tma_load_2d(dst + HALF, map, bar, col + 64, row);
+}
+
+// acc = A_tile(64 rows) x B_tile(64 rows)^T over the 128 columns: m64n64, 8 steps
+__device__ __forceinline__ void mma_rows_x_rows(float* acc, uint32_t a, uint32_t b)
+{
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_ss<0, 0>(acc, desc_k(a, kk), desc_k(b, kk), kk > 0 ? 1 : 0);
+}
+// acc[64 x 128] += P[64 x 64] (register fragments of an m64n64 fp32 block) x tile[64 rows x 128]
+__device__ __forceinline__ void mma_regs_x_tile(float* acc, const uint32_t (*frag)[4], uint32_t t)
+{
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_rs<1>(acc, frag[kk], desc_mn(t, kk), 1);
+}
+// m64n64 fp32 accumulator -> bf16 A fragments of four k16 steps
+__device__ __forceinline__ void to_frags(const float* s, uint32_t (*f)[4])
+{
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        f[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+        f[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+        f[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+        f[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+}
+__device__ __forceinline__ float quad_max(float v)
+{
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v)
+{
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+// store a 64 x 128 fp32 accumulator (times `mul`) as bf16 rows `row0 + r` (r < rows) of a [*, ld] matrix at column col0
+__device__ __forceinline__ void store_acc(const float* acc, __nv_bfloat16* base, int64_t ld, int row_local, int rows, int col0,
+                                          int c_in, float mul0, float mul1)
+{
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int r = row_local + 8 * i;
+        if (r >= rows) continue;
+        const float m = i ? mul1 : mul0;
+        __nv_bfloat16* dst = base + static_cast<int64_t>(r) * ld + col0 + c_in;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16(acc[4 * j + 2 * i] * m, acc[4 * j + 2 * i + 1] * m);
+    }
+}
+
+struct FwdParams {
+    __nv_bfloat16* o;   // [B*S, ld_o], head h at columns [h*D, (h+1)*D)
+    float* lse;         // [B, Hq, S] natural-log sum-exp of the scaled scores
+    int ld_o;
+    int S, Hq, Hkv;
+    float scale_log2;   // softmax scale * log2(e)
+    int causal;
+};
+
+namespace kf {  // forward shared-memory plan
+constexpr int KV_STAGES = 3;
+constexpr uint32_t SM_Q = 0;                              // 2 tiles (one per consumer warpgroup)
+constexpr uint32_t SM_KV = SM_Q + 2 * TILE;               // KV_STAGES x (K tile, V tile)
+constexpr uint32_t SM_BAR = SM_KV + KV_STAGES * 2 * TILE;
+constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
+}  // namespace kf
+
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                const __grid_constant__ CUtensorMap map_v, const FwdParams p)
+{
+    using namespace kf;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t q_full = sbase + SM_BAR;
+    auto kv_full = [&](int s) { return sbase + SM_BAR + 8 * (1 + s); };
+    auto kv_empty = [&](int s) { return sbase + SM_BAR + 8 * (1 + KV_STAGES + s); };
+
+    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
+    const int kvh = h / (p.Hq / p.Hkv);
+    const int row_base = b * p.S;
+    const int n_blocks = (p.S + BS - 1) / BS;
+    const int n_kv = p.causal ? min(n_blocks, (q0 + BQ) / BS) : n_blocks;
+
+    if (threadIdx.x == kProducer) {
+        mbar_init(q_full, 1);
+        for (int s = 0; s < KV_STAGES; ++s) {
+            mbar_init(kv_full(s), 1);
+            mbar_init(kv_empty(s), 8);  // one arrival per consumer warp
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kProducer) {
+        if (threadIdx.x == kProducer) {
+            prefetch_map(&map_q);
+            prefetch_map(&map_k);
+            prefetch_map(&map_v);
+            mbar_expect_tx(q_full, 2 * TILE);
+            load_tile(sbase + SM_Q, &map_q, q_full, h * D, row_base + q0);
+            load_tile(sbase + SM_Q + TILE, &map_q, q_full, h * D, row_base + q0 + BS);
+            for (int j = 0; j < n_kv; ++j) {
+                const int s = j % KV_STAGES;
+                mbar_wait(kv_empty(s), ((j / KV_STAGES) & 1) ^ 1);
+                mbar_expect_tx(kv_full(s), 2 * TILE);
+                const uint32_t dst = sbase + SM_KV + s * 2 * TILE;
+                load_tile(dst, &map_k, kv_full(s), kvh * D, row_base + j * BS);
+                load_tile(dst + TILE, &map_v, kv_full(s), kvh * D, row_base + j * BS);
+            }
+        }
+        return;
+    }
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const int qr0 = q0 + wg * BS;                              // first query row of this warpgroup
+    const int r_loc = 16 * (warp & 3) + (lane >> 2);          // this thread's rows: qr0 + r_loc (+8)
+    const int c_in = 2 * (lane & 3);
+    const uint32_t sq = sbase + SM_Q + wg * TILE;
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    float m_run[2] = {kNegInf, kNegInf}, l_run[2] = {0.f, 0.f};
+    mbar_wait(q_full, 0);
+
+    for (int j = 0; j < n_kv; ++j) {
+        const int s = j % KV_STAGES;
+        mbar_wait(kv_full(s), (j / KV_STAGES) & 1);
+        if (!(p.causal && j * BS > qr0 + BS - 1)) {  // a block entirely above the diagonal contributes nothing
+            const uint32_t sk = sbase + SM_KV + s * 2 * TILE, sv = sk + TILE;
+            float sc[32];
+            wgmma_fence();
+            mma_rows_x_rows(sc, sq, sk);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs<32>(sc);
+            float mx[2] = {kNegInf, kNegInf};
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int key = j * BS + 8 * jj + c_in + e;
+                        const int row = qr0 + r_loc + 8 * i;
+                        float x = sc[4 * jj + 2 * i + e] * p.scale_log2;
+                        if (key >= p.S || (p.causal && key > row)) x = kNegInf;
+                        sc[4 * jj + 2 * i + e] = x;
+                        mx[i] = fmaxf(mx[i], x);
+                    }
+            float alpha[2], m_use[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const float m_new = fmaxf(m_run[i], quad_max(mx[i]));
+                m_use[i] = m_new == kNegInf ? 0.f : m_new;  // a row with nothing visible yet keeps zero state
+                alpha[i] = ex2(m_run[i] - m_use[i]);        // 0 on the first block (m_run = -inf)
+                m_run[i] = m_new;
+                l_run[i] *= alpha[i];
+            }
+#pragma unroll
+            for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    o[4 * jj + 2 * i] *= alpha[i];
+                    o[4 * jj + 2 * i + 1] *= alpha[i];
+                }
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float pe = ex2(sc[4 * jj + 2 * i + e] - m_use[i]);
+                        sc[4 * jj + 2 * i + e] = pe;
+                        l_run[i] += pe;
+                    }
+            uint32_t pf[4][4];
+            to_frags(sc, pf);
+            wgmma_fence();
+            mma_regs_x_tile(o, pf, sv);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs<64>(o);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(kv_empty(s));
+    }
+
+    // ---- epilogue: O / l -> bf16 -> global, LSE ----------------------------------------------------------------------------
+    float inv[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        l_run[i] = quad_sum(l_run[i]);
+        inv[i] = l_run[i] > 0.f ? 1.f / l_run[i] : 0.f;
+    }
+    const int rows = p.S - qr0;  // rows of this warpgroup inside the sequence
+    store_acc(o, p.o + static_cast<int64_t>(row_base + qr0) * p.ld_o, p.ld_o, r_loc, rows < BS ? rows : BS, h * D, c_in,
+              inv[0], inv[1]);
+    if (p.lse != nullptr && (lane & 3) == 0) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int row = qr0 + r_loc + 8 * i;
+            if (row < p.S)
+                p.lse[(static_cast<int64_t>(b) * p.Hq + h) * p.S + row] = (m_run[i] + log2f(l_run[i])) * 0.6931471805599453f;
+        }
+    }
+}
+
+// =============================================================================================================================
+// Backward.  Two kernels, no atomics, every accumulator in registers:
+//   (A) dK / dV: one CTA per (128 keys, KV head, batch), 64 keys per consumer warpgroup, keeps K_j, V_j resident and streams
+//       (query head of the GQA group) x (64-row query block): dP^T = V dO^T and S^T = K Q^T (M = keys), P^T = 2^(S^T*c -
+//       lse[q]) and dS^T = P^T (dP^T - delta[q]) * scale on the fragments, then dV += P^T dO and dK += dS^T Q with P^T / dS^T
+//       as register A operands; dK / dV accumulate over ALL query heads of the group -- GQA needs no reduction pass.
+//   (B) dQ: one CTA per (128 queries, query head, batch) keeps Q, dO resident and streams 64-key blocks:
+//       S = Q K^T, dP = dO V^T, dS on the fragments, dQ += dS K.
+// S / P / dS are recomputed on chip; only Q, K, V, O, dO, LSE are read.  `delta = rowsum(dO * O)` and `lse * log2(e)` come
+// from a small pre-pass.
+// =============================================================================================================================
+struct BwdParams {
+    __nv_bfloat16 *dq, *dk, *dv;  // outputs, 2-D [B*S, ld]: head h at columns [h*D, +D)
+    int ld_dq, ld_dk, ld_dv;
+    const float* lse2;   // [B, Hq, S]  log-sum-exp * log2(e)
+    const float* delta;  // [B, Hq, S]  rowsum(dO * O)
+    int S, Hq, Hkv;
+    float scale, scale_log2;
+    int causal;
+};
+
+// delta[b,h,s] = sum_d dO * O ; lse2 = lse * log2(e).  One warp per (token, head) row of 128 elements.
+__global__ void __launch_bounds__(256)
+attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o, const float* __restrict__ lse,
+                     float* __restrict__ delta, float* __restrict__ lse2, int B, int S, int Hq, int ld_o, int ld_do)
+{
+    const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    const int64_t rows = static_cast<int64_t>(B) * S * Hq;
+    if (w >= rows) return;
+    const int h = static_cast<int>(w % Hq);
+    const int64_t t = w / Hq;  // token row b*S + s
+    const __nv_bfloat16* po = o + t * ld_o + h * D + lane * 4;
+    const __nv_bfloat16* pd = d_o + t * ld_do + h * D + lane * 4;
+    const uint2 a = *reinterpret_cast<const uint2*>(po);
+    const uint2 g = *reinterpret_cast<const uint2*>(pd);
+    float acc = 0.f;
+    acc = fmaf(__uint_as_float(a.x << 16), __uint_as_float(g.x << 16), acc);
+    acc = fmaf(__uint_as_float(a.x & 0xffff0000u), __uint_as_float(g.x & 0xffff0000u), acc);
+    acc = fmaf(__uint_as_float(a.y << 16), __uint_as_float(g.y << 16), acc);
+    acc = fmaf(__uint_as_float(a.y & 0xffff0000u), __uint_as_float(g.y & 0xffff0000u), acc);
+    acc = warp_reduce<SumOp>(acc);
+    if (lane == 0) {
+        const int b = static_cast<int>(t / S), s_ = static_cast<int>(t % S);
+        const int64_t idx = (static_cast<int64_t>(b) * Hq + h) * S + s_;
+        delta[idx] = acc;
+        lse2[idx] = lse[idx] * 1.4426950408889634f;
+    }
+}
+
+namespace kb {  // shared-memory plan of both backward kernels: 4 resident tiles + 2 stages x 2 streamed tiles
+constexpr int STAGES = 2;
+constexpr uint32_t SM_RES = 0;                            // [X_wg0, X_wg1, Y_wg0, Y_wg1]
+constexpr uint32_t SM_STR = SM_RES + 4 * TILE;            // STAGES x (X tile, Y tile)
+constexpr uint32_t SM_BAR = SM_STR + STAGES * 2 * TILE;
+constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
+}  // namespace kb
+
+// ---- (A) dK, dV ---------------------------------------------------------------------------------------------------------------
+// dK and dV both live in registers (128 fp32 per thread), so at the 168 registers a 288-thread CTA can launch with the
+// compiler spills a little and serialises the wgmma issue of this kernel.
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                     const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
+{
+    using namespace kb;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t res_full = sbase + SM_BAR;
+    auto full = [&](int s) { return sbase + SM_BAR + 8 * (1 + s); };
+    auto empty = [&](int s) { return sbase + SM_BAR + 8 * (1 + STAGES + s); };
+
+    const int k0 = blockIdx.x * BQ, kvh = blockIdx.y, b = blockIdx.z;
+    const int rep = p.Hq / p.Hkv;
+    const int row_base = b * p.S;
+    const int qb0 = p.causal ? k0 / BS : 0;  // query blocks before the first key of the CTA see none of its keys
+    const int n_qb = p.S / BS;
+
+    if (threadIdx.x == kProducer) {
+        mbar_init(res_full, 1);
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(full(s), 1);
+            mbar_init(empty(s), 8);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kProducer) {
+        if (threadIdx.x == kProducer) {
+            mbar_expect_tx(res_full, 4 * TILE);
+            for (int w = 0; w < 2; ++w) {
+                load_tile(sbase + SM_RES + w * TILE, &map_k, res_full, kvh * D, row_base + k0 + w * BS);
+                load_tile(sbase + SM_RES + (2 + w) * TILE, &map_v, res_full, kvh * D, row_base + k0 + w * BS);
+            }
+            int it = 0;
+            for (int qh = kvh * rep; qh < (kvh + 1) * rep; ++qh)
+                for (int qb = qb0; qb < n_qb; ++qb, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
+                    mbar_expect_tx(full(s), 2 * TILE);
+                    const uint32_t dst = sbase + SM_STR + s * 2 * TILE;
+                    load_tile(dst, &map_q, full(s), qh * D, row_base + qb * BS);
+                    load_tile(dst + TILE, &map_do, full(s), qh * D, row_base + qb * BS);
+                }
+        }
+        return;
+    }
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const int kr0 = k0 + wg * BS;
+    const int r_loc = 16 * (warp & 3) + (lane >> 2);
+    const int c_in = 2 * (lane & 3);
+    const uint32_t sk = sbase + SM_RES + wg * TILE, sv = sbase + SM_RES + (2 + wg) * TILE;
+    float dk[64], dv[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) dk[i] = dv[i] = 0.f;
+    mbar_wait(res_full, 0);
+
+    int it = 0;
+    for (int qh = kvh * rep; qh < (kvh + 1) * rep; ++qh) {
+        const float* lse2 = p.lse2 + (static_cast<int64_t>(b) * p.Hq + qh) * p.S;
+        const float* delta = p.delta + (static_cast<int64_t>(b) * p.Hq + qh) * p.S;
+        for (int qb = qb0; qb < n_qb; ++qb, ++it) {
+            const int s = it % STAGES;
+            mbar_wait(full(s), (it / STAGES) & 1);
+            if (!(p.causal && qb * BS + BS - 1 < kr0)) {
+                const uint32_t sq = sbase + SM_STR + s * 2 * TILE, sdo = sq + TILE;
+                float st[32], dpt[32];
+                wgmma_fence();
+                mma_rows_x_rows(dpt, sv, sdo);  // dP^T = V dO^T
+                mma_rows_x_rows(st, sk, sq);    // S^T  = K Q^T
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs<32>(st);
+                fence_regs<32>(dpt);
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int q = qb * BS + 8 * jj + c_in + e;
+                        const float l2 = __ldg(lse2 + q), dl = __ldg(delta + q);
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const int key = kr0 + r_loc + 8 * i;
+                            const int x = 4 * jj + 2 * i + e;
+                            const float pe = (p.causal && q < key) ? 0.f : ex2(fmaf(st[x], p.scale_log2, -l2));
+                            st[x] = pe;
+                            dpt[x] = pe * (dpt[x] - dl) * p.scale;
+                        }
+                    }
+                uint32_t pf[4][4], df[4][4];
+                to_frags(st, pf);
+                to_frags(dpt, df);
+                wgmma_fence();
+                mma_regs_x_tile(dv, pf, sdo);  // dV += P^T dO
+                mma_regs_x_tile(dk, df, sq);   // dK += dS^T Q
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs<64>(dv);
+                fence_regs<64>(dk);
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty(s));
+        }
+    }
+    const int64_t r0 = row_base + kr0;
+    store_acc(dk, p.dk + r0 * p.ld_dk, p.ld_dk, r_loc, BS, kvh * D, c_in, 1.f, 1.f);
+    store_acc(dv, p.dv + r0 * p.ld_dv, p.ld_dv, r_loc, BS, kvh * D, c_in, 1.f, 1.f);
+}
+
+// ---- (B) dQ -------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads, 1)
+attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
+                   const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
+{
+    using namespace kb;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t res_full = sbase + SM_BAR;
+    auto full = [&](int s) { return sbase + SM_BAR + 8 * (1 + s); };
+    auto empty = [&](int s) { return sbase + SM_BAR + 8 * (1 + STAGES + s); };
+
+    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
+    const int kvh = h / (p.Hq / p.Hkv);
+    const int row_base = b * p.S;
+    const int n_kv = p.causal ? (q0 + BQ) / BS : p.S / BS;
+
+    if (threadIdx.x == kProducer) {
+        mbar_init(res_full, 1);
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(full(s), 1);
+            mbar_init(empty(s), 8);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kProducer) {
+        if (threadIdx.x == kProducer) {
+            mbar_expect_tx(res_full, 4 * TILE);
+            for (int w = 0; w < 2; ++w) {
+                load_tile(sbase + SM_RES + w * TILE, &map_q, res_full, h * D, row_base + q0 + w * BS);
+                load_tile(sbase + SM_RES + (2 + w) * TILE, &map_do, res_full, h * D, row_base + q0 + w * BS);
+            }
+            for (int j = 0; j < n_kv; ++j) {
+                const int s = j % STAGES;
+                mbar_wait(empty(s), ((j / STAGES) & 1) ^ 1);
+                mbar_expect_tx(full(s), 2 * TILE);
+                const uint32_t dst = sbase + SM_STR + s * 2 * TILE;
+                load_tile(dst, &map_k, full(s), kvh * D, row_base + j * BS);
+                load_tile(dst + TILE, &map_v, full(s), kvh * D, row_base + j * BS);
+            }
+        }
+        return;
+    }
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const int qr0 = q0 + wg * BS;
+    const int r_loc = 16 * (warp & 3) + (lane >> 2);
+    const int c_in = 2 * (lane & 3);
+    const uint32_t sq = sbase + SM_RES + wg * TILE, sdo = sbase + SM_RES + (2 + wg) * TILE;
+    const int64_t stat = (static_cast<int64_t>(b) * p.Hq + h) * p.S + qr0 + r_loc;
+    const float l2[2] = {p.lse2[stat], p.lse2[stat + 8]};
+    const float dl[2] = {p.delta[stat], p.delta[stat + 8]};
+    float dq[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+    mbar_wait(res_full, 0);
+
+    for (int j = 0; j < n_kv; ++j) {
+        const int s = j % STAGES;
+        mbar_wait(full(s), (j / STAGES) & 1);
+        if (!(p.causal && j * BS > qr0 + BS - 1)) {
+            const uint32_t sk = sbase + SM_STR + s * 2 * TILE, sv = sk + TILE;
+            float sc[32], dp[32];
+            wgmma_fence();
+            mma_rows_x_rows(sc, sq, sk);   // S  = Q K^T
+            mma_rows_x_rows(dp, sdo, sv);  // dP = dO V^T
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs<32>(sc);
+            fence_regs<32>(dp);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int key = j * BS + 8 * jj + c_in + e;
+                        const int row = qr0 + r_loc + 8 * i;
+                        const int x = 4 * jj + 2 * i + e;
+                        const float pe = (p.causal && key > row) ? 0.f : ex2(fmaf(sc[x], p.scale_log2, -l2[i]));
+                        dp[x] = pe * (dp[x] - dl[i]) * p.scale;
+                    }
+            uint32_t df[4][4];
+            to_frags(dp, df);
+            wgmma_fence();
+            mma_regs_x_tile(dq, df, sk);  // dQ += dS K
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs<64>(dq);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty(s));
+    }
+    store_acc(dq, p.dq + static_cast<int64_t>(row_base + qr0) * p.ld_dq, p.ld_dq, r_loc, BS, h * D, c_in, 1.f, 1.f);
+}
+
+}  // namespace attn
+}  // namespace dsb
+
+using namespace dsb::attn;
+
+// q / k / v: 2-D bf16 tensors [B*S, *] (row stride ld_*), head `i` at columns [i*128, +128) -- for a packed QKV
+// projection output all three point into the same buffer.  o: [B*S, ld_o] (head h at h*128).  lse: fp32 [B, Hq, S] or null.
+DSB_EXPORT int dsb_attn_fwd_bf16(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int Hq,
+                                 int Hkv, int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
+                                 int v_cols, float scale, int causal, cudaStream_t stream)
+{
+    if (head_dim != D || S <= 0 || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
+    if (B > 1 && S % BQ) return -2;  // ragged lengths: one sequence per launch (rows of the next one would be read as keys)
+    if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+         reinterpret_cast<uintptr_t>(o)) & 15)
+        return -2;
+    CUtensorMap mq, mk, mv;
+    int rc;
+    const uint64_t rows = static_cast<uint64_t>(B) * S;
+    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
+    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
+    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kf::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    FwdParams p;
+    p.o = static_cast<__nv_bfloat16*>(o);
+    p.lse = lse;
+    p.ld_o = ld_o;
+    p.S = S;
+    p.Hq = Hq;
+    p.Hkv = Hkv;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.causal = causal;
+    dim3 grid((S + BQ - 1) / BQ, Hq, B);
+    attn_fwd_kernel<<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+// Backward.  q/k/v as in the forward; o, d_o: [B*S, ld] with head h at h*128; lse from the forward.
+// dq / dk / dv: 2-D outputs (may be column ranges of ONE packed buffer).  work: fp32 scratch of 2 * B * Hq * S elements.
+DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                                 void* dq, void* dk, void* dv, float* work, int B, int S, int Hq, int Hkv, int head_dim,
+                                 int ld_q, int ld_k, int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
+                                 int k_cols, int v_cols, float scale, int causal, cudaStream_t stream)
+{
+    if (head_dim != D || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
+    CUtensorMap mq, mk, mv, mdo;
+    int rc;
+    const uint64_t rows = static_cast<uint64_t>(B) * S;
+    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
+    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
+    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
+    if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * D, ld_do, BS))) return rc;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        e = cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    float* delta = work;
+    float* lse2 = work + static_cast<int64_t>(B) * Hq * S;
+    const int64_t prep_rows = static_cast<int64_t>(B) * S * Hq;
+    attn_bwd_prep_kernel<<<static_cast<unsigned>((prep_rows * 32 + 255) / 256), 256, 0, stream>>>(
+        static_cast<const __nv_bfloat16*>(o), static_cast<const __nv_bfloat16*>(d_o), lse, delta, lse2, B, S, Hq, ld_o, ld_do);
+    BwdParams p;
+    p.dq = static_cast<__nv_bfloat16*>(dq);
+    p.dk = static_cast<__nv_bfloat16*>(dk);
+    p.dv = static_cast<__nv_bfloat16*>(dv);
+    p.ld_dq = ld_dq;
+    p.ld_dk = ld_dk;
+    p.ld_dv = ld_dv;
+    p.lse2 = lse2;
+    p.delta = delta;
+    p.S = S;
+    p.Hq = Hq;
+    p.Hkv = Hkv;
+    p.scale = scale;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.causal = causal;
+    attn_bwd_dkdv_kernel<<<dim3(S / BQ, Hkv, B), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    attn_bwd_dq_kernel<<<dim3(S / BQ, Hq, B), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    DSB_CHECK_LAUNCH();
+    return 0;
+}

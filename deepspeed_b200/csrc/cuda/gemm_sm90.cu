@@ -1,0 +1,642 @@
+// Hand-written sm_90a GEMM: C[M,N] (bf16) = op(A)[M,K] x op(B)[N,K]^T, bf16 operands, fp32 accumulate.
+//
+//   * operands staged global -> shared by TMA (cp.async.bulk.tensor, 128-byte swizzle) through a 4-stage mbarrier ring;
+//     every operand box is [64 rows x 64 bf16], so K-major ([rows, k]) and MN-major ([k, rows]) operands share one ring
+//   * two consumer warpgroups each own 64 rows of the 128 x 256 tile and issue wgmma.m64n256k16 straight from the shared
+//     tiles (MN-major operands through the transpose bits), 128 fp32 accumulators per thread; a producer warpgroup hands
+//     its registers to the consumers (setmaxnreg) and one of its threads issues the TMA
+//   * persistent CTAs (one per SM) walk the tile list; the producer runs ahead into the next tile while the consumers
+//     run the epilogue of the current one
+//   * fused epilogues: plain store, accumulate into C (dW over micro-batches), SwiGLU (gate and up rows of the same 128
+//     features share one tile), dSwiGLU
+//   * grouped (MoE) form: the tile list is built on the device from the expert offsets (no host synchronisation)
+//   * OPTIONAL fused all-gather: when `ag` is given, the weight matrix B is being assembled in local memory from the
+//     other ranks' ZeRO shards *by this same kernel*: `ag.comm_ctas` CTAs pull the peers' shard bytes over NVLink
+//     (peer-mapped addresses) chunk by chunk and publish a per-chunk ready flag (st.release.gpu); the producer of each
+//     MMA CTA acquires the flag of the chunk(s) backing a B tile before loading it, and tiles are visited starting with
+//     the locally owned rows, so transfer and math overlap tile by tile with no NCCL call.
+//
+// The reference has no tensor-core GEMM of its own for training (cuBLAS via csrc/transformer/
+// cublas_wrappers.cu:65 or torch.matmul); this kernel is the framework's native path.
+#include "dsb_tc.cuh"
+
+namespace dsb {
+namespace gemm {
+using namespace dsb::tc;
+
+constexpr int BM = 128, BN = 256, BK = 64;
+constexpr int STAGES = 4;
+constexpr int kConsumerThreads = 256;                 // two warpgroups, 64 rows each
+constexpr int kThreads = kConsumerThreads + 128;      // + the producer warpgroup
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
+constexpr uint32_t BOX = 64 * 64 * 2;                 // one TMA box: 8 KiB
+constexpr uint32_t STAGE_BYTES = 6 * BOX;             // A: 2 boxes, B: 4 boxes
+constexpr uint32_t SMEM_BAR = STAGES * STAGE_BYTES;   // 192 KiB (also the all-gather ring: 3 x 64 KiB)
+constexpr int kMaxGroups = 256;
+constexpr uint32_t SMEM_GRP = SMEM_BAR + 256;         // grouped form: int tile_prefix[kMaxGroups + 1]
+constexpr uint32_t SMEM_TOTAL = SMEM_GRP + (kMaxGroups + 1) * 4 + 1024;
+
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read()
+{
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+// ---- fused all-gather descriptor ------------------------------------------------------------------------
+struct AgParams {
+    // B (= this unit's gathered weights) lives in `local_full`; rank p's shard is `shard_bytes` long and is
+    // found at peers[p] (peer-mapped VA).  Chunk c covers bytes [c*chunk_bytes, (c+1)*chunk_bytes) of the
+    // unit's flat buffer; flags[c] becomes `epoch` once the chunk is resident in local_full.
+    const void* peers[8];
+    void* local_full;
+    uint32_t* flags;
+    int64_t shard_bytes;
+    int64_t chunk_bytes;
+    int64_t b_offset_bytes;  // byte offset of B's first element inside the unit flat buffer
+    int64_t b_bytes;         // extent of B: its chunks are gathered FIRST so the multiply can start while the rest streams
+    int n_chunks;
+    int world;
+    int rank;
+    int comm_ctas;  // trailing CTAs of the grid that do the gathering
+    uint32_t epoch;
+    int enabled;
+};
+
+__device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* p)
+{
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_release_gpu_u32(uint32_t* p, uint32_t v)
+{
+    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// Gather role: CTA `ci` of `nc` copies chunks ci, ci+nc, ... in the order "own shard first, then rank+1, ...".
+// The copy is done by the TMA engine, not by SM load/store instructions: one elected thread streams each chunk through a
+// ring of 3 x 64 KiB shared-memory buffers with  cp.async.bulk (peer global -> smem, mbarrier complete_tx)  followed by
+// cp.async.bulk (smem -> local global, bulk_group);  192 KiB in flight per CTA hides the NVLink round trip, so a dozen
+// gather CTAs saturate the links while leaving their SMs' issue slots idle.
+constexpr uint32_t AG_PIECE = 64 * 1024;
+constexpr int AG_BUFS = 3;
+
+__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_smem),
+                 "l"(src), "r"(bytes), "r"(bar)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src_smem, uint32_t bytes)
+{
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src_smem), "r"(bytes)
+                 : "memory");
+}
+
+__device__ void ag_gather_role(const AgParams& ag, int ci, int nc, uint8_t* smem)
+{
+    if (threadIdx.x != 0) return;
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t bar0 = sbase + AG_BUFS * AG_PIECE;  // AG_BUFS mbarriers after the ring
+    for (int b = 0; b < AG_BUFS; ++b) mbar_init(bar0 + 8 * b, 1);
+    fence_barrier_init();
+    const int chunks_per_shard = static_cast<int>(ag.shard_bytes / ag.chunk_bytes);
+    // chunks holding the matrix this very kernel multiplies by go first (pass 0), the rest of the unit follows (pass 1)
+    const int b_c0 = static_cast<int>(ag.b_offset_bytes / ag.chunk_bytes);
+    const int b_c1 = static_cast<int>((ag.b_offset_bytes + ag.b_bytes - 1) / ag.chunk_bytes);
+    uint32_t issued = 0;           // pieces issued so far (ring position = issued % AG_BUFS)
+    for (int pass = 0; pass < 2; ++pass)
+    for (int j = ci; j < ag.n_chunks; j += nc) {
+        // visit order: shards rotated so that every rank starts pulling from a different peer
+        const int k = j / chunks_per_shard;
+        const int within = j - k * chunks_per_shard;
+        const int peer = (ag.rank + k) % ag.world;
+        const int chunk = peer * chunks_per_shard + within;
+        if ((chunk >= b_c0 && chunk <= b_c1) != (pass == 0)) continue;
+        const int64_t off = static_cast<int64_t>(within) * ag.chunk_bytes;
+        const char* src = static_cast<const char*>(ag.peers[peer]) + off;
+        char* dst = static_cast<char*>(ag.local_full) + static_cast<int64_t>(peer) * ag.shard_bytes + off;
+        const int n_pieces = static_cast<int>((ag.chunk_bytes + AG_PIECE - 1) / AG_PIECE);
+        // software pipeline inside the chunk: loads run AG_BUFS-1 pieces ahead of the stores
+        int loaded = 0, stored = 0;
+        uint32_t first = issued;
+        while (stored < n_pieces) {
+            while (loaded < n_pieces && loaded - stored < AG_BUFS) {
+                const uint32_t slot = (first + loaded) % AG_BUFS;
+                // the store that last read this slot must have finished reading shared memory
+                if (first + loaded >= static_cast<uint32_t>(AG_BUFS)) tma_store_wait_read<0>();
+                const int64_t po = static_cast<int64_t>(loaded) * AG_PIECE;
+                const int64_t rem = ag.chunk_bytes - po;
+                const uint32_t bytes = static_cast<uint32_t>(rem < static_cast<int64_t>(AG_PIECE) ? rem : AG_PIECE);
+                mbar_expect_tx(bar0 + 8 * slot, bytes);
+                bulk_g2s(sbase + slot * AG_PIECE, src + po, bytes, bar0 + 8 * slot);
+                ++loaded;
+            }
+            const uint32_t n = first + stored;
+            const uint32_t slot = n % AG_BUFS;
+            mbar_wait(bar0 + 8 * slot, (n / AG_BUFS) & 1);
+            const int64_t po = static_cast<int64_t>(stored) * AG_PIECE;
+            const int64_t rem2 = ag.chunk_bytes - po;
+            const uint32_t bytes = static_cast<uint32_t>(rem2 < static_cast<int64_t>(AG_PIECE) ? rem2 : AG_PIECE);
+            bulk_s2g(dst + po, sbase + slot * AG_PIECE, bytes);
+            tma_store_commit();
+            ++stored;
+        }
+        issued = first + n_pieces;
+        tma_store_wait_all();  // the chunk's bytes are written before the flag is published
+        __threadfence();
+        st_release_gpu_u32(ag.flags + chunk, ag.epoch);
+    }
+}
+
+// Wait until every chunk overlapping B rows [n0, n0+rows) is resident.
+__device__ __forceinline__ void ag_wait_rows(const AgParams& ag, int n0, int rows, int K)
+{
+    const int64_t lo = ag.b_offset_bytes + static_cast<int64_t>(n0) * K * 2;
+    const int64_t hi = lo + static_cast<int64_t>(rows) * K * 2;
+    int c0 = static_cast<int>(lo / ag.chunk_bytes);
+    int c1 = static_cast<int>((hi - 1) / ag.chunk_bytes);
+    if (c1 >= ag.n_chunks) c1 = ag.n_chunks - 1;
+    for (int c = c0; c <= c1; ++c) {
+        while (ld_acquire_gpu_u32(ag.flags + c) != ag.epoch) __nanosleep(64);
+    }
+    // the chunk was written through the async proxy (bulk copies) and is about to be read through it (TMA loads)
+    asm volatile("fence.proxy.async;" ::: "memory");
+}
+
+static_assert(AG_BUFS * AG_PIECE + 8 * AG_BUFS <= SMEM_TOTAL, "all-gather ring must fit the GEMM's shared memory");
+
+// ---- fused epilogues ------------------------------------------------------------------------------------------
+// EPI_STORE    C = acc
+// EPI_ACCUM    C = C + acc                                   (dW accumulation over micro-batches: no addmm, no memset)
+// EPI_SWIGLU   B = [gate; up] stacked ([2I, K]); a tile multiplies 128 gate rows and the matching 128 up rows so
+//              accumulator columns 0-127 / 128-255 are gate / up of the SAME 128 features:  C[M, I] = silu(gate) * up,
+//              optionally gate|up saved to out2 [M, 2I] for backward.
+// EPI_DSWIGLU  acc = d_act tile (dY W_down); aux = saved gate|up [M, 2I]:
+//              dgate = acc * up * silu'(gate) -> C (the [M, I] left half of dgate_up),  dup = acc * silu(gate) -> out2 + I.
+// (cuBLAS cannot express the last two: they remove one full pass over the [tokens, 2I] / [tokens, I] activations each.)
+enum : int { EPI_STORE = 0, EPI_ACCUM = 1, EPI_SWIGLU = 2, EPI_DSWIGLU = 3 };
+enum : int { MODE_PLAIN = 0, MODE_GROUPED = 1, MODE_ALLGATHER = 2 };
+
+struct EpiParams {
+    const __nv_bfloat16* aux;  // DSWIGLU: saved gate|up
+    __nv_bfloat16* out2;       // SWIGLU: gate|up save (nullable); DSWIGLU: dgate_up base (dup goes to + inter)
+    __nv_bfloat16* c;          // output
+    int ld_aux, ld_out2, ldc;
+    int inter;                 // I
+    int group_m;               // rasterisation: m-blocks per L2 super-group
+    const int* offsets;        // grouped: expert row offsets [E + 1] on the device
+    int E;
+};
+
+__device__ __forceinline__ float silu_f(float g) { return g / (1.f + __expf(-g)); }
+__device__ __forceinline__ float dsilu_f(float g)
+{
+    const float sg = 1.f / (1.f + __expf(-g));
+    return sg * (1.f + g * (1.f - sg));
+}
+
+// Grouped rasterisation: tiles are numbered so that `group_m` consecutive m-blocks share every n-block before the next
+// group starts -- one wave of CTAs then touches ~group_m A-blocks and ~CTAs/group_m B-blocks instead of all A-blocks
+// and a few B-blocks, which keeps the wave's operand set inside L2 for the wide (N = 28672 / 128256) problems.
+__device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int group_m, int& m_blk, int& n_blk)
+{
+    const int per_group = group_m * num_n;
+    const int g = tile / per_group;
+    const int first_m = g * group_m;
+    const int gm = (num_m - first_m) < group_m ? (num_m - first_m) : group_m;
+    const int local = tile - g * per_group;
+    m_blk = first_m + local % gm;
+    n_blk = local / gm;
+}
+
+__device__ __forceinline__ float2 ld_bf16x2(const __nv_bfloat16* p)
+{
+    return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+}
+__device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float lo, float hi)
+{
+    *reinterpret_cast<uint32_t*>(p) = pack_bf16(lo, hi);
+}
+
+// Where one tile lives: first row of A / C, rows of C it may write, first B row of each half of the B tile (K-major B:
+// each half is two 64-row boxes), first C column (MN-major B: also the first B column).
+struct Tile {
+    int row0, rows, b0, b1, col0;
+};
+
+template <int EPI, int MODE>
+struct Sched {
+    static constexpr int TN = (EPI == EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
+    int num_m, num_n, num_tiles, group_m, n_rot, M, N;
+    const int* offsets;
+    const int* prefix;  // grouped: tile_prefix in shared memory
+    int e;              // grouped: current expert (tiles are visited in increasing order)
+
+    __device__ void init(const EpiParams& ep, const AgParams& ag, int M_, int N_, int K, const int* pre)
+    {
+        M = M_;
+        N = N_;
+        num_n = (N + TN - 1) / TN;
+        offsets = ep.offsets;
+        prefix = pre;
+        e = 0;
+        n_rot = 0;
+        if (MODE == MODE_GROUPED) {
+            num_m = 0;
+            num_tiles = pre[ep.E];
+            group_m = 1;
+        } else {
+            num_m = (M + BM - 1) / BM;
+            num_tiles = num_m * num_n;
+            group_m = (MODE == MODE_PLAIN && ep.group_m > 0) ? ep.group_m : num_m;
+        }
+        if (MODE == MODE_ALLGATHER) {
+            // n-blocks are visited starting at the locally owned rows
+            const int64_t own_lo = static_cast<int64_t>(ag.rank) * ag.shard_bytes - ag.b_offset_bytes;
+            int64_t row = own_lo > 0 ? (own_lo + static_cast<int64_t>(K) * 2 - 1) / (static_cast<int64_t>(K) * 2) : 0;
+            n_rot = static_cast<int>((row + BN - 1) / BN) % num_n;
+        }
+    }
+    __device__ Tile at(int tile, int inter)
+    {
+        Tile t;
+        int m_blk, n_blk;
+        if (MODE == MODE_GROUPED) {
+            while (tile >= prefix[e + 1]) ++e;
+            const int lo = offsets[e], cnt = offsets[e + 1] - lo;
+            const int nm = (cnt + BM - 1) / BM;
+            const int local = tile - prefix[e];
+            m_blk = local % nm;
+            n_blk = local / nm;
+            t.row0 = lo + m_blk * BM;
+            t.rows = cnt - m_blk * BM;
+            t.col0 = n_blk * TN;
+            t.b0 = e * N + t.col0;
+            t.b1 = t.b0 + BN / 2;
+            return t;
+        }
+        tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
+        if (MODE == MODE_ALLGATHER) n_blk = (n_blk + n_rot) % num_n;
+        t.row0 = m_blk * BM;
+        t.rows = M - t.row0;
+        t.col0 = n_blk * TN;
+        t.b0 = t.col0;
+        t.b1 = (EPI == EPI_SWIGLU) ? inter + t.col0 : t.col0 + BN / 2;
+        return t;
+    }
+};
+
+template <bool A_MN, bool B_MN, int EPI, int MODE>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
+            const EpiParams ep, const AgParams ag)
+{
+    extern __shared__ uint8_t smem_raw[];
+    // 1024-byte alignment required by SWIZZLE_128B
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t bar_base = sbase + SMEM_BAR;
+    auto full_bar = [&](int s) { return bar_base + 8 * s; };
+    auto empty_bar = [&](int s) { return bar_base + 8 * (STAGES + s); };
+    int* tile_prefix = reinterpret_cast<int*>(smem + SMEM_GRP);
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int mma_ctas = MODE == MODE_ALLGATHER ? static_cast<int>(gridDim.x) - ag.comm_ctas : static_cast<int>(gridDim.x);
+
+    if (MODE == MODE_ALLGATHER && static_cast<int>(blockIdx.x) >= mma_ctas) {
+        ag_gather_role(ag, static_cast<int>(blockIdx.x) - mma_ctas, ag.comm_ctas, smem);
+        return;
+    }
+
+    if (threadIdx.x == kConsumerThreads) {
+        prefetch_map(&map_a);
+        prefetch_map(&map_b);
+        for (int s = 0; s < STAGES; ++s) {
+            mbar_init(full_bar(s), 1);
+            mbar_init(empty_bar(s), kConsumerThreads / 32);  // one arrival per consumer warp
+        }
+        fence_barrier_init();
+        if (MODE == MODE_GROUPED) {
+            const int nn = (N + Sched<EPI, MODE>::TN - 1) / Sched<EPI, MODE>::TN;
+            int acc = 0;
+            tile_prefix[0] = 0;
+            for (int e = 0; e < ep.E; ++e) {
+                const int cnt = ep.offsets[e + 1] - ep.offsets[e];
+                acc += ((cnt + BM - 1) / BM) * nn;
+                tile_prefix[e + 1] = acc;
+            }
+        }
+    }
+    __syncthreads();
+
+    Sched<EPI, MODE> sch;
+    sch.init(ep, ag, M, N, K, tile_prefix);
+    const int num_k = (K + BK - 1) / BK;
+
+    if (threadIdx.x >= kConsumerThreads) {
+        // ===================== TMA producer warpgroup =====================
+        setmaxnreg_dec<kProducerRegs>();
+        if (threadIdx.x == kConsumerThreads) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int tile = blockIdx.x; tile < sch.num_tiles; tile += mma_ctas) {
+                const Tile t = sch.at(tile, ep.inter);
+                if (MODE == MODE_ALLGATHER) ag_wait_rows(ag, t.col0, (N - t.col0) < BN ? (N - t.col0) : BN, K);
+                for (int kb = 0; kb < num_k; ++kb) {
+                    mbar_wait(empty_bar(stage), phase ^ 1);
+                    const uint32_t sa = sbase + stage * STAGE_BYTES, sb = sa + 2 * BOX;  // B: 4 boxes of 64 rows
+                    const uint32_t fb = full_bar(stage);
+                    mbar_expect_tx(fb, STAGE_BYTES);
+                    if (A_MN) {
+                        tma_load_2d(sa, &map_a, fb, t.row0, kb * BK);
+                        tma_load_2d(sa + BOX, &map_a, fb, t.row0 + 64, kb * BK);
+                    } else {
+                        tma_load_2d(sa, &map_a, fb, kb * BK, t.row0);
+                        tma_load_2d(sa + BOX, &map_a, fb, kb * BK, t.row0 + 64);
+                    }
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) {
+                        if (B_MN) tma_load_2d(sb + i * BOX, &map_b, fb, t.col0 + 64 * i, kb * BK);
+                        else tma_load_2d(sb + i * BOX, &map_b, fb, kb * BK, (i < 2 ? t.b0 : t.b1) + 64 * (i & 1));
+                    }
+                    if (++stage == STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================== consumers: warpgroup `wg` owns rows [64 wg, 64 wg + 64) of the tile =====================
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = threadIdx.x >> 7;
+    const int r_in = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // first of this thread's two rows (+8)
+    const int c_in = 2 * (lane & 3);                             // first of this thread's column pairs (+8 j)
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[128];
+    for (int tile = blockIdx.x; tile < sch.num_tiles; tile += mma_ctas) {
+        const Tile t = sch.at(tile, ep.inter);
+        int prev = -1;
+        for (int kb = 0; kb < num_k; ++kb) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t sa = sbase + stage * STAGE_BYTES + wg * BOX, sb = sbase + stage * STAGE_BYTES + 2 * BOX;
+            const uint64_t da = A_MN ? desc_mnmajor_sw128(sa, BOX) : desc_kmajor_sw128(sa);
+            const uint64_t db = B_MN ? desc_mnmajor_sw128(sb, BOX) : desc_kmajor_sw128(sb);
+            // per 16-element K step: K-major advances 32 B inside the swizzle row, MN-major 16 k-rows = 2 KiB
+            constexpr uint64_t ka = A_MN ? (2048 >> 4) : (32 >> 4);
+            constexpr uint64_t kbs = B_MN ? (2048 >> 4) : (32 >> 4);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k)
+                wgmma_m64n256k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da + ka * k, db + kbs * k, (kb > 0 || k > 0) ? 1 : 0);
+            wgmma_commit();
+            wgmma_wait<1>();  // the previous stage's products have retired: hand its buffers back
+            if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+            prev = stage;
+            if (++stage == STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+        wgmma_wait<0>();
+        fence_regs<128>(acc);
+        if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+
+        // ---- epilogue straight from the accumulators: thread holds rows r_in (+8), column pairs c_in + 8 j ----
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int lr = r_in + 8 * i;
+            if (lr >= t.rows || lr >= BM) continue;
+            const int64_t grow = static_cast<int64_t>(t.row0 + lr);
+            if constexpr (EPI == EPI_SWIGLU) {
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = t.col0 + 8 * j + c_in;
+                    if (col >= N) continue;
+                    const float g0 = acc[4 * j + 2 * i], g1 = acc[4 * j + 2 * i + 1];
+                    const float u0 = acc[4 * (j + 16) + 2 * i], u1 = acc[4 * (j + 16) + 2 * i + 1];
+                    st_bf16x2(ep.c + grow * ep.ldc + col, silu_f(g0) * u0, silu_f(g1) * u1);
+                    if (ep.out2 != nullptr) {
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + col, g0, g1);
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + ep.inter + col, u0, u1);
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const int col = t.col0 + 8 * j + c_in;
+                    if (col >= N) continue;
+                    float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+                    __nv_bfloat16* dst = ep.c + grow * ep.ldc + col;
+                    if constexpr (EPI == EPI_ACCUM) {
+                        const float2 o = ld_bf16x2(dst);
+                        v0 += o.x;
+                        v1 += o.y;
+                    }
+                    if constexpr (EPI == EPI_DSWIGLU) {
+                        const float2 g = ld_bf16x2(ep.aux + grow * ep.ld_aux + col);
+                        const float2 u = ld_bf16x2(ep.aux + grow * ep.ld_aux + ep.inter + col);
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + ep.inter + col, v0 * silu_f(g.x), v1 * silu_f(g.y));
+                        v0 = v0 * u.x * dsilu_f(g.x);
+                        v1 = v1 * u.y * dsilu_f(g.y);
+                    }
+                    st_bf16x2(dst, v0, v1);
+                }
+            }
+        }
+    }
+}
+
+}  // namespace gemm
+}  // namespace dsb
+
+using namespace dsb::gemm;
+
+static int g_sm_count = 0;
+
+static int sm_count()
+{
+    if (!g_sm_count) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
+    }
+    return g_sm_count;
+}
+
+template <bool A_MN, bool B_MN, int EPI, int MODE>
+static int launch_kernel(const CUtensorMap& ma, const CUtensorMap& mb, int M, int N, int K, int grid, const EpiParams& ep,
+                         const AgParams& ag, cudaStream_t stream)
+{
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(gemm_kernel<A_MN, B_MN, EPI, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             SMEM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    gemm_kernel<A_MN, B_MN, EPI, MODE><<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, ag);
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+template <int EPI>
+static int dispatch_major(int a_mn, int b_mn, const CUtensorMap& ma, const CUtensorMap& mb, int M, int N, int K, int grid,
+                          const EpiParams& ep, const AgParams& ag, cudaStream_t stream)
+{
+    if (a_mn && b_mn) return launch_kernel<true, true, EPI, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+    if (a_mn) return launch_kernel<true, false, EPI, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+    if (b_mn) return launch_kernel<false, true, EPI, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+    return launch_kernel<false, false, EPI, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+}
+
+// General GEMM with selectable operand majorness and fused epilogue:  C[M,N] = epi(op(A) x op(B)), bf16 in/out, fp32
+// accumulate.  (The `_2cta` names are kept for API stability; on sm_90a one CTA computes one 128 x 256 tile.)
+//   a_mn == 0: A is stored [M, K] row-major (K-major)      a_mn == 1: A is stored [K, M] row-major (MN-major)
+//   b_mn == 0: B is stored [N, K] row-major (K-major)      b_mn == 1: B is stored [K, N] row-major (MN-major)
+// so (0,0) = "NT" (y = x W^T), (0,1) = "NN" (dx = dy W), (1,1) = "TN" (dW = dy^T x).  lda/ldb are row strides in elements.
+//   epi: 0 store, 1 accumulate into C, 2 SwiGLU (B = [gate; up] stacked [2*inter, K], N = inter, C = [M, inter], out2 =
+//   optional gate|up save [M, 2*inter]), 3 dSwiGLU (N = inter, aux = saved gate|up, C = out2 = dgate|dup [M, 2*inter]).
+//   group_m: m-blocks (of 128 rows) per rasterisation super-group, <= 0 = column-major tile order.
+DSB_EXPORT int dsb_gemm_bf16_2cta_ex(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc,
+                                     int a_mn, int b_mn, int epi, const void* aux, int ld_aux, void* out2, int ld_out2,
+                                     int inter, int group_m, int sms, cudaStream_t stream)
+{
+    if (M <= 0 || N <= 0 || K <= 0) return -2;
+    if (lda % 8 || ldb % 8 || ldc % 8) return -2;
+    if ((a_mn ? M : K) % 8 || (b_mn ? N : K) % 8 || N % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) return -2;
+    if (epi < 0 || epi > 3) return -2;
+    if (epi == EPI_SWIGLU && (a_mn || b_mn || inter != N || inter % (BN / 2) || (out2 && (ld_out2 % 8)))) return -2;
+    if (epi == EPI_DSWIGLU && (a_mn || !aux || !out2 || inter != N || ld_aux % 8 || ld_out2 % 8)) return -2;
+    if ((reinterpret_cast<uintptr_t>(aux) | reinterpret_cast<uintptr_t>(out2)) & 15) return -2;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = a_mn ? make_map(&ma, a, K, M, lda, 64) : make_map(&ma, a, M, K, lda, 64))) return rc;
+    const uint64_t b_rows = (epi == EPI_SWIGLU) ? static_cast<uint64_t>(2) * inter : static_cast<uint64_t>(N);
+    if ((rc = b_mn ? make_map(&mb, b, K, N, ldb, 64) : make_map(&mb, b, b_rows, K, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.aux = static_cast<const __nv_bfloat16*>(aux);
+    ep.out2 = static_cast<__nv_bfloat16*>(out2);
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ld_aux = ld_aux;
+    ep.ld_out2 = ld_out2;
+    ep.ldc = ldc;
+    ep.inter = inter;
+    ep.group_m = group_m;
+    AgParams ag;
+    memset(&ag, 0, sizeof(ag));
+    int grid = sms > 0 ? sms : sm_count();
+    const int tn = (epi == EPI_SWIGLU) ? BN / 2 : BN;
+    const int tiles = ((M + BM - 1) / BM) * ((N + tn - 1) / tn);
+    if (grid > tiles) grid = tiles;
+    switch (epi) {
+        case EPI_STORE: return dispatch_major<EPI_STORE>(a_mn, b_mn, ma, mb, M, N, K, grid, ep, ag, stream);
+        case EPI_ACCUM: return dispatch_major<EPI_ACCUM>(a_mn, b_mn, ma, mb, M, N, K, grid, ep, ag, stream);
+        case EPI_SWIGLU: return launch_kernel<false, false, EPI_SWIGLU, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+        default:
+            return b_mn ? launch_kernel<false, true, EPI_DSWIGLU, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream)
+                        : launch_kernel<false, false, EPI_DSWIGLU, MODE_PLAIN>(ma, mb, M, N, K, grid, ep, ag, stream);
+    }
+}
+
+DSB_EXPORT int dsb_gemm_bf16_2cta(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc,
+                                  int a_mn, int b_mn, int sms, cudaStream_t stream)
+{
+    return dsb_gemm_bf16_2cta_ex(a, b, c, M, N, K, lda, ldb, ldc, a_mn, b_mn, EPI_STORE, nullptr, 0, nullptr, 0, 0, 8, sms,
+                                 stream);
+}
+
+DSB_EXPORT int dsb_gemm_nt_bf16_2cta(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc,
+                                     int sms, cudaStream_t stream)
+{
+    return dsb_gemm_bf16_2cta(a, b, c, M, N, K, lda, ldb, ldc, 0, 0, sms, stream);
+}
+
+// C[M,N] = A[M,K] @ B[N,K]^T   (bf16 in/out, fp32 accumulate).  sms <= 0 -> all SMs.
+DSB_EXPORT int dsb_gemm_nt_bf16(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc,
+                                int sms, cudaStream_t stream)
+{
+    return dsb_gemm_bf16_2cta_ex(a, b, c, M, N, K, lda, ldb, ldc, 0, 0, EPI_STORE, nullptr, 0, nullptr, 0, 0, 0, sms, stream);
+}
+
+// Fused all-gather + GEMM.  `b` points at B inside `local_full` (the unit's gathered buffer); the kernel
+// fills local_full from peers[] (each `shard_bytes` long) while multiplying.  `flags` holds n_chunks words.
+DSB_EXPORT int dsb_gemm_nt_bf16_allgather(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb,
+                                          int ldc, void* const* peers, void* local_full, uint32_t* flags,
+                                          int64_t shard_bytes, int64_t chunk_bytes, int64_t b_offset_bytes, int world,
+                                          int rank, int comm_ctas, uint32_t epoch, int sms, cudaStream_t stream)
+{
+    if (world > 8 || chunk_bytes <= 0 || shard_bytes % chunk_bytes || chunk_bytes % 16) return -2;
+    if (M <= 0 || N <= 0 || K <= 0 || K % 8 || N % 8 || lda % 8 || ldb % 8 || ldc % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) return -2;
+    AgParams ag;
+    memset(&ag, 0, sizeof(ag));
+    for (int i = 0; i < world; ++i) ag.peers[i] = peers[i];
+    ag.local_full = local_full;
+    ag.flags = flags;
+    ag.shard_bytes = shard_bytes;
+    ag.chunk_bytes = chunk_bytes;
+    ag.b_offset_bytes = b_offset_bytes;
+    ag.b_bytes = static_cast<int64_t>(N) * ldb * 2;
+    ag.n_chunks = static_cast<int>(shard_bytes / chunk_bytes) * world;
+    ag.world = world;
+    ag.rank = rank;
+    ag.comm_ctas = comm_ctas;
+    ag.epoch = epoch;
+    ag.enabled = 1;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map(&ma, a, M, K, lda, 64))) return rc;
+    if ((rc = make_map(&mb, b, N, K, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ldc = ldc;
+    // every CTA (math and gather) must be resident at once: the math CTAs spin on flags the gather CTAs publish
+    int grid = sms > 0 ? sms : sm_count();
+    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    int mma = grid - comm_ctas;
+    if (mma < 1) return -2;
+    if (mma > tiles) mma = tiles;
+    return launch_kernel<false, false, EPI_STORE, MODE_ALLGATHER>(ma, mb, M, N, K, mma + comm_ctas, ep, ag, stream);
+}
+
+// Grouped GEMM for expert-sorted rows: c[r, :] = a[r, :] @ w[e]^T for offsets[e] <= r < offsets[e+1].
+// a [rows, K] (lda), w [E, N, K] contiguous, c [rows, N] (ldc), offsets int32 [E+1] ON THE DEVICE.
+DSB_EXPORT int dsb_gemm_grouped_nt_bf16(const void* a, const void* w, void* c, const int* offsets, int rows, int E, int N, int K,
+                                        int lda, int ldc, int sms, cudaStream_t stream)
+{
+    if (rows <= 0 || E <= 0) return 0;
+    if (E > kMaxGroups || K % 8 || N % 8 || lda % 8 || ldc % 8) return -3;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(c)) & 15) return -3;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map(&ma, a, rows, K, lda, 64))) return rc;
+    if ((rc = make_map(&mb, w, static_cast<uint64_t>(E) * N, K, K, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ldc = ldc;
+    ep.offsets = offsets;
+    ep.E = E;
+    AgParams ag;
+    memset(&ag, 0, sizeof(ag));
+    int grid = sms > 0 ? sms : sm_count();
+    // upper bound of the tile count (each expert adds at most one partial m-tile) so tiny problems do not launch idle CTAs
+    const int64_t max_tiles = (static_cast<int64_t>(rows + BM - 1) / BM + E) * ((N + BN - 1) / BN);
+    if (grid > max_tiles) grid = static_cast<int>(max_tiles);
+    return launch_kernel<false, false, EPI_STORE, MODE_GROUPED>(ma, mb, rows, N, K, grid, ep, ag, stream);
+}
+
+DSB_EXPORT int dsb_gemm_tile_m() { return BM; }
+DSB_EXPORT int dsb_gemm_tile_n() { return BN; }
+DSB_EXPORT int dsb_gemm_tile_k() { return BK; }

@@ -1,4 +1,4 @@
-// Remaining device ops of the reference kernel inventory, re-implemented for sm_100a:
+// Remaining device ops of the reference kernel inventory, re-implemented for sm_90a:
 //   * dropout forward / backward with a counter-based RNG (+bias, +residual fusions)        [N7 dropout_kernels.cu]
 //   * masked attention softmax forward / backward over [b, h, sq, sk] (causal / additive mask / alibi /
 //     local window)                                                       [N7 softmax_kernels.cu, N8 softmax.cu]

@@ -1,4 +1,4 @@
-// MoE routing + ragged-batch (continuous batching) device ops for sm_100a.
+// MoE routing + ragged-batch (continuous batching) device ops for sm_90a.
 //   * top_k_gating         : softmax over experts, top-k selection, optional renormalisation, expert histogram
 //   * moe_assign_positions : deterministic slot of every (token, k) assignment inside its expert's segment
 //   * moe_scatter          : token rows -> expert-major buffer (the producer side of the EP all-to-all)

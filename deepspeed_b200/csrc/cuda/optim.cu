@@ -1,8 +1,8 @@
-// Fused optimizer kernels for sm_100a: Adam/AdamW, Lion, LAMB, Adagrad, SGD(momentum), plus the
+// Fused optimizer kernels for sm_90a: Adam/AdamW, Lion, LAMB, Adagrad, SGD(momentum), plus the
 // gradient utilities that surround them in a ZeRO step (sum-of-squares + inf/nan scan, scale).
 //
 // Role parity: reference csrc/adam/multi_tensor_adam.cu (N1), csrc/lion/multi_tensor_lion.cu and
-// csrc/lamb/fused_lamb_cuda_kernel.cu (N4).  Design differences (B200-first):
+// csrc/lamb/fused_lamb_cuda_kernel.cu (N4).  Design differences (H100-first):
 //   * ZeRO keeps each rank's shard as ONE flat buffer, so the primary entry points are flat
 //     kernels moving 8 elements / thread / iteration with 16-byte streaming accesses; the
 //     multi-tensor variant walks a device-resident chunk table (no 4 KB kernel-arg struct, no

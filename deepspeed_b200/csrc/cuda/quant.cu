@@ -1,4 +1,4 @@
-// Quantization kernels for sm_100a.
+// Quantization kernels for sm_90a.
 //   * group-wise INT8 / INT4 symmetric + asymmetric quantize / dequantize (ZeRO++ qwZ weights)
 //   * swizzled quantize: quantize AND lay partitions out in (device, node) order for the 2-hop all-to-all (qgZ)
 //   * fused dequantize -> reduce -> requantize across the chunks received from N peers (qgZ middle step),

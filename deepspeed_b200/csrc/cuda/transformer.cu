@@ -1,4 +1,4 @@
-// Transformer elementwise / normalisation kernels for sm_100a (training + inference):
+// Transformer elementwise / normalisation kernels for sm_90a (training + inference):
 //   RMSNorm / LayerNorm forward+backward (optional fused residual add), rotary embedding
 //   forward+backward, gated activations (SwiGLU / GEGLU / ReGLU) forward+backward, bias+activation,
 //   fused softmax-cross-entropy forward+backward (in-place gradient), bias/residual adds.
@@ -766,7 +766,7 @@ DSB_EXPORT int dsb_norm_bwd_grid(int rows)
 {
     // HBM-bound persistent kernel: exactly one wave of resident CTAs (4 per SM at 128 threads x ~120 registers); more
     // CTAs only add a second, half-empty wave and more dw partial rows for the column-sum pass.
-    const int cap = kSmCountB200 * 4;
+    const int cap = kSmCountH100 * 4;
     return rows < cap ? rows : cap;
 }
 
@@ -790,7 +790,7 @@ DSB_EXPORT int dsb_norm_bwd(const void* dy, const void* x, const void* w, const 
         const int vpt = hidden / 1024;
         const size_t smem = static_cast<size_t>(nb::kStages) * 3 * hidden * 2 + hidden * 2 + 64 + 16 * nb::kStages + 64;
         const int per_sm = smem <= 110 * 1024 ? 2 : 1;
-        const int g2 = rows < kSmCountB200 * per_sm ? rows : kSmCountB200 * per_sm;
+        const int g2 = rows < kSmCountH100 * per_sm ? rows : kSmCountH100 * per_sm;
         grid = g2;
         cudaError_t e = cudaSuccess;
 #define DSB_LAUNCH_NB(V)                                                                                                    \

@@ -14,7 +14,7 @@
 // a 16-bit 128.0 / 1024.0 pair and one packed subtract, with the activation pairs permuted to match), each chunk accumulates
 // into its own fp32 tile and the group scale is applied to that tile in fp32 -- scaling before the rounding to bf16 would
 // cost an instruction per weight and lose bits.  Partial sums of the 8 warps are reduced through shared memory.
-// (mma.sync on purpose: at M <= 64 a tcgen05 tile would be >75% padding and the kernel is bound by the weight stream.)
+// (mma.sync on purpose: at M <= 64 a wgmma tile would be >75% padding and the kernel is bound by the weight stream.)
 #include <cuda_fp8.h>
 #include <type_traits>
 #include "dsb_common.cuh"
@@ -316,7 +316,7 @@ void launch(const void* x, const void* wq, const float* scales, const void* bias
                                                                          (const T*)bias, (T*)out, M, N, K, gs, S);      \
     } while (0)
     // wide CTAs (32 features) once there are enough of them to fill the machine twice over; otherwise 16 features per CTA
-    const bool wide = N / 32 >= 2 * kSmCountB200;
+    const bool wide = N / 32 >= 2 * kSmCountH100;
     if (M <= 16) {
         if (wide) WQ_GO(4, 1); else WQ_GO(2, 1);
     } else {

@@ -1,22 +1,20 @@
-// Weight-only-quantised linear on the 5th-gen tensor cores for 32 < M <= a few hundred rows (batched decode, chunked
+// Weight-only-quantised linear on the Hopper tensor cores for 32 < M <= a few hundred rows (batched decode, chunked
 // prefill, MoE expert slices):   out[M, N] = x[M, K] @ dequant(Wq)[N, K]^T   with Wq in FP6 (E3M2) / FP8 (E4M3) / INT8 /
 // INT4, one fp32 scale per group of `group_size` consecutive K elements.
 //
-// The packed weights are the only large operand, so they go where tcgen05 wants the 128-row operand ("swap AB"):
-//   D^T[128 features, M tokens] = Wdq[128 features, K] * x[M tokens, K]^T
-//   * warps 2-9 (256 threads, two per FEATURE row, 32 K-elements each per step) stream their row's packed bytes straight from
-//     global memory one pipeline step AHEAD into registers (the load latency of step k+1 hides behind the decode of step k),
-//     decode to bf16 with the group scale folded in, and write the 128-byte-swizzled K-major A tile in shared memory -- the
-//     dequantised weight never exists in HBM (the reference's FP6-LLM kernel dequantises in
-//     registers for mma.sync, inference/v2/kernels/core_ops/cuda_linear/include/kernel_matmul.cuh:22; cutlass mixed_gemm
-//     does the same for int8/int4)
-//   * warp 0 TMA-loads the activation tile x[M_tile, 64] (B operand, N = M_tile <= 256: up to 256 rows reuse one pass over
-//     the weights), warp 1's elected thread issues tcgen05.mma (M = 128, N = M_tile, K = 16) into TMEM; 4-stage mbarrier ring
-//   * epilogue: the feature-row threads read their accumulator row, add the bias and store the transposed tile (lanes of a
-//     warp write 32 consecutive features of one token: 64-byte segments).
+// The packed weights are the only large operand, so they go where wgmma wants the 64-row operand ("swap AB"):
+//   D^T[128 features, 128 tokens] = Wdq[128 features, K] * x[128 tokens, K]^T
+//   * the two consumer warpgroups (64 feature rows each, two threads per row, 32 K-elements each per step) stream their
+//     rows' packed bytes straight from global memory one pipeline step AHEAD into registers (the load latency of step
+//     k+1 hides behind the decode of step k), decode to bf16 with the group scale folded in, and write the
+//     128-byte-swizzled K-major A tile in shared memory -- the dequantised weight never exists in HBM (the reference's
+//     FP6-LLM kernel dequantises in registers for mma.sync, inference/v2/kernels/core_ops/cuda_linear/include/
+//     kernel_matmul.cuh:22; cutlass mixed_gemm does the same for int8/int4)
+//   * a producer warp TMA-loads the activation tile x[128 tokens, 64] (B operand: up to 128 rows reuse one pass over the
+//     weights); each warpgroup issues wgmma.m64n128k16 on its own 64 rows; 4-stage ring, accumulators in registers
+//   * epilogue: add the bias and store the transposed tile.
 // For M <= 32 the mma.sync kernel of wq_gemm.cu (no padding waste) stays faster; for very large M dequantise-once + the
 // bf16 GEMM amortises better -- the Python layer picks (inference/quantization/layers.py).
-#include <cuda.h>
 #include <cuda_fp8.h>
 #include "dsb_tc.cuh"
 
@@ -24,12 +22,12 @@ namespace dsb {
 namespace wqtc {
 using namespace dsb::tc;
 
-constexpr int BF = 128;   // features per CTA (MMA M)
+constexpr int BF = 128;   // features per CTA (two warpgroups x 64)
 constexpr int BK = 64;    // K elements per pipeline step (one 128-byte swizzle row of bf16)
-constexpr int BT = 256;   // max tokens per CTA (MMA N)
+constexpr int BT = 128;   // tokens per CTA (MMA N)
 constexpr int kStages = 4;
-constexpr int kProducerWarps = 8;
-constexpr int kThreads = 64 + kProducerWarps * 32;
+constexpr int kConsumerThreads = 256;
+constexpr int kThreads = kConsumerThreads + 32;
 constexpr uint32_t A_BYTES = BF * BK * 2;  // 16 KiB
 constexpr uint32_t B_BYTES = BT * BK * 2;  // 16 KiB
 constexpr uint32_t SM_A = 0, SM_B = kStages * A_BYTES, SM_BAR = SM_B + kStages * B_BYTES;
@@ -118,13 +116,9 @@ wq_tc_kernel(const __grid_constant__ CUtensorMap map_x, const Params p)
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const uint32_t sbase = smem_u32(smem);
     const uint32_t bar = sbase + SM_BAR;
-    auto a_full = [&](int s) { return bar + 8 * s; };
-    auto b_full = [&](int s) { return bar + 8 * (kStages + s); };
-    auto empty = [&](int s) { return bar + 8 * (2 * kStages + s); };
-    const uint32_t acc_done = bar + 8 * (3 * kStages);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 8 * (3 * kStages + 1));
+    auto b_full = [&](int s) { return bar + 8 * s; };
+    auto b_empty = [&](int s) { return bar + 8 * (kStages + s); };
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int f0 = blockIdx.x * BF;  // first feature of this CTA
     int t0 = blockIdx.y * BT;        // first token
     int t_end = p.M;
@@ -134,131 +128,100 @@ wq_tc_kernel(const __grid_constant__ CUtensorMap map_x, const Params p)
         t_end = p.offsets[expert + 1];
     }
     if (t0 >= t_end) return;  // this expert has fewer token tiles (uniform for the CTA: nothing was initialised yet)
-    const int mt = min(BT, ((t_end - t0) + 15) & ~15);  // MMA N: tokens of this tile rounded up to 16
     const int num_k = p.K / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == kConsumerThreads) {
         prefetch_map(&map_x);
         for (int s = 0; s < kStages; ++s) {
-            mbar_init(a_full(s), kProducerWarps);
             mbar_init(b_full(s), 1);
-            mbar_init(empty(s), 1);
+            mbar_init(b_empty(s), kConsumerThreads / 32);
         }
-        mbar_init(acc_done, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), BT);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    if (warp == 0) {
-        if (elect_one()) {
+    if (threadIdx.x >= kConsumerThreads) {
+        if (threadIdx.x == kConsumerThreads) {
             for (int kb = 0; kb < num_k; ++kb) {
                 const int st = kb % kStages;
-                mbar_wait(empty(st), ((kb / kStages) & 1) ^ 1);
+                mbar_wait(b_empty(st), ((kb / kStages) & 1) ^ 1);
                 mbar_expect_tx(b_full(st), B_BYTES);
                 tma_load_2d(sbase + SM_B + st * B_BYTES, &map_x, b_full(st), kb * BK, t0);
             }
         }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            const uint32_t idesc = idesc_bf16(BF, mt, false, false);
-            for (int kb = 0; kb < num_k; ++kb) {
-                const int st = kb % kStages;
-                const uint32_t par = (kb / kStages) & 1;
-                mbar_wait(a_full(st), par);
-                mbar_wait(b_full(st), par);
-                tc_fence_after();
-                const uint32_t sa = sbase + SM_A + st * A_BYTES, sb = sbase + SM_B + st * B_BYTES;
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k)
-                    umma_bf16(tmem, desc_kmajor_sw128(sa + k * 32), desc_kmajor_sw128(sb + k * 32), idesc,
-                              (kb > 0 || k > 0) ? 1u : 0u);
-                umma_commit(empty(st));
-            }
-            umma_commit(acc_done);
-        }
-    } else {
-        // ---- dequantising producers: two threads per feature row, each owns 32 of the 64 K elements of a step ------------------
-        const int q4 = warp & 3;             // TMEM lane quadrant this warp may read in the epilogue
-        const int hk = (warp - 2) >> 2;      // which half of the K step (and of the token columns in the epilogue)
-        const int r = q4 * 32 + lane;
-        const int feat = f0 + r;
-        const bool feat_ok = feat < p.N;
-        constexpr int B8 = bytes_per_8<MODE>();
-        constexpr int NR = 4 * B8 / 8;       // 8-byte words of packed weights per thread and step
-        const int64_t row_bytes = static_cast<int64_t>(p.K) / 8 * B8;
-        const int64_t slab = static_cast<int64_t>(expert) * p.N;  // rows of the stacked [E, N, K] weight before this expert
-        const uint8_t* wrow = p.wq + (slab + (feat_ok ? feat : 0)) * row_bytes + hk * 4 * B8;
-        const float* srow = p.scales + (slab + (feat_ok ? feat : 0)) * (p.K / p.group_size);
-        uint2 cur[NR], nxt[NR];
-        float sc_cur, sc_nxt = 0.f;
-        auto fetch = [&](int kb, uint2* dst, float& sc) {
-            const uint2* g = reinterpret_cast<const uint2*>(wrow + static_cast<int64_t>(kb) * (BK / 8) * B8);
-#pragma unroll
-            for (int i = 0; i < NR; ++i) dst[i] = feat_ok ? __ldg(g + i) : make_uint2(0u, 0u);
-            sc = feat_ok ? __ldg(srow + (kb * BK) / p.group_size) : 0.f;
-        };
-        fetch(0, cur, sc_cur);
-        for (int kb = 0; kb < num_k; ++kb) {
-            const int st = kb % kStages;
-            if (kb + 1 < num_k) fetch(kb + 1, nxt, sc_nxt);  // in flight while this step is decoded
-            mbar_wait(empty(st), ((kb / kStages) & 1) ^ 1);
-            uint8_t* arow = smem + SM_A + st * A_BYTES + r * 128;
-            const uint8_t* raw = reinterpret_cast<const uint8_t*>(cur);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                float f[8];
-                decode8<MODE>(raw + j * B8, sc_cur, f);
-                const int c = hk * 4 + j;
-                *reinterpret_cast<Vec16*>(arow + ((c ^ (r & 7)) << 4)) = Elem<__nv_bfloat16>::pack(f);
-            }
-            fence_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(a_full(st));
-#pragma unroll
-            for (int i = 0; i < NR; ++i) cur[i] = nxt[i];
-            sc_cur = sc_nxt;
-        }
-        // ---- epilogue: transposed store of D^T[feature r, tokens] --------------------------------------------------------------
-        mbar_wait(acc_done, 0);
-        tc_fence_after();
-        const float bias = (p.bias != nullptr && feat_ok) ? __bfloat162float(p.bias[slab + feat]) : 0.f;
-        const uint32_t lane_addr = static_cast<uint32_t>(q4 * 32) << 16;
-        for (int c = hk * 32; c < mt; c += 64) {  // the two threads of a feature row alternate 32-token column blocks
-            uint32_t v[32];
-            tmem_ld_32x32(tmem + lane_addr + c, v);
-            tmem_ld_wait();
-            if (feat_ok) {
-#pragma unroll
-                for (int e = 0; e < 32; ++e) {
-                    const int tok = t0 + c + e;
-                    if (tok < t_end) p.out[static_cast<int64_t>(tok) * p.ldo + feat] = __float2bfloat16_rn(__uint_as_float(v[e]) + bias);
-                }
-            }
-        }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem, BT);
-}
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_fn()
-{
-    static EncodeTiledFn fn = nullptr;
-    if (fn) return fn;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &st) != cudaSuccess ||
-        st != cudaDriverEntryPointSuccess)
-        return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    return fn;
+    // ---- consumers: dequantise this warpgroup's 64 feature rows, multiply, store ------------------------------------------
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = warp >> 2;
+    const int tw = threadIdx.x & 127;
+    const int r = wg * 64 + (tw & 63);   // feature row inside the CTA tile
+    const int hk = tw >> 6;              // which half of the K step this thread decodes
+    const int feat = f0 + r;
+    const bool feat_ok = feat < p.N;
+    constexpr int B8 = bytes_per_8<MODE>();
+    constexpr int NR = 4 * B8 / 8;       // 8-byte words of packed weights per thread and step
+    const int64_t row_bytes = static_cast<int64_t>(p.K) / 8 * B8;
+    const int64_t slab = static_cast<int64_t>(expert) * p.N;  // rows of the stacked [E, N, K] weight before this expert
+    const uint8_t* wrow = p.wq + (slab + (feat_ok ? feat : 0)) * row_bytes + hk * 4 * B8;
+    const float* srow = p.scales + (slab + (feat_ok ? feat : 0)) * (p.K / p.group_size);
+    uint2 cur[NR], nxt[NR];
+    float sc_cur, sc_nxt = 0.f;
+    auto fetch = [&](int kb, uint2* dst, float& sc) {
+        const uint2* g = reinterpret_cast<const uint2*>(wrow + static_cast<int64_t>(kb) * (BK / 8) * B8);
+#pragma unroll
+        for (int i = 0; i < NR; ++i) dst[i] = feat_ok ? __ldg(g + i) : make_uint2(0u, 0u);
+        sc = feat_ok ? __ldg(srow + (kb * BK) / p.group_size) : 0.f;
+    };
+    float acc[64];
+    fetch(0, cur, sc_cur);
+    for (int kb = 0; kb < num_k; ++kb) {
+        const int st = kb % kStages;
+        if (kb + 1 < num_k) fetch(kb + 1, nxt, sc_nxt);  // in flight while this step is decoded
+        // the products that last read this A slot (step kb - kStages) retired: at most one group is left in flight
+        uint8_t* arow = smem + SM_A + st * A_BYTES + r * 128;
+        const uint8_t* raw = reinterpret_cast<const uint8_t*>(cur);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            float f[8];
+            decode8<MODE>(raw + j * B8, sc_cur, f);
+            const int c = hk * 4 + j;
+            *reinterpret_cast<Vec16*>(arow + ((c ^ (r & 7)) << 4)) = Elem<__nv_bfloat16>::pack(f);
+        }
+        fence_async_smem();
+        named_sync(1 + wg, 128);
+        mbar_wait(b_full(st), (kb / kStages) & 1);
+        const uint64_t da = desc_kmajor_sw128(sbase + SM_A + st * A_BYTES + wg * (A_BYTES / 2));
+        const uint64_t db = desc_kmajor_sw128(sbase + SM_B + st * B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) wgmma_m64n128k16_ss<0, 0>(acc, da + 2 * k, db + 2 * k, (kb > 0 || k > 0) ? 1 : 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) mbar_arrive(b_empty((kb - 1) % kStages));
+#pragma unroll
+        for (int i = 0; i < NR; ++i) cur[i] = nxt[i];
+        sc_cur = sc_nxt;
+    }
+    wgmma_wait<0>();
+    fence_regs<64>(acc);
+    // ---- epilogue: transposed store of D^T[feature, token] --------------------------------------------------------------
+    const int fr = f0 + wg * 64 + 16 * (warp & 3) + (lane >> 2);  // this thread's features: fr, fr + 8
+    const int c_in = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        const int f = fr + 8 * i;
+        if (f >= p.N) continue;
+        const float bias = p.bias != nullptr ? __bfloat162float(p.bias[slab + f]) : 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int tok = t0 + 8 * j + c_in + e;
+                if (tok < t_end) p.out[static_cast<int64_t>(tok) * p.ldo + f] = __float2bfloat16_rn(acc[4 * j + 2 * i + e] + bias);
+            }
+    }
 }
 
 template <int MODE>
@@ -292,7 +255,7 @@ DSB_EXPORT int dsb_wq_tc_gemm(const void* x, const void* wq, const float* scales
 }
 
 // Grouped (MoE) form: x / out rows sorted by expert, `offsets` int32 [E + 1] ON THE DEVICE, wq / scales / bias stacked [E, ...].
-// M = total rows (an upper bound for every expert's row count: the grid covers ceil(M / 256) token tiles per expert and CTAs
+// M = total rows (an upper bound for every expert's row count: the grid covers ceil(M / 128) token tiles per expert and CTAs
 // beyond an expert's range exit at once) -- no host synchronisation, CUDA-graph capturable.
 DSB_EXPORT int dsb_wq_tc_gemm_grouped(const void* x, const void* wq, const float* scales, const void* bias, void* out,
                                       const int* offsets, int E, int M, int N, int K, int mode, int group_size, int ldx,
@@ -308,16 +271,8 @@ static int wq_tc_impl(const void* x, const void* wq, const float* scales, const 
     if (M <= 0 || N <= 0) return 0;
     if (K % BK || group_size % BK || K % group_size || ldx % 8 || mode < 0 || mode > 3) return -3;
     if (reinterpret_cast<uintptr_t>(x) & 15) return -3;
-    EncodeTiledFn fn = encode_fn();
-    if (!fn) return -3;
     CUtensorMap mx;
-    cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(M)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(ldx) * 2};
-    cuuint32_t box[2] = {BK, BT};
-    cuuint32_t estr[2] = {1, 1};
-    if (fn(&mx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(x), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return -3;
+    if (make_map(&mx, x, M, K, ldx, BT)) return -3;
     Params p;
     p.wq = static_cast<const uint8_t*>(wq);
     p.scales = scales;

@@ -1,7 +1,7 @@
-// Shared device helpers for the deepspeed_b200 sm_100a kernels.
+// Shared device helpers for the deepspeed_b200 sm_90a kernels.
 //
 // Role parity: reference csrc/includes/{memory_access_utils.h, reduction_utils.h,
-// conversion_utils.h} (N20 in SURVEY.md).  Written from scratch for sm_100a: 16-byte vector
+// conversion_utils.h} (N20 in SURVEY.md).  Written from scratch for sm_90a: 16-byte vector
 // accesses with explicit cache policies, warp-shuffle + smem block reductions, and packed
 // bf16/fp16 <-> fp32 conversion helpers.
 #pragma once
@@ -21,7 +21,7 @@
 namespace dsb {
 
 constexpr int kWarp = 32;
-constexpr int kSmCountB200 = 148;
+constexpr int kSmCountH100 = 132;
 
 // dtype codes shared with Python (deepspeed_b200/ops/native.py)
 enum DType : int { kF32 = 0, kF16 = 1, kBF16 = 2, kI8 = 3, kU8 = 4, kF8E4M3 = 5, kF8E5M2 = 6 };
@@ -226,7 +226,7 @@ __host__ __device__ __forceinline__ int64_t ceil_div(int64_t a, int64_t b) { ret
 
 // Grid sizing for bandwidth-bound flat kernels: a multiple of the SM count, capped so each
 // block has enough work to amortise launch (grid-stride loops handle the rest).
-inline int flat_grid(int64_t n_vec, int threads, int blocks_per_sm = 8, int sm_count = kSmCountB200)
+inline int flat_grid(int64_t n_vec, int threads, int blocks_per_sm = 8, int sm_count = kSmCountH100)
 {
     int64_t need = ceil_div(n_vec, threads);
     int64_t cap = static_cast<int64_t>(sm_count) * blocks_per_sm;

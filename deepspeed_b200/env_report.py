@@ -14,8 +14,8 @@ YES, NO = f"{GREEN}[YES]{END}", f"{YELLOW}[NO]{END}"
 
 def op_report(verbose=True):
     from deepspeed_b200.op_builder import ALL_OPS
-    print("-" * 50 + "\nDeepSpeed-B200 native op report\n" + "-" * 50)
-    print("NOTE: native ops are built in-tree into deepspeed_b200/lib (sm_100a only); 'installed' means the shared\n"
+    print("-" * 50 + "\nDeepSpeed-H100 native op report\n" + "-" * 50)
+    print("NOTE: native ops are built in-tree into deepspeed_b200/lib (sm_90a only); 'installed' means the shared\n"
           "      object is present and up to date, 'compatible' means the toolchain can (re)build it here.\n" + "-" * 50)
     print(f"{'op name':<24}{'installed':<22}{'compatible'}\n" + "-" * 50)
     for name, builder in ALL_OPS.items():
@@ -89,7 +89,7 @@ def debug_report():
     shm, shm_warn = get_shm_size()
     rows.append(("shared memory (/dev/shm) size", shm))
     rows.append(("host memory", f"{psutil.virtual_memory().total / 2**30:.1f} GiB"))
-    print("DeepSpeed-B200 general environment info:")
+    print("DeepSpeed-H100 general environment info:")
     for k, v in rows:
         print(f"{k} {'.' * (40 - len(k))} {v}")
     for w in shm_warn:
@@ -119,7 +119,7 @@ if __name__ == "__main__":
 
 
 def installed_cann_path():
-    """Ascend toolkits are not a target of this build (single-vendor: NVIDIA sm_100a)."""
+    """Ascend toolkits are not a target of this build (single-vendor: NVIDIA sm_90a)."""
     return None
 
 

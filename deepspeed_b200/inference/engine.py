@@ -364,7 +364,7 @@ class InferenceEngine(nn.Module):
 def ragged_generate(ragged, input_ids, uid0, max_out_tokens, eos_default=None, **kwargs):
     """Greedy / sampling generation on a ragged engine; returns (tokens [B, S+new], next free uid)."""
     if kwargs.get("num_beams", 1) > 1:
-        raise NotImplementedError("DeepSpeed-B200 kernel-injected generate supports greedy / sampling only")
+        raise NotImplementedError("DeepSpeed-H100 kernel-injected generate supports greedy / sampling only")
     max_new = kwargs.get("max_new_tokens")
     if max_new is None:
         max_new = kwargs.get("max_length", input_ids.shape[1] + 20) - input_ids.shape[1]

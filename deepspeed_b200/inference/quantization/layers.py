@@ -64,15 +64,16 @@ def maybe_quantized_linear(x, w, b=None):
 
 
 _TC_MODES = {"int8": 0, "int4": 1, "fp8": 2, "fp6": 3}
-# Row count up to which the fused kernel beats dequantise-once + bf16 GEMM, per weight format, measured on B200 at
-# [rows x 14336 x 4096] (scripts/bench_wq_tc.py -> profiles/wq_tc_bench_r2.json): int8 1.9x at <= 256 rows, 1.15x at 512,
-# 0.78x at 1024; int4 2.5x / 1.6x / 1.05x; fp8 3.9x / 2.3x / 1.4x; fp6 3.7x / 2.1x / 1.26x.
-WQ_TC_MAX_ROWS_BY_MODE = {"int8": 512, "int4": 1024, "fp8": 1024, "fp6": 1024}
-WQ_TC_MAX_ROWS = 1024
+# Row count up to which the fused kernel beats dequantise-once + bf16 GEMM, per weight format, measured on an H100 80GB HBM3
+# at a 400 W power limit at [rows x 14336 x 4096] (scripts/bench_wq_tc.py), fused speedup at 128 / 256 / 512 / 1024 rows:
+# int8 2.22x / 1.28x / 0.81x / 0.63x; int4 2.47x / 1.57x / 1.03x / 0.80x; fp8 2.69x / 1.65x / 1.02x / 0.78x;
+# fp6 2.73x / 1.69x / 1.02x / 0.74x.  The kernel covers 128 tokens per CTA, so every further 128 rows re-read the weights.
+WQ_TC_MAX_ROWS_BY_MODE = {"int8": 256, "int4": 512, "fp8": 512, "fp6": 512}
+WQ_TC_MAX_ROWS = 512
 
 
 def wq_tc_linear(x, qw: "QuantizedWeight", b=None, max_rows=None):
-    """32 < rows <= ``WQ_TC_MAX_ROWS``: fused dequantise-in-shared-memory + tcgen05 GEMM (``csrc/cuda/wq_tc_gemm.cu``) for
+    """32 < rows <= ``WQ_TC_MAX_ROWS``: fused dequantise-in-shared-memory + wgmma GEMM (``csrc/cuda/wq_tc_gemm.cu``) for
     FP6 / FP8 / INT8 / INT4 weights -- the dequantised weight never exists in HBM.  None -> not eligible."""
     if not (x.is_cuda and x.dtype == torch.bfloat16 and qw.mode in _TC_MODES and qw.dtype == torch.bfloat16):
         return None

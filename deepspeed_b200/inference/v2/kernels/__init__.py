@@ -20,7 +20,7 @@ def mixed_gemm(x, qweight, bias=None):
 def moe_gemm(x_sorted, expert_weights, offsets, out=None):
     """Grouped GEMM over expert-sorted rows (reference cutlass ``moe_gemm``): ``x_sorted`` [rows, K] with expert e owning
     rows ``offsets[e]:offsets[e+1]``, ``expert_weights`` [E, N, K] (or a list).  On the device with bf16 stacked weights
-    this is ONE persistent tcgen05 launch driven by the device-resident offsets (``gemm_grouped_nt_kernel``); otherwise
+    this is ONE persistent wgmma launch driven by the device-resident offsets (``gemm_grouped_nt_kernel``); otherwise
     one GEMM per non-empty expert."""
     import torch
     from deepspeed_b200.ops.kernels import gemm_sm100

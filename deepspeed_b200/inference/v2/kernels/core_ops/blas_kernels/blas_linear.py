@@ -1,4 +1,4 @@
-"""``out = hidden @ W^T`` through the autotuned GEMM (cuBLAS or the tcgen05 kernels).
+"""``out = hidden @ W^T`` through the autotuned GEMM (cuBLAS or the wgmma kernels).
 
 Reference ``inference/v2/kernels/core_ops/blas_kernels/blas_linear.py``."""
 import torch

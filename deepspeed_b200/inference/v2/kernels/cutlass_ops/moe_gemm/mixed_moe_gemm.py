@@ -1,7 +1,7 @@
 """Grouped GEMM with weight-only-quantised expert weights.
 
 Reference ``inference/v2/kernels/cutlass_ops/moe_gemm/mixed_moe_gemm.py`` (cutlass ``moe_gemm`` with a dequantising
-prologue).  Here: ONE launch of the grouped form of the tcgen05 dequantise-in-shared-memory kernel
+prologue).  Here: ONE launch of the grouped form of the wgmma dequantise-in-shared-memory kernel
 (``csrc/cuda/wq_tc_gemm.cu``): blockIdx.z = expert, the expert extents are read from the device-resident cumulative row
 counts (no ``.tolist()`` host synchronisation, CUDA-graph capturable), the packed weights of all experts are stacked once."""
 import torch

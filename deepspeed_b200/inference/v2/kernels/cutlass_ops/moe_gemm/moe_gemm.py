@@ -22,7 +22,7 @@ class MoEGEMM(DSKernelBase):
         """``weights`` [E, out, in]; expert e owns rows ``cumsum_rows[e-1]:cumsum_rows[e]`` of the sorted input."""
         from ... import moe_gemm
         if torch.is_tensor(cumsum_rows) and cumsum_rows.is_cuda and biases is None and torch.is_tensor(weights):
-            # device-resident offsets -> single grouped tcgen05 launch, no host synchronisation
+            # device-resident offsets -> single grouped wgmma launch, no host synchronisation
             off = torch.cat([cumsum_rows.new_zeros(1), cumsum_rows]).to(torch.int32)
             moe_gemm(ordered_input, weights, off, out=ordered_output)
             if self.act_fn == ActivationFuncType.GELU:

@@ -25,7 +25,7 @@ class BlockedFlashAttn(DSKernelBase):
 
 
 def get_q_block_size(head_size: int) -> int:
-    """Query tile of the prefill attention kernel: 128 rows (one tcgen05 M=128 tile) for every head size it supports."""
+    """Query tile of the prefill attention kernel: 128 rows (one wgmma M=128 tile) for every head size it supports."""
     if head_size % 16 != 0 or head_size > 256:
         raise ValueError(f"unsupported head size {head_size}")
     return 128

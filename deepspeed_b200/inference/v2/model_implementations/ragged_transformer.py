@@ -152,7 +152,7 @@ class RaggedTransformer:
         for t0, n in dense:
             rows = qkv[t0:t0 + n]
             if os.environ.get("DSB200_PREFILL_ATTN", "native") == "native" and A.supports_fwd(rows, hq, hkv, d, 1, n):
-                # the in-tree tcgen05 attention forward, straight on the packed rows (K/V were just rotated in place by
+                # the in-tree wgmma attention forward, straight on the packed rows (K/V were just rotated in place by
                 # kv_rotary_append) and straight into the output rows: no head transposes, any prompt length
                 qv, kv_, vv = A.split_packed(rows, hq, hkv)
                 A.fwd(qv, kv_, vv, 1, n, hq, hkv, causal=True, out=out[t0:t0 + n], need_lse=False)
@@ -192,7 +192,7 @@ class RaggedTransformer:
         capturing = x.is_cuda and torch.cuda.is_current_stream_capturing()
         if (x.is_cuda and x.dtype == torch.bfloat16 and torch.is_tensor(lw.experts_up) and torch.is_tensor(lw.experts_down)
                 and lw.experts_up.dtype == torch.bfloat16 and os.environ.get("DSB200_MOE_GROUPED", "1") != "0"):
-            # device-driven grouped GEMM: one persistent tcgen05 launch per projection streams only the experts that
+            # device-driven grouped GEMM: one persistent wgmma launch per projection streams only the experts that
             # received tokens; offsets never leave the device, so prefill and (graph-captured) decode share this path
             from deepspeed_b200.inference.v2.kernels import moe_gemm
             positions, _, offsets = M.route(ids, sp.num_experts, counts=counts)

@@ -2,7 +2,7 @@
 
 One tensor per cache group, laid out ``[layers, blocks, block_size, 2, kv_heads, head_dim]`` so that a layer's
 slice is exactly what ``kv_rotary_append`` / ``paged_attention`` consume.  Sizing defaults to "everything HBM
-has left after weights minus a reserve" — on a 180 GB B200 that is usually >100 GB of KV.
+has left after weights minus a reserve" — on a 80 GB H100 that is usually >100 GB of KV.
 """
 from typing import Iterable, Optional, Tuple
 

@@ -16,7 +16,7 @@ PID_FILE_BASEPATH = "/tmp"
 
 
 def parse_args(argv=None):
-    p = argparse.ArgumentParser(description="DeepSpeed-B200 per-node process launcher")
+    p = argparse.ArgumentParser(description="DeepSpeed-H100 per-node process launcher")
     p.add_argument("--node_rank", type=int, default=0)
     p.add_argument("--master_addr", default="127.0.0.1", type=str)
     p.add_argument("--master_port", default=29500, type=int)

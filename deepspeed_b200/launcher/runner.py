@@ -23,7 +23,7 @@ from .multinode_runner import RUNNERS
 
 
 def parse_args(args=None):
-    p = argparse.ArgumentParser(description="DeepSpeed-B200 runner: launch single- or multi-node training jobs")
+    p = argparse.ArgumentParser(description="DeepSpeed-H100 runner: launch single- or multi-node training jobs")
     p.add_argument("-H", "--hostfile", type=str, default=K.DLTS_HOSTFILE,
                    help="Hostfile path (MPI style): lines of `hostname slots=N`")
     p.add_argument("-i", "--include", type=str, default="",

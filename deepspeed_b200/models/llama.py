@@ -2,7 +2,7 @@
 
 This is the flagship training model of the framework (``BASELINE.json``: Llama-3-8B ZeRO-3 bf16).
 The reference ships no training model; its users bring HF ``LlamaForCausalLM`` whose hot path on
-B200 is PyTorch ops.  B200-first choices here:
+H100 is PyTorch ops.  H100-first choices here:
 
 * packed ``qkv`` and ``gate_up`` projections -> 4 large GEMMs per layer instead of 7;
 * residual-add fused into RMSNorm (one pass over the residual stream per norm);
@@ -13,7 +13,7 @@ B200 is PyTorch ops.  B200-first choices here:
 * LM head + cross entropy chunked over tokens with the softmax gradient produced in place, so the
   ``[tokens, vocab]`` logits never exist (role of the reference ``FPDT_LogitsLoss``,
   ``sequence/fpdt_layer.py:1137``);
-* attention core through ``ops.attention`` (cuDNN/flash SDPA library path or the native sm_100a kernel).
+* attention core through ``ops.attention`` (cuDNN/flash SDPA library path or the native sm_90a kernel).
 """
 import math
 from dataclasses import dataclass, field
@@ -79,6 +79,10 @@ class LlamaConfig:
 
 
 PRESETS = {
+    # Llama-3.2-3B's shape with an untied LM head (3.6 B parameters): the largest Llama-3 shape whose full ZeRO training
+    # state fits one 80 GB card
+    "llama3.2-3b": dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_hidden_layers=28,
+                        num_attention_heads=24, num_key_value_heads=8, rope_theta=500000.0, max_position_embeddings=8192),
     "llama3-8b": dict(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                       num_attention_heads=32, num_key_value_heads=8, rope_theta=500000.0, max_position_embeddings=8192),
     "llama3-70b": dict(vocab_size=128256, hidden_size=8192, intermediate_size=28672, num_hidden_layers=80,

@@ -30,7 +30,7 @@ class Experts(nn.Module):
 
 
 class GroupedSwiGLUExperts(nn.Module):
-    """Stacked SwiGLU experts evaluated with batched GEMMs: ``w13`` [E, 2I, H], ``w2`` [E, H, I].  The B200
+    """Stacked SwiGLU experts evaluated with batched GEMMs: ``w13`` [E, 2I, H], ``w2`` [E, H, I].  The H100
     path for Mixtral-style layers (one strided-batched GEMM per projection instead of E small ones)."""
 
     def __init__(self, num_local_experts, hidden, intermediate, expert_group_name=None, act="silu"):
@@ -48,7 +48,7 @@ class GroupedSwiGLUExperts(nn.Module):
     def forward(self, inputs):
         """``inputs``: [E_local, tokens, hidden] (capacity-padded dispatch buffer) -> same shape."""
         if inputs.is_cuda and inputs.dtype == torch.bfloat16 and self.act == "silu" and inputs.shape[1] >= 256:
-            # tcgen05 path: per expert the fused gate|up GEMM (+) SwiGLU, down GEMM, and in backward the dSwiGLU-fused
+            # wgmma path: per expert the fused gate|up GEMM (+) SwiGLU, down GEMM, and in backward the dSwiGLU-fused
             # input-gradient GEMM plus weight-gradient GEMMs written straight into the stacked parameters' flat ZeRO
             # gradient views (one launch per expert and projection: every problem is [tokens x 14336 x 4096]-sized)
             from deepspeed_b200.ops.linear import grouped_swiglu_mlp

@@ -59,7 +59,7 @@ def _parse_size(s):
 
 
 def ds_io_main(argv=None):
-    p = argparse.ArgumentParser(description="DeepSpeed-B200 NVMe I/O benchmark")
+    p = argparse.ArgumentParser(description="DeepSpeed-H100 NVMe I/O benchmark")
     p.add_argument("--folder", "--nvme_dir", dest="folder", type=str, required=True)
     p.add_argument("--io_size", type=str, default="256M")
     p.add_argument("--read", action="store_true")

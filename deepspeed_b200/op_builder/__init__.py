@@ -2,7 +2,7 @@
 
 Two shared libraries hold every native component:
 
-* ``libdsb200_cuda.so`` -- all sm_100a kernels + the symmetric-memory (VMM/NVLS) runtime.
+* ``libdsb200_cuda.so`` -- all sm_90a kernels + the symmetric-memory (VMM/NVLS) runtime.
 * ``libdsb200_cpu.so``  -- host runtime: AVX-512/AVX2 optimizers, async file I/O engine,
   shared-memory collectives, ragged-batch host helpers.
 
@@ -25,9 +25,9 @@ class CudaKernelsBuilder(CUDAOpBuilder):
         "cuda/moe_ragged.cu",
         "cuda/misc.cu",
         "cuda/symm_coll.cu",
-        "cuda/gemm_sm100.cu",
+        "cuda/gemm_sm90.cu",
         "cuda/attention.cu",
-        "cuda/attn_sm100.cu",
+        "cuda/attn_sm90.cu",
         "cuda/attn_bias.cu",
         "cuda/moe_symm.cu",
         "cuda/wq_gemm.cu",
@@ -152,7 +152,7 @@ def build_all(verbose=True):
 
 
 def get_default_compute_capabilities():
-    return "10.0a"
+    return "9.0a"
 
 
 # ---- per-op module paths of the reference (``op_builder/fused_adam.py`` ...) ------------------------------------------------

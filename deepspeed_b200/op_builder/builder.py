@@ -3,8 +3,8 @@
 Parity target: reference ``op_builder/builder.py`` (``OpBuilder.load :523``, ``jit_load :542``,
 ``CUDAOpBuilder.compute_capability_args :610``).  Design differences:
 
-* One arch only: ``-gencode arch=compute_100a,code=sm_100a`` (the ``a`` suffix is required for
-  tcgen05 / TMEM / ``multimem``).  No arch sweep, no ``TORCH_CUDA_ARCH_LIST``.
+* One arch only: ``-gencode arch=compute_90a,code=sm_90a`` (the ``a`` suffix is required for
+  ``wgmma`` / ``setmaxnreg`` / ``multimem``).  No arch sweep, no ``TORCH_CUDA_ARCH_LIST``.
 * Kernels expose a C ABI and never include torch headers, so a full rebuild is seconds and the
   ``.so`` files live in ``deepspeed_b200/lib`` (in-tree: they travel with the repo snapshot and are
   visible in ``/proc/self/maps`` of every process that uses them).
@@ -26,7 +26,7 @@ CSRC = ROOT / "csrc"
 LIB_DIR = ROOT / "lib"
 OBJ_DIR = LIB_DIR / "obj"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
               "--expt-relaxed-constexpr", "-DNDEBUG"]
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-fopenmp", "-fvisibility=hidden", "-DNDEBUG", "-pthread"]
@@ -96,7 +96,7 @@ class CUDAMismatchException(Exception):
     pass
 
 
-DEFAULT_COMPUTE_CAPABILITIES = "10.0a"
+DEFAULT_COMPUTE_CAPABILITIES = "9.0a"
 
 
 def installed_cuda_version(name=""):
@@ -117,12 +117,12 @@ def get_default_compute_capabilities():
 
 
 def assert_no_cuda_mismatch(name=""):
-    """The toolkit must be able to target sm_100a (CUDA ≥ 12.8) and share torch's CUDA major version; minor-version skew
+    """The toolkit must be able to target sm_90a (CUDA ≥ 12.0) and share torch's CUDA major version; minor-version skew
     is tolerated (the kernels use a C ABI, no torch headers).  ``DS_SKIP_CUDA_CHECK=1`` downgrades errors to warnings."""
     major, minor = installed_cuda_version(name)
     problems = []
-    if (major, minor) < (12, 8):
-        problems.append(f"CUDA {major}.{minor} cannot compile for sm_100a (needs >= 12.8)")
+    if (major, minor) < (12, 0):
+        problems.append(f"CUDA {major}.{minor} cannot compile for sm_90a (needs >= 12.0)")
     try:
         import torch
         tv = torch.version.cuda
@@ -134,7 +134,7 @@ def assert_no_cuda_mismatch(name=""):
         if os.environ.get("DS_SKIP_CUDA_CHECK", "0") == "1":
             print("[WARNING] " + "; ".join(problems))
             return True
-        raise CUDAMismatchException(f">- DeepSpeed-B200 op builder ({name}): " + "; ".join(problems))
+        raise CUDAMismatchException(f">- DeepSpeed-H100 op builder ({name}): " + "; ".join(problems))
     return True
 
 
@@ -344,8 +344,8 @@ class CUDAOpBuilder(OpBuilder):
         return list(ARCH_FLAGS)
 
     def filter_ccs(self, ccs):
-        """Only sm_100a is ever built: every requested capability collapses to it."""
-        return [["10", "0a"]]
+        """Only sm_90a is ever built: every requested capability collapses to it."""
+        return [["9", "0a"]]
 
     def version_dependent_macros(self):
         return ["-DVERSION_GE_1_1", "-DVERSION_GE_1_3", "-DVERSION_GE_1_5"]

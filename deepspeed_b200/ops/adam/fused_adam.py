@@ -1,4 +1,4 @@
-"""``FusedAdam`` -- multi-tensor Adam/AdamW on sm_100a.
+"""``FusedAdam`` -- multi-tensor Adam/AdamW on sm_90a.
 
 Parity target: reference ``ops/adam/fused_adam.py`` + ``csrc/adam/multi_tensor_adam.cu`` (N1).
 One kernel launch updates every tensor of a (dtype-homogeneous) param group: a device-resident

@@ -6,9 +6,9 @@ returns ``[B*S, hq*d]``.  The backward produces one packed ``dqkv`` buffer and u
 
 Attention-core backends (``backend=`` or ``DSB200_ATTN``):
   * ``cudnn`` / ``flash`` / ``efficient`` / ``math`` -- ``torch.nn.functional.scaled_dot_product_attention``
-    with that SDPA backend (library path; cuDNN has a Blackwell FMHA);
+    with that SDPA backend (library path; cuDNN has a Hopper FMHA);
   * ``flash_attn`` -- the flash-attn package;
-  * ``native`` -- the framework's own sm_100a kernel (``csrc/cuda/attention.cu``) when built;
+  * ``native`` -- the framework's own sm_90a kernel (``csrc/cuda/attn_sm90.cu``) when built;
   * ``auto`` -- native if available, else cudnn -> flash -> efficient -> math priority order.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
@@ -91,10 +91,10 @@ _TABLE = None
 
 
 def _native_wins(B, S, hq, hkv, d) -> bool:
-    """``auto``: the measured per-shape choice between the in-tree tcgen05 kernel and the cuDNN library kernel
-    (``attention_table.json`` next to this file, written from ``scripts/bench_attention.py`` runs on a B200: fwd + bwd
-    milliseconds of both).  Unknown shapes use the library: on the shapes measured so far cuDNN's Blackwell FMHA is faster
-    (Llama-3-8B shape: forward 0.21 ms vs 0.64 ms), so the in-tree kernel is opt-in (``attention_backend="native"``)."""
+    """``auto``: the measured per-shape choice between the in-tree wgmma kernel and the cuDNN library kernel
+    (``attention_table.json`` next to this file, written from ``scripts/bench_attention.py`` runs on an H100: fwd + bwd
+    milliseconds of both).  Shapes not in the table use the library; no table has been measured on H100, so the in-tree
+    kernel is opt-in there (``attention_backend="native"``)."""
     global _TABLE
     if _TABLE is None:
         import json

@@ -2,8 +2,8 @@
 
 The weight arrives in :class:`FP_Quantize`'s flat layout (groups of ``quantization_group_size`` consecutive elements of
 the row-major ``[K, N]`` tensor, one fp32 scale per group). It is expanded once by the dequantisation kernel and the
-product runs on the library bf16 GEMM -- on B200 the expansion is bandwidth-trivial next to the GEMM for every ``M`` the
-training path uses. (Serving-side weight-only GEMMs with their own ``[N, K]`` group layout and a fused tcgen05 kernel live in
+product runs on the library bf16 GEMM -- on H100 the expansion is bandwidth-trivial next to the GEMM for every ``M`` the
+training path uses. (Serving-side weight-only GEMMs with their own ``[N, K]`` group layout and a fused wgmma kernel live in
 ``inference/quantization``.)"""
 import torch
 

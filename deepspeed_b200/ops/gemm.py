@@ -8,11 +8,11 @@ Every matrix product of the Llama-family step goes through one of
 * :func:`gate_up_swiglu`   ``silu(x Wg^T) * (x Wu^T)`` with the activation applied in the GEMM epilogue
 * :func:`down_dx_dswiglu`  ``(dY Wd) (.) dSwiGLU(gate, up)`` with the activation backward applied in the GEMM epilogue
 
-and is served either by the framework's own tcgen05 / TMEM / TMA kernel (``csrc/cuda/gemm_sm100.cu``, "own") or by
+and is served either by the framework's own wgmma / TMA kernel (``csrc/cuda/gemm_sm90.cu``, "own") or by
 cuBLASLt through ``torch.mm`` (+ the separate element-wise kernel for the fused forms, "lib").
 
 Which one runs is decided **per problem shape by a persisted table** (``gemm_table.json`` next to this file, produced by
-``scripts/tune_gemm.py`` on a B200 from >= 20 warm iterations per candidate with the clocks recorded).  A shape that is not
+``scripts/tune_gemm.py`` on an H100 from >= 20 warm iterations per candidate with the clocks recorded).  A shape that is not
 in the table is measured on first use with the same protocol (interleaved candidates, 5 warm-up + 20 timed iterations each,
 median), and the own kernel is kept unless the library is more than ``TIE_MARGIN`` faster: inside a training step both are
 power-capped, so an isolated few-percent edge of either does not survive, while the own kernel's fused epilogues do.
@@ -101,7 +101,7 @@ def _own_available():
         except Exception:
             _own_ok = False
         if not _own_ok and _backend == "own":
-            raise RuntimeError("DSB200_GEMM=own requested but the native tcgen05 GEMM failed its self check")
+            raise RuntimeError("DSB200_GEMM=own requested but the native wgmma GEMM failed its self check")
     return _own_ok
 
 

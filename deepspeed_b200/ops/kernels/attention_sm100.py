@@ -1,4 +1,4 @@
-"""Python face of ``csrc/cuda/attn_sm100.cu`` -- the tcgen05 / TMEM training attention (head dim 128, bf16, GQA, causal).
+"""Python face of ``csrc/cuda/attn_sm90.cu`` -- the wgmma training attention (head dim 128, bf16, GQA, causal).
 
 ``fwd`` / ``bwd`` work on 2-D ``[B*S, heads*128]`` views (row stride free), so the packed QKV projection output is consumed
 in place: Q, K and V are column ranges of ONE buffer and the backward writes dQ | dK | dV into one packed buffer that the

@@ -1,6 +1,6 @@
 """Flat-buffer optimizer / gradient ops (python face of ``csrc/cuda/optim.cu``).
 
-On CUDA tensors these call the sm_100a kernels (a missing native library is a hard error).  On
+On CUDA tensors these call the sm_90a kernels (a missing native library is a hard error).  On
 host tensors they run an equivalent pure-torch implementation so the gloo/CPU test tier exercises
 the same engine logic.  Reference counterparts: ``ops/adam/fused_adam.py`` (N1),
 ``runtime/utils.py`` norm/clip helpers, ``stage3.py:2178 unscale_and_clip_grads``.

@@ -1,4 +1,4 @@
-"""Python face of ``csrc/cuda/gemm_sm100.cu`` -- the hand-written tcgen05 / TMEM / TMA GEMM."""
+"""Python face of ``csrc/cuda/gemm_sm90.cu`` -- the hand-written wgmma / TMA GEMM for sm_90a."""
 import ctypes
 
 import torch
@@ -44,7 +44,7 @@ def supports_grouped(x, w, offsets) -> bool:
 
 
 def grouped_matmul_nt(x, w, offsets, out=None, sms=0):
-    """Grouped (MoE) GEMM: ``out[r] = x[r] @ w[e]^T`` for ``offsets[e] <= r < offsets[e+1]`` in ONE persistent tcgen05
+    """Grouped (MoE) GEMM: ``out[r] = x[r] @ w[e]^T`` for ``offsets[e] <= r < offsets[e+1]`` in ONE persistent wgmma
     launch; ``offsets`` stays on the device (no host sync, CUDA-graph capturable)."""
     R, K = x.shape
     E, Nn, _ = w.shape
@@ -57,7 +57,7 @@ def grouped_matmul_nt(x, w, offsets, out=None, sms=0):
 
 
 def matmul_nt_2cta(a, b, out=None, sms=0):
-    """Same contract as :func:`matmul_nt`, CTA-pair kernel (``tcgen05.mma.cta_group::2``, 256x256 tiles)."""
+    """Same contract as :func:`matmul_nt` through the general entry point (grouped tile rasterisation)."""
     M, K = a.shape
     Nn = b.shape[0]
     if out is None:
@@ -72,7 +72,7 @@ EPI_STORE, EPI_ACCUM, EPI_SWIGLU, EPI_DSWIGLU = 0, 1, 2, 3
 
 
 def matmul_2cta(a, b, a_mn: bool, b_mn: bool, out=None, sms=0, epi=EPI_STORE, aux=None, out2=None, inter=0, group_m=8):
-    """CTA-pair kernel with selectable operand majorness and fused epilogue.
+    """General kernel with selectable operand majorness and fused epilogue.
 
     ``a_mn=False``: ``a`` is [M, K];  ``a_mn=True``: ``a`` is [K, M] (the kernel multiplies by its transpose).
     ``b_mn=False``: ``b`` is [N, K];  ``b_mn=True``: ``b`` is [K, N].
@@ -80,7 +80,7 @@ def matmul_2cta(a, b, a_mn: bool, b_mn: bool, out=None, sms=0, epi=EPI_STORE, au
     ``epi``: ``EPI_ACCUM`` adds into ``out``; ``EPI_SWIGLU`` -- ``b`` is ``[2*inter, K]`` (gate rows, then up rows), ``out``
     is ``[M, inter]`` = ``silu(gate) * up`` and ``out2`` (optional ``[M, 2*inter]``) receives gate|up; ``EPI_DSWIGLU`` --
     ``aux`` is the saved gate|up ``[M, 2*inter]``, ``out`` the dgate half and ``out2`` the whole ``[M, 2*inter]`` dgate|dup.
-    ``group_m``: m-blocks per rasterisation super-group (L2 locality)."""
+    ``group_m``: 128-row m-blocks per rasterisation super-group (L2 locality)."""
     M, K = (a.shape[1], a.shape[0]) if a_mn else (a.shape[0], a.shape[1])
     if epi == EPI_SWIGLU:
         Nn = inter

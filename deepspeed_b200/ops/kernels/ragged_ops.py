@@ -92,7 +92,7 @@ def paged_attention(qkv, cache, seq_of, pos_of, block_table, hq, hkv, d, block_s
     if qkv.is_cuda:
         out = torch.empty(T, hq * d, dtype=qkv.dtype, device=qkv.device)
         if _decode_eligible(qkv, hq, hkv, d) and os.environ.get("DSB200_PAGED_V1", "0") != "1":
-            # split the KV range so (tokens x kv_heads x splits) covers the 148 SMs a few times over; the split count
+            # split the KV range so (tokens x kv_heads x splits) covers the 132 SMs a few times over; the split count
             # depends only on static shapes (graph-capturable: no device->host read of the positions)
             max_ctx = max_blocks * block_size
             nsplit = 1

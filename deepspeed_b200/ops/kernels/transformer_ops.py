@@ -1,7 +1,7 @@
 """Autograd-aware python face of ``csrc/cuda/transformer.cu``.
 
 ``rms_norm`` / ``layer_norm`` / ``rope`` / ``gated_act`` (SwiGLU...) / ``softmax_cross_entropy`` /
-``bias_act``.  CUDA tensors go to the sm_100a kernels (hard error if the native library is missing);
+``bias_act``.  CUDA tensors go to the sm_90a kernels (hard error if the native library is missing);
 host tensors use an equivalent fp32 torch implementation so models run unchanged in the CPU tier.
 Reference counterparts: ``ops/transformer/inference/op_binding/*`` (N8 wrappers) and the training
 layer's norm / gelu ops (N7).

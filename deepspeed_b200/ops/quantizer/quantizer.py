@@ -2,7 +2,7 @@
 
 Parity target: reference ``ops/quantizer/quantizer.py`` + ``csrc/quantization/pt_binding.cpp:372-401``
 (``quantize``, ``dequantize``, ``swizzle_quant``, ``quantized_reduction``, ``loco_*``, ``ds_quantize_*``,
-``ds_sr_quantize_*``).  CUDA tensors use the sm_100a kernels; host tensors use an equivalent torch path so
+``ds_sr_quantize_*``).  CUDA tensors use the sm_90a kernels; host tensors use an equivalent torch path so
 ZeRO++ logic is testable on CPU.
 """
 import ctypes

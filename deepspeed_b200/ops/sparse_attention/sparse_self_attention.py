@@ -1,7 +1,7 @@
 """Block-sparse self attention (reference ``ops/sparse_attention/sparse_self_attention.py`` +
 Triton ``matmul.py``/``softmax.py``).
 
-B200 formulation: on the GPU (bf16 / fp16, head dim 16 / 32 / 64, power-of-two block >= 16) ONE flash-attention kernel
+H100 formulation: on the GPU (bf16 / fp16, head dim 16 / 32 / 64, power-of-two block >= 16) ONE flash-attention kernel
 (``csrc/cuda/attn_bias.cu``) replaces the reference's SDD-matmul -> block softmax -> DSD-matmul chain: the layout is read
 inside the kernel, score tiles without any active block are skipped (work scales with the number of non-zero blocks),
 inactive blocks inside a tile are masked, and the key-padding / attention masks ride the kernel's two additive-bias slots;

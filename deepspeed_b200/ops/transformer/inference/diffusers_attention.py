@@ -30,7 +30,7 @@ class DeepSpeedDiffusersAttention(nn.Module):
 
 
 def load_triton_flash_attn():
-    """The reference swaps in a Triton flash-attention for diffusers shapes; the fused SDPA (cuDNN flash on sm_100a) plays
+    """The reference swaps in a Triton flash-attention for diffusers shapes; the fused SDPA (cuDNN flash on sm_90a) plays
     that role here, so there is nothing to load -- returns the function used."""
     return F.scaled_dot_product_attention
 

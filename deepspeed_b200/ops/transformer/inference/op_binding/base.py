@@ -1,7 +1,7 @@
 """Base of the v1 inference op bindings (reference ``ops/transformer/inference/op_binding/base.py``).
 
 The reference resolves each op to a ``*_fp16`` / ``*_bf16`` / ``*_fp32`` symbol of one monolithic extension.  Here every
-op is a thin callable over the typed sm_100a kernels in ``ops/kernels`` (dtype dispatch happens in the C ABI), with a
+op is a thin callable over the typed sm_90a kernels in ``ops/kernels`` (dtype dispatch happens in the C ABI), with a
 torch path for host tensors, so a binding holds nothing but the layer config.
 """
 import torch
@@ -22,7 +22,7 @@ class BaseOp(torch.nn.Module):
 
 def gemm_linear(x, weight, bias=None):
     """``x @ weight^T (+ bias)`` for the inference op bindings: bf16 CUDA problems with at least one 256x128 tile go to the
-    framework's tcgen05 GEMM through :mod:`deepspeed_b200.ops.gemm` (persisted per-shape choice vs cuBLAS), weight-only
+    framework's wgmma GEMM through :mod:`deepspeed_b200.ops.gemm` (persisted per-shape choice vs cuBLAS), weight-only
     quantised weights to the fused dequant kernels, everything else (decode-sized rows, fp16/fp32, host) to the library --
     the role of the reference's ``cublas_gemm_ex`` calls in ``csrc/transformer/inference/csrc/pt_binding.cpp``."""
     import torch.nn.functional as F

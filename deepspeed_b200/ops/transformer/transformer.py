@@ -4,8 +4,8 @@ API parity: reference ``ops/transformer/transformer.py`` (``DeepSpeedTransformer
 ``DeepSpeedTransformerLayer :296``) over the ``csrc/transformer`` kernels (N7).  One layer =
 ``[LN] -> QKV GEMM -> (bias + [b,s,3,h,d]->[3,b,h,s,d]) -> attention (flash, or scores+masked-softmax+dropout when
 attention dropout is on) -> out GEMM -> bias+dropout+residual -> [LN] -> FF1 GEMM + bias-GELU -> FF2 GEMM ->
-bias+dropout+residual [-> LN]``.  The elementwise stages are this repo's sm_100a kernels (``transformer.cu``,
-``misc.cu``); GEMMs go through ``ops.gemm`` (tcgen05 / cuBLAS).  ``normalize_invertible`` / ``gelu_checkpoint`` /
+bias+dropout+residual [-> LN]``.  The elementwise stages are this repo's sm_90a kernels (``transformer.cu``,
+``misc.cu``); GEMMs go through ``ops.gemm`` (wgmma / cuBLAS).  ``normalize_invertible`` / ``gelu_checkpoint`` /
 ``attn_dropout_checkpoint`` map to activation recomputation of the corresponding stage.
 """
 import json
@@ -18,7 +18,7 @@ from torch.utils.checkpoint import checkpoint
 
 from deepspeed_b200.ops.kernels import misc_ops as K
 from deepspeed_b200.ops.kernels import transformer_ops as T
-from deepspeed_b200.ops.linear import flat_linear  # forward + both backward GEMMs on the tcgen05 kernel (ops.gemm)
+from deepspeed_b200.ops.linear import flat_linear  # forward + both backward GEMMs on the wgmma kernel (ops.gemm)
 
 
 class TransformerConfig:

@@ -225,7 +225,7 @@ class FlopsProfiler:
         p = partial(print, file=out)
         total_flops, total_macs = self.get_total_flops(), self.get_total_macs()
         total_dur, total_params = self.get_total_duration(), self.get_total_params()
-        p("\n-------------------------- DeepSpeed-B200 Flops Profiler --------------------------")
+        p("\n-------------------------- DeepSpeed-H100 Flops Profiler --------------------------")
         p(f"Profile Summary at step {profile_step}:")
         p("Notations:\n  data parallel size (dp_size), model parallel size(mp_size),\n  number of parameters (params), "
           "number of multiply-accumulate operations(MACs),\n  number of floating-point operations (flops), "

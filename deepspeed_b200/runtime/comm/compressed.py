@@ -38,7 +38,7 @@ def _native(t):
 
 def compress_with_feedback(work: torch.Tensor, error_out: torch.Tensor):
     """``work`` (already holding value + previous error) -> ``(packed signs, scale)``; writes the new error
-    ``work - scale * sign(work)`` into ``error_out``.  One fused sm_100a pass on the device (``misc.cu onebit_pack``)."""
+    ``work - scale * sign(work)`` into ``error_out``.  One fused sm_90a pass on the device (``misc.cu onebit_pack``)."""
     scale = work.norm() / (work.numel()**0.5)
     if _native(work) and _native(error_out) and work.numel() % 8 == 0:
         from deepspeed_b200.ops import native as N

@@ -1,5 +1,5 @@
 """Sign-bit packing backend (reference ``runtime/compression/cupy.py:CupyBackend``), without cupy: the packing is the
-``pack_signs`` / ``unpack_signs`` pair of ``runtime/comm/compressed.py`` (sm_100a kernel on device, torch on host)."""
+``pack_signs`` / ``unpack_signs`` pair of ``runtime/comm/compressed.py`` (sm_90a kernel on device, torch on host)."""
 import torch
 
 from deepspeed_b200.runtime.comm.compressed import pack_signs, unpack_signs

@@ -260,7 +260,7 @@ class CompileConfig(DeepSpeedConfigModel):
 
 
 class CUDAGraphConfig(DeepSpeedConfigModel):
-    """B200-native addition: capture the optimizer step / small-model step in a CUDA graph."""
+    """H100-native addition: capture the optimizer step / small-model step in a CUDA graph."""
     enabled: bool = False
     capture_optimizer_step: bool = True
     capture_full_step: bool = False

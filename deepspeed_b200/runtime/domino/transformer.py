@@ -3,7 +3,7 @@
 Parity target: reference ``runtime/domino/transformer.py`` (``DominoTransformerLayer :228``, ``forward
 :349-451``, ``ShardedAttention :137``).  The micro-batch is split in two halves; the row-parallel all-reduce of
 half 0 (attention output, then MLP output) is launched asynchronously and waited for only after half 1's
-compute of the same stage has been issued, so NVLink traffic overlaps tcgen05 math.  Backward uses the same
+compute of the same stage has been issued, so NVLink traffic overlaps wgmma math.  Backward uses the same
 trick through autograd hooks on the async handles (``_AsyncAllReduce``).
 """
 import torch

@@ -950,10 +950,10 @@ class DeepSpeedEngine(CheckpointMixin, EngineConfigAccessors, nn.Module):
         reload_states(self.optimizer, non_blocking)
 
     def compile(self, backend=None, compile_kwargs=None, schedule=None):
-        """The reference wraps ``torch.compile``; on B200 the hot path is hand-written CUDA plus CUDA
+        """The reference wraps ``torch.compile``; on H100 the hot path is hand-written CUDA plus CUDA
         graphs, so this only records the request (kept for API compatibility)."""
         self._is_compiled = True
-        log_dist("engine.compile(): no-op -- deepspeed_b200 uses native sm_100a kernels + CUDA graphs", ranks=[0])
+        log_dist("engine.compile(): no-op -- deepspeed_b200 uses native sm_90a kernels + CUDA graphs", ranks=[0])
 
     @property
     def is_compiled(self):

@@ -1,6 +1,6 @@
 """ZeRO config (reference: ``runtime/zero/config.py:86 DeepSpeedZeroConfig``).
 
-All reference keys are accepted with the same defaults.  B200-specific additions live under
+All reference keys are accepted with the same defaults.  H100-specific additions live under
 ``b200_*`` keys and default to the fused NVLink paths when the symmetric arena is available:
 
 * ``b200_fused_collectives``: ``"auto" | true | false`` -- use in-kernel peer-memory
@@ -112,7 +112,7 @@ class DeepSpeedZeroConfig(DeepSpeedConfigModel):
     override_module_apply: bool = True
     log_trace_cache_warnings: bool = False
 
-    # ---- B200-native knobs -------------------------------------------------------------
+    # ---- H100-native knobs -------------------------------------------------------------
     b200_fused_collectives: Optional[bool] = None  # None == auto (on when symmetric arena is up)
     b200_unit_prefetch: int = Field(1, ge=0)
     b200_fused_optimizer_in_backward: Optional[bool] = None  # None == auto (on when no clipping / GAS==1)

@@ -1,7 +1,7 @@
 """Optimizers that act on the rank-local flat arenas of :class:`ZeroShardedOptimizer`.
 
 A *flat optimizer* owns optimizer state tensors with the same length as the master arena and
-updates one contiguous segment per call.  This is how the fused sm_100a kernels are reached: one
+updates one contiguous segment per call.  This is how the fused sm_90a kernels are reached: one
 launch per (param-group run) instead of the reference's per-tensor multi-tensor-apply chunking
 (``ops/adam/fused_adam.py`` + ``csrc/adam/multi_tensor_apply.cuh``).
 

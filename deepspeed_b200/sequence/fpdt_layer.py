@@ -12,7 +12,7 @@ written on a device->host stream and prefetched one pair ahead on a host->device
 query chunks from last to first, calling the per-pair flash backward with the GLOBAL log-sum-exp of the query chunk, so no
 pair is recomputed in forward mode and device memory holds O(chunk) activations for arbitrarily long sequences.
 
-The per-pair kernels are the framework's own: head dim 128 / bf16 -> the tcgen05 flash attention (``attn_sm100.cu``, returns
+The per-pair kernels are the framework's own: head dim 128 / bf16 -> the wgmma flash attention (``attn_sm90.cu``, returns
 LSE, takes it back in backward), head dim 16 / 32 / 64 -> the register-accumulator kernels of ``attn_bias.cu``; anything
 else (CPU, fp32) uses the fp32 PyTorch formulation below.
 """

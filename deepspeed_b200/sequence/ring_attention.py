@@ -15,7 +15,7 @@ from deepspeed_b200 import comm as dist
 
 
 class _RingAttention(torch.autograd.Function):
-    """Per-hop attention and its backward run on the framework's pair kernels (``fpdt_layer._pair_fwd / _pair_bwd``: tcgen05
+    """Per-hop attention and its backward run on the framework's pair kernels (``fpdt_layer._pair_fwd / _pair_bwd``: wgmma
     flash attention for head dim 128 / bf16, the register-accumulator kernels for head dims 16-64, fp32 PyTorch otherwise);
     like FPDT, the backward of every (local Q, visiting K/V) pair uses the FINAL output and log-sum-exp of the local queries,
     so the pair contributions simply add and nothing is recomputed in forward mode."""

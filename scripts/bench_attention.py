@@ -1,4 +1,4 @@
-"""Training-attention micro-benchmark at the Llama-3-8B shape: the in-tree tcgen05 kernel vs cuDNN / flash SDPA.
+"""Training-attention micro-benchmark at the Llama-3-8B shape: the in-tree wgmma kernel vs cuDNN / flash SDPA.
 CUDA events, 5 warm-up + 20 timed iterations, inputs (100+ MB per call) rotate through 4 buffers so L2 does not help."""
 import argparse
 import json

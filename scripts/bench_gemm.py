@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs cuBLAS on the Llama-3-8B forward shapes (CUDA events, L2 flushed between iterations)."""
+"""wgmma GEMM vs cuBLAS on the Llama-3-8B forward shapes (CUDA events, L2 flushed between iterations)."""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Ragged-engine serving microbenchmark: prefill + CUDA-graphed decode throughput on one B200.
+"""Ragged-engine serving microbenchmark: prefill + CUDA-graphed decode throughput on one H100.
 python scripts/bench_inference.py [--model llama3-8b] [--batch 64] [--prompt 512] [--new 64]"""
 import argparse
 import json

@@ -1,4 +1,4 @@
-"""Mixtral-8x7B MoE block (H=4096, I=14336, 8 experts, top-2) on the ragged engine: grouped tcgen05 GEMM path vs the
+"""Mixtral-8x7B MoE block (H=4096, I=14336, 8 experts, top-2) on the ragged engine: grouped wgmma GEMM path vs the
 per-expert / dense-all-experts paths.  Device-timed, L2 flushed between iterations."""
 import json
 import os

@@ -1,4 +1,4 @@
-"""Weight-only-quantised linear at prefill / batched-decode sizes: the fused dequantise-in-smem tcgen05 kernel
+"""Weight-only-quantised linear at prefill / batched-decode sizes: the fused dequantise-in-smem wgmma kernel
 (csrc/cuda/wq_tc_gemm.cu) vs dequantise-once + bf16 GEMM, per mode and row count.  CUDA events, rotating weights (> L2),
 median of 20.  Writes gpurun_out/wq_tc_bench.json; the crossover feeds WQ_TC_MAX_ROWS in inference/quantization/layers.py."""
 import json

@@ -17,7 +17,7 @@ echo "gpu tests rc=$?" >> gpurun_out/r2a_status.txt
 tail -3 gpurun_out/r2a_gemm_tests.log; grep -E "dswiglu|wrote" gpurun_out/r2a_tune.log; for f in gpurun_out/r2a_bench_n1*.json; do python - "$f" <<'PY'
 import json,sys
 try:
-    d=json.loads(open(sys.argv[1]).read().strip().splitlines()[-1]); print(sys.argv[1], d["value"], d["ms_per_step"], d["e2e"]["value"], d["details"]["gemm_choices"]["own_tcgen05"], d["details"]["gemm_choices"]["cublas_shapes"], d["details"]["fused_in_backward_optimizer"])
+    d=json.loads(open(sys.argv[1]).read().strip().splitlines()[-1]); print(sys.argv[1], d["value"], d["ms_per_step"], d["e2e"]["value"], d["details"]["gemm_choices"]["own_wgmma"], d["details"]["gemm_choices"]["cublas_shapes"], d["details"]["fused_in_backward_optimizer"])
 except Exception as e: print(sys.argv[1], "ERR", e)
 PY
 done; tail -3 gpurun_out/r2a_gpu_tests.log; cat gpurun_out/r2a_status.txt

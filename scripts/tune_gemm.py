@@ -1,4 +1,4 @@
-"""Build ``deepspeed_b200/ops/gemm_table.json``: the persisted per-shape choice between the in-tree tcgen05 GEMM ("own") and
+"""Build ``deepspeed_b200/ops/gemm_table.json``: the persisted per-shape choice between the in-tree wgmma GEMM ("own") and
 cuBLASLt ("lib") for every GEMM problem of the benchmark models' training step.
 
 Protocol per problem: candidates alternate (so clock drift hits them equally), 5 warm-up + ``--iters`` (>= 20) timed

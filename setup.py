@@ -2,7 +2,7 @@
 """Packaging for deepspeed_b200.
 
 ``pip install .`` installs the Python package and the ``bin/`` entry points.  The two native libraries
-(``libdsb200_cuda.so`` for sm_100a, ``libdsb200_cpu.so`` for the host runtime) are built IN-TREE into ``deepspeed_b200/lib``:
+(``libdsb200_cuda.so`` for sm_90a, ``libdsb200_cpu.so`` for the host runtime) are built IN-TREE into ``deepspeed_b200/lib``:
 
 * ``python setup.py build_ext --inplace`` (or ``DS_BUILD_OPS=1 pip install .``) compiles them ahead of time;
 * otherwise they are compiled on first use by the op builders (``deepspeed_b200/op_builder``), like the reference's JIT path.
@@ -34,7 +34,7 @@ def read_requirements(name):
 
 class BuildNative(Command):
     """Compile both native libraries into ``deepspeed_b200/lib``."""
-    description = "build the sm_100a CUDA library and the host runtime library in-tree"
+    description = "build the sm_90a CUDA library and the host runtime library in-tree"
     user_options = [("inplace", "i", "accepted for compatibility (libraries are always built in-tree)"),
                     ("parallel=", "j", "number of parallel compile jobs")]
 
@@ -65,7 +65,7 @@ scripts = [os.path.join("bin", f) for f in sorted(os.listdir(os.path.join(ROOT, 
 setup(
     name="deepspeed_b200",
     version=read_version(),
-    description="B200-native (sm_100a) large-model training and inference framework with the DeepSpeed feature set",
+    description="H100-native (sm_90a) large-model training and inference framework with the DeepSpeed feature set",
     long_description=open(os.path.join(ROOT, "README.md")).read(),
     long_description_content_type="text/markdown",
     packages=find_packages(include=["deepspeed_b200", "deepspeed_b200.*"]),

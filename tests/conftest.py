@@ -11,7 +11,7 @@ os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100 with -m gpu)")
     config.addinivalue_line("markers", "world_size(n): number of ranks for a distributed test")
     config.addinivalue_line("markers", "slow: long-running test")
 

@@ -1,4 +1,4 @@
-"""GPU tier: the tcgen05 training attention kernel against an fp32 reference."""
+"""GPU tier: the wgmma training attention kernel against an fp32 reference."""
 import math
 
 import pytest
@@ -36,7 +36,7 @@ def test_attn_fwd_matches_fp32(B, S, hq, hkv, causal):
     assert torch.isfinite(got).all()
     assert (got - ref_o).abs().max().item() < 2e-2, (got - ref_o).abs().max().item()
     assert (lse - ref_lse).abs().max().item() < 2e-2
-    # repeated launches: barrier phases / TMEM reuse stay correct
+    # repeated launches: barrier phases / registers reuse stay correct
     o2, _ = A.fwd(q2, k2, v2, B, S, hq, hkv, causal=causal)
     assert torch.equal(o, o2)
 

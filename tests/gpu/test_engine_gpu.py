@@ -1,4 +1,4 @@
-"""GPU tier: engine + flagship model end to end on one B200."""
+"""GPU tier: engine + flagship model end to end on one H100."""
 import pytest
 import torch
 

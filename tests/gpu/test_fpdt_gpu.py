@@ -1,4 +1,4 @@
-"""FPDT chunked attention on the GPU: native per-pair kernels (tcgen05 for head dim 128, register-accumulator kernels for
+"""FPDT chunked attention on the GPU: native per-pair kernels (wgmma for head dim 128, register-accumulator kernels for
 head dim 64) + the double-buffered host offload of q / k / v / o chunks, against dense SDPA."""
 import pytest
 import torch

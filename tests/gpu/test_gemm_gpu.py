@@ -1,4 +1,4 @@
-"""GPU tier: the tcgen05 GEMM against an fp32 reference."""
+"""GPU tier: the wgmma GEMM against an fp32 reference."""
 import pytest
 import torch
 
@@ -38,7 +38,7 @@ def test_gemm_strided_views_and_fewer_sms():
 @pytest.mark.parametrize("shape", [(256, 256, 64), (128, 256, 64), (512, 512, 128), (384, 768, 320), (1000, 1000, 264),
                                    (2048, 6144, 4096), (4096, 4096, 14336), (8192, 28672, 4096)])
 def test_gemm_2cta_matches_fp32(shape):
-    """CTA-pair (tcgen05.mma.cta_group::2) kernel, including M/N edges that leave one CTA of a pair without rows."""
+    """General-entry kernel, including M/N edges that leave a tile partly or entirely outside the matrix."""
     from deepspeed_b200.ops.kernels import gemm_sm100
     M, N, K = shape
     torch.manual_seed(M + N + K)
@@ -49,7 +49,7 @@ def test_gemm_2cta_matches_fp32(shape):
     lib = torch.matmul(a, b.t())
     scale = lib.float().abs().max().item()
     assert (c.float() - lib.float()).abs().max().item() < 2e-2 * scale + 1e-2
-    # repeated launches (barrier phases, TMEM double buffering across many tiles) stay correct
+    # repeated launches (barrier phases, registers double buffering across many tiles) stay correct
     for _ in range(3):
         c2 = gemm_sm100.matmul_nt_2cta(a, b)
     assert torch.equal(c, c2)
@@ -98,7 +98,7 @@ def test_flat_linear_backward_uses_native_gemm_and_matches_autograd():
 @pytest.mark.parametrize("counts", [[300, 0, 17, 128, 1, 513], [0, 0, 5, 0], [256, 256]])
 @pytest.mark.parametrize("N,K", [(512, 256), (328, 192)])
 def test_grouped_gemm_matches_per_expert_loop(counts, N, K):
-    """Device-driven grouped tcgen05 GEMM (MoE): ragged expert extents incl. empty experts, N not a tile multiple."""
+    """Device-driven grouped wgmma GEMM (MoE): ragged expert extents incl. empty experts, N not a tile multiple."""
     from deepspeed_b200.ops.kernels import gemm_sm100
     torch.manual_seed(0)
     E, rows = len(counts), sum(counts)
@@ -174,7 +174,7 @@ def test_gemm_swiglu_epilogue(T, H, I):
 
 @pytest.mark.parametrize("T,H,I", [(256, 128, 256), (1000, 320, 392), (4096, 4096, 14336)])
 def test_gemm_dswiglu_epilogue(T, H, I):
-    """EPI_DSWIGLU: dgate|dup = dSwiGLU(dY W_down, gate|up) with the [T, I] intermediate gradient kept in TMEM."""
+    """EPI_DSWIGLU: dgate|dup = dSwiGLU(dY W_down, gate|up) with the [T, I] intermediate gradient kept in registers."""
     from deepspeed_b200.ops.kernels import gemm_sm100
     torch.manual_seed(T + I)
     dy = (torch.randn(T, H, device="cuda") * 0.5).bfloat16()
@@ -219,7 +219,7 @@ def test_swiglu_mlp_matches_autograd(backend):
 
 
 def test_grouped_swiglu_experts_match_bmm_reference():
-    """MoE training experts: tcgen05 per-expert fused path vs the batched-GEMM autograd reference."""
+    """MoE training experts: wgmma per-expert fused path vs the batched-GEMM autograd reference."""
     from deepspeed_b200.moe.experts import GroupedSwiGLUExperts
     torch.manual_seed(0)
     E, C, H, I = 2, 512, 256, 384

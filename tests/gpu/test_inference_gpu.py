@@ -1,4 +1,4 @@
-"""Ragged inference kernels + engine on a B200: device kernels vs their host definitions, engine vs HF."""
+"""Ragged inference kernels + engine on an H100: device kernels vs their host definitions, engine vs HF."""
 import pytest
 import torch
 
@@ -204,7 +204,7 @@ def test_layerwise_kernel_injection_bf16_gpu():
 @pytest.mark.parametrize("mode", ["fp6", "fp8", "int8", "int4"])
 @pytest.mark.parametrize("M,N,K", [(48, 256, 512), (200, 384, 1024), (128, 4096, 4096)])
 def test_wq_tc_gemm_matches_dequant_reference(mode, M, N, K):
-    """Fused dequantise-in-smem + tcgen05 weight-only GEMM (FP6 / FP8 / INT8 / INT4) vs dequantise + fp32 matmul."""
+    """Fused dequantise-in-smem + wgmma weight-only GEMM (FP6 / FP8 / INT8 / INT4) vs dequantise + fp32 matmul."""
     import torch
     from deepspeed_b200.inference.quantization.layers import quantize_weight, wq_tc_linear
     torch.manual_seed(M + N)
@@ -213,7 +213,7 @@ def test_wq_tc_gemm_matches_dequant_reference(mode, M, N, K):
     b = (torch.randn(N, device="cuda") * 0.1).bfloat16()
     qw = quantize_weight(w, mode, group_size=128)
     y = wq_tc_linear(x, qw, b)
-    assert y is not None, "shape should be eligible for the tcgen05 weight-only kernel"
+    assert y is not None, "shape should be eligible for the wgmma weight-only kernel"
     ref = x.float() @ qw.dequantize().float().t() + b.float()
     assert torch.isfinite(y.float()).all()
     assert (y.float() - ref).abs().max().item() < 2e-2 * ref.abs().max().item() + 2e-2
@@ -221,7 +221,7 @@ def test_wq_tc_gemm_matches_dequant_reference(mode, M, N, K):
 
 @pytest.mark.parametrize("mode", ["int8", "fp6"])
 def test_mixed_moe_gemm_grouped_single_launch(mode):
-    """MixedMoEGEMM: expert-sorted rows x weight-only-quantised expert weights in one grouped tcgen05 launch (device-side
+    """MixedMoEGEMM: expert-sorted rows x weight-only-quantised expert weights in one grouped wgmma launch (device-side
     expert extents) vs the per-expert dequantise + matmul reference; includes an empty expert and a ragged tail."""
     import torch
     from deepspeed_b200.inference.quantization.layers import quantize_weight

@@ -1,4 +1,4 @@
-"""GPU tier: every sm_100a kernel against a plain PyTorch fp32 reference of the same op."""
+"""GPU tier: every sm_90a kernel against a plain PyTorch fp32 reference of the same op."""
 import math
 
 import pytest

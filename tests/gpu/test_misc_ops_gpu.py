@@ -1,4 +1,4 @@
-"""sm_100a kernels of misc.cu / quant.cu / moe_ragged.cu vs their host (plain PyTorch fp32) definitions."""
+"""sm_90a kernels of misc.cu / quant.cu / moe_ragged.cu vs their host (plain PyTorch fp32) definitions."""
 import pytest
 import torch
 

@@ -104,8 +104,7 @@ def test_symm_collectives(world):
 
 def _rs_adam_kernel():
     """The fused reduce-scatter (+) AdamW kernel against a torch reference of the same update, at a Llama-3-8B unit size,
-    normal and tail (all-SM) launch; records achieved NVLink bytes/s as a fraction of the 770 GB/s per-direction peer-copy
-    reference (B200_PROFILING.md) in gpurun_out/."""
+    normal and tail (all-SM) launch."""
     import json
     import types
     import torch.distributed as dist

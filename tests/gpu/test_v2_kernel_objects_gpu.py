@@ -1,4 +1,4 @@
-"""Kernel objects / module layer of the ragged engine on the device: the sm_100a kernels behind them must agree with the
+"""Kernel objects / module layer of the ragged engine on the device: the sm_90a kernels behind them must agree with the
 host (plain torch fp32) path of the very same objects."""
 import pytest
 import torch

@@ -401,56 +401,14 @@ def test_deepspeed_checkpoint_layer_file_maps(tmp_path):
     ck1.show_pp_transformer_map()
 
 
-# ---- interop with the UNMODIFIED reference (baseline/_ref), both directions -------------------------------------------
-_REF = os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), "baseline", "_ref")
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(_REF, "deepspeed")), reason="baseline/_ref is not installed")
-
-_REF_SAVE = r'''
-import os, sys
-sys.path.insert(0, {ref!r})
-os.environ.setdefault("DS_ACCELERATOR", "cpu")
-import torch, torch.distributed as dist
-import deepspeed
-sys.path.insert(0, {root!r})
-from tests.unit.simple_model import SimpleModel, make_batch
-out, stage = sys.argv[1], int(sys.argv[2])
-deepspeed.init_distributed(dist_backend="gloo")
-r, w = dist.get_rank(), dist.get_world_size()
-torch.manual_seed(0)
-model = SimpleModel()
-cfg = {{"train_micro_batch_size_per_gpu": 4, "zero_optimization": {{"stage": stage, "stage3_param_persistence_threshold": 0}},
-       "zero_allow_untested_optimizer": True, "zero_force_ds_cpu_optimizer": False}}
-opt = torch.optim.AdamW(model.parameters(), lr=1e-2, weight_decay=0.01)
-eng, *_ = deepspeed.initialize(model=model, optimizer=opt, config=cfg)
-g = torch.Generator().manual_seed(1)
-def steps(n):
-    for _ in range(n):
-        x, y = make_batch(w, 4, g)
-        eng.backward(eng(x[r*4:(r+1)*4], y[r*4:(r+1)*4])); eng.step()
-steps(3)
-eng.save_checkpoint(out, tag="ref3", client_state={{"hello": 7}})
-steps(2)
-from deepspeed.utils import safe_get_full_fp32_param
-full = {{n: safe_get_full_fp32_param(p).detach().cpu().clone() for n, p in eng.module.named_parameters()}}
-if r == 0:
-    torch.save(full, os.path.join(out, "expect_after5.pt"))
-dist.barrier()
-'''
-
-
-def _run_ref_save(d, stage):
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    script = os.path.join(d, "ref_save.py")
-    with open(script, "w") as f:
-        f.write(_REF_SAVE.format(ref=_REF, root=root))
-    env = dict(os.environ, DS_ACCELERATOR="cpu", PYTHONPATH=root)
-    port = 29700 + os.getpid() % 200
-    p = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr",
-                        "127.0.0.1", "--master-port", str(port), script, d, str(stage)], env=env, capture_output=True,
-                       text=True, timeout=600)
-    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
+# ---- interop with stock DeepSpeed, both directions -------------------------------------------------------------------
+# Fixtures under tests/golden/checkpoint, made once with the original DeepSpeed package (CPU, gloo, 2 ranks, SimpleModel):
+#   stock_s{2,3}/  what stock DeepSpeed saved at ZeRO-2 / ZeRO-3 after 3 AdamW steps (tag "ref3", client_state
+#                  {"hello": 7}), plus expect_after5.pt: its full fp32 parameters after 2 more steps on the next batches of
+#                  the same generator;
+#   ours_s{1,3}/   what _save_worker below saves (tag "t3"), plus consolidated/pytorch_model.bin: the output of stock
+#                  DeepSpeed's own zero_to_fp32.py run on exactly that checkpoint.
+_GOLDEN_CKPT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "golden", "checkpoint")
 
 
 def _resume_from_ref_worker(d, stage):
@@ -475,37 +433,50 @@ def _resume_from_ref_worker(d, stage):
         torch.testing.assert_close(safe_get_full_fp32_param(p).cpu(), exp[n], atol=2e-6, rtol=1e-5)
 
 
-@needs_ref
 @pytest.mark.parametrize("stage", [2, 3])
 def test_resume_in_engine_from_stock_deepspeed_checkpoint(tmp_path, stage):
-    """(i) the unmodified reference trains 3 steps on gloo ws=2 and saves; this engine resumes from those files and its
-    next 2 steps land on the reference's own continuation."""
-    d = str(tmp_path)
-    _run_ref_save(d, stage)
+    """(i) stock DeepSpeed trained 3 steps on gloo ws=2 and saved; this engine resumes from those files and its next 2
+    steps land on stock DeepSpeed's own continuation."""
+    import shutil
+    d = str(tmp_path / "ckpt")
+    shutil.copytree(os.path.join(_GOLDEN_CKPT, f"stock_s{stage}"), d)
     run_distributed(_resume_from_ref_worker, 2, (d, stage))
 
 
-@needs_ref
+def _assert_same_layout(mine, ref, where):
+    """Same nesting, keys, tensor shapes / dtypes and scalar metadata; tensor values equal to fp32 rounding."""
+    if isinstance(ref, dict):
+        assert isinstance(mine, dict) and set(mine) == set(ref), f"{where}: {sorted(map(str, set(mine) ^ set(ref)))}"
+        for k in ref:
+            _assert_same_layout(mine[k], ref[k], f"{where}.{k}")
+    elif isinstance(ref, (list, tuple)):
+        assert type(mine) is type(ref) and len(mine) == len(ref), where
+        for i, (x, y) in enumerate(zip(mine, ref)):
+            _assert_same_layout(x, y, f"{where}[{i}]")
+    elif torch.is_tensor(ref):
+        assert torch.is_tensor(mine) and mine.shape == ref.shape and mine.dtype == ref.dtype, where
+        torch.testing.assert_close(mine.float(), ref.float(), atol=1e-6, rtol=1e-5, msg=where)
+    elif isinstance(ref, (bool, int, float, str, type(None))):
+        assert mine == ref, f"{where}: {mine!r} != {ref!r}"
+    else:
+        assert type(mine).__name__ == type(ref).__name__, where
+
+
 @pytest.mark.parametrize("stage", [1, 3])
 def test_stock_zero_to_fp32_reads_our_checkpoint(tmp_path, stage):
-    """(ii) a checkpoint saved HERE is consolidated by the reference's own ``zero_to_fp32.py`` (no deepspeed_b200 import)."""
-    import subprocess
-    import sys
+    """(ii) stock DeepSpeed's own ``zero_to_fp32.py`` consolidated the checkpoint this engine saves (stored with its
+    output): a checkpoint saved now has that very layout, and the stock tool's result equals this run's parameters."""
     d = str(tmp_path)
     run_distributed(_save_worker, 2, (d, stage))
-    import shutil
-    script = os.path.join(d, "stock_zero_to_fp32.py")  # the reference copies its script next to the checkpoint too
-    shutil.copyfile(os.path.join(_REF, "deepspeed", "utils", "zero_to_fp32.py"), script)
-    out = os.path.join(d, "consolidated")
-    env = dict(os.environ, PYTHONPATH=_REF, DS_ACCELERATOR="cpu")  # the stock script imports the stock package only
-    p = subprocess.run([sys.executable, script, d, out, "--tag", "t3"], env=env, capture_output=True, text=True, timeout=600,
-                       cwd=d)
-    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
-    files = [f for f in os.listdir(out) if f.endswith(".bin") or f.endswith(".pt")]
-    assert files, os.listdir(out)
-    got = {}
-    for f in files:
-        got.update(torch.load(os.path.join(out, f), map_location="cpu", weights_only=False))
+    ref_dir = os.path.join(_GOLDEN_CKPT, f"ours_s{stage}")
+    assert open(os.path.join(d, "latest")).read().strip() == open(os.path.join(ref_dir, "latest")).read().strip()
+    ref_files = sorted(os.listdir(os.path.join(ref_dir, "t3")))
+    assert sorted(os.listdir(os.path.join(d, "t3"))) == ref_files
+    for f in ref_files:
+        mine = torch.load(os.path.join(d, "t3", f), map_location="cpu", weights_only=False)
+        ref = torch.load(os.path.join(ref_dir, "t3", f), map_location="cpu", weights_only=False)
+        _assert_same_layout(mine, ref, f)
+    got = torch.load(os.path.join(ref_dir, "consolidated", "pytorch_model.bin"), map_location="cpu", weights_only=False)
     exp = torch.load(os.path.join(d, "expect_at_save.pt"))
     assert set(exp) <= set(got)
     for n, v in exp.items():

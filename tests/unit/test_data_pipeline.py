@@ -1,3 +1,4 @@
+import os
 import numpy as np
 import pytest
 import torch
@@ -122,17 +123,14 @@ def test_random_ltd_wrapper_and_scheduler():
     assert all(".random_ltd_layer" not in k for k in save_without_random_ltd(model))
 
 
-def _load_reference_indexed_dataset():
-    import importlib.util
-    import os
-    for root in ("/root/reference/deepspeed", os.path.join(os.path.dirname(__file__), "..", "..", "baseline", "_ref", "deepspeed")):
-        f = os.path.join(root, "runtime", "data_pipeline", "data_sampling", "indexed_dataset.py")
-        if os.path.exists(f):
-            spec = importlib.util.spec_from_file_location("_ref_indexed_dataset", f)
-            mod = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mod)
-            return mod
-    return None
+# Files written by the original project's indexed_dataset.py for the three samples of the test below (int32 / uint16
+# MMIDIDX, int32 legacy TNTIDX); the interop checks compare against them byte for byte.
+_GOLDEN = os.path.join(os.path.dirname(__file__), "..", "golden", "indexed_dataset")
+
+
+def _same_bytes(prefix, golden):
+    return all(open(f"{prefix}.{ext}", "rb").read() == open(os.path.join(_GOLDEN, f"{golden}.{ext}"), "rb").read()
+               for ext in ("bin", "idx"))
 
 
 def test_indexed_dataset_formats_and_interop(tmp_path):
@@ -167,23 +165,15 @@ def test_indexed_dataset_formats_and_interop(tmp_path):
     assert I.code(np.int64) == 5 and I.code(torch.int16) == 3 and I.create_doc_idx([3, 0, 2, 0]) == [0, 2, 4]
     p, tot = I.get_pointers_with_total([2, 3, 4], 4, np.int64)
     assert p.tolist() == [0, 8, 20] and tot == 36
-    # --- cross-check both directions against the reference implementation when its source is around
-    R = _load_reference_indexed_dataset()
-    if R is None:
-        return
-    rds = R.MMapIndexedDataset(meg, skip_warmup=True)
-    assert len(rds) == 3 and all(np.array_equal(rds[i], s) for i, s in enumerate(samples))
-    assert rds.doc_idx.tolist() == ds.doc_idx.tolist()
-    theirs = str(tmp_path / "theirs")
-    rb = R.MMapIndexedDatasetBuilder(R.data_file_path(theirs), dtype=np.int32)
-    for s in samples:
-        rb.add_item(torch.from_numpy(s))
-        rb.end_document()
-    rb.finalize(R.index_file_path(theirs))
+    # --- interop with the original implementation, both directions: it writes exactly these bytes for the same
+    # samples (so it reads ours as its own), and we read what it wrote
+    assert _same_bytes(meg, "ref_mmap_u16") and _same_bytes(pre, "ref_legacy_i32")
+    theirs = os.path.join(_GOLDEN, "ref_mmap_i32")
     mine = I.MMapIndexedDataset(theirs)
     assert mine.dtype == np.int32 and all(np.array_equal(mine[i], s) for i, s in enumerate(samples))
-    rl = R.IndexedDataset(pre)
-    assert all(np.array_equal(rl[i], s) for i, s in enumerate(samples))
+    assert mine.doc_idx.tolist() == ds.doc_idx.tolist()
+    legacy = I.make_dataset(os.path.join(_GOLDEN, "ref_legacy_i32"), "lazy")
+    assert all(np.array_equal(legacy[i], s) for i, s in enumerate(samples))
 
 
 def _dist_helpers():
