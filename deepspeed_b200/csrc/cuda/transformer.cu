@@ -583,12 +583,13 @@ bias_act_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ x, const T* 
 // ------------------------------------------------------------------------------------------------
 // Fused softmax cross-entropy.  One block per row.  Pass 1: online max / sum-exp.  Pass 2 (second
 // read hits L2): loss and, if dlogits != null, gradient (softmax - onehot) * gscale written to
-// dlogits (may alias logits for in-place).  Rows whose label == ignore_index give loss 0 / grad 0.
+// dlogits (may alias logits for in-place).  Rows whose label is ignore_index or outside [0, vocab) give
+// loss 0 / grad 0.
 // ------------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(1024)
-softmax_xent_kernel(const T* __restrict__ logits, const int64_t* __restrict__ labels, float* __restrict__ loss,
-                    float* __restrict__ lse_out, T* __restrict__ dlogits, int vocab, int64_t row_stride,
+softmax_xent_kernel(const T* logits, const int64_t* __restrict__ labels, float* __restrict__ loss,
+                    float* __restrict__ lse_out, T* dlogits, int vocab, int64_t row_stride,
                     int64_t ignore_index, float gscale, const float* __restrict__ d_gscale)
 {
     __shared__ float scratch[64];
@@ -596,6 +597,10 @@ softmax_xent_kernel(const T* __restrict__ logits, const int64_t* __restrict__ la
     const int64_t row = blockIdx.x;
     const T* lr = logits + row * row_stride;
     const int64_t label = labels[row];
+    const bool ignored = (label == ignore_index) || label < 0 || label >= vocab;
+    // read the label's logit before the block reductions: their barriers order it ahead of the in-place gradient
+    // stores, which other warps start as soon as the last reduction returns
+    const float x_label = (threadIdx.x == 0 && !ignored) ? Elem<T>::to_f(lr[label]) : 0.f;
     const int nvec = vocab / kPer;
     const bool aligned = (row_stride % kPer) == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0;
     float mx = -INFINITY, sum = 0.f;
@@ -632,9 +637,8 @@ softmax_xent_kernel(const T* __restrict__ logits, const int64_t* __restrict__ la
     const float part = (mx == -INFINITY) ? 0.f : sum * __expf(mx - gmx);
     const float gsum = block_reduce<SumOp>(part, scratch);
     const float lse = gmx + __logf(gsum);
-    const bool ignored = (label == ignore_index) || label < 0 || label >= vocab;
     if (threadIdx.x == 0) {
-        loss[row] = ignored ? 0.f : (lse - Elem<T>::to_f(lr[label]));
+        loss[row] = ignored ? 0.f : (lse - x_label);
         if (lse_out) lse_out[row] = lse;
     }
     if (dlogits == nullptr) return;
@@ -770,6 +774,14 @@ DSB_EXPORT int dsb_norm_bwd_grid(int rows)
     return rows < cap ? rows : cap;
 }
 
+// Which kernel dsb_norm_bwd launches: 1 the bulk-async RMSNorm kernel, 0 the register-cached kernel.  `aligned`: dy, x,
+// dres (when given) and dx all start on 16-byte boundaries.
+DSB_EXPORT int dsb_norm_bwd_path(int rows, int hidden, int kind, int dtype, int aligned)
+{
+    return kind == 0 && dtype == kBF16 && hidden % 1024 == 0 && hidden <= 8192 && rows >= 1024 && aligned &&
+           !dsb_norm_bwd_bulk_disabled();
+}
+
 // dw_part/db_part: fp32 scratch [dsb_norm_bwd_grid(rows), hidden].  dw/db: outputs in `wdtype`.
 DSB_EXPORT int dsb_norm_bwd(const void* dy, const void* x, const void* w, const float* mean, const float* rstd,
                             const void* dres, void* dx, float* dw_part, float* db_part, void* dw, void* db,
@@ -782,9 +794,9 @@ DSB_EXPORT int dsb_norm_bwd(const void* dy, const void* x, const void* w, const 
     const int threads = norm_threads(hidden, per);
     if (threads > 512) return -2;
     int grid = dsb_norm_bwd_grid(rows);
-    const bool bulk = kind == 0 && dtype == kBF16 && hidden % 1024 == 0 && hidden <= 8192 && rows >= 1024 &&
-                      ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dres) |
-                        reinterpret_cast<uintptr_t>(dx)) & 15) == 0 && !dsb_norm_bwd_bulk_disabled();
+    const bool aligned = ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dres) |
+                           reinterpret_cast<uintptr_t>(dx)) & 15) == 0;
+    const bool bulk = dsb_norm_bwd_path(rows, hidden, kind, dtype, aligned) == 1;
     if (bulk) {
         // 2 CTAs per SM: 4 stages x 3 rows each
         const int vpt = hidden / 1024;

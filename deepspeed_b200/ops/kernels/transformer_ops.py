@@ -62,6 +62,12 @@ def _norm_bwd_native(dy2, x2, w, mean, rstd, dres2, kind, need_db):
     return dx, dw, db
 
 
+def norm_bwd_path(rows, hidden, kind, dtype, aligned=True) -> str:
+    """``"bulk"`` or ``"register"``: the kernel the CUDA norm backward runs for this problem (``kind`` 0 RMSNorm,
+    1 LayerNorm; ``aligned``: dy, x, dres and dx start on 16-byte boundaries)."""
+    return "bulk" if N.cuda().dsb_norm_bwd_path(rows, hidden, kind, N.dt(dtype), int(aligned)) == 1 else "register"
+
+
 class _NormFn(torch.autograd.Function):
     """y = norm(x (+ residual)); returns (y, x+residual) when a residual is given."""
 
@@ -358,10 +364,17 @@ def bias_residual(x, bias, residual):
 # ---------------------------------------------------------------------------------------------------
 # softmax cross entropy
 # ---------------------------------------------------------------------------------------------------
+def xent_valid(labels, vocab, ignore_index=-100):
+    """Rows that contribute to the loss: the label is in ``[0, vocab)`` and is not ``ignore_index``.  Every other row
+    (including a label out of range) is ignored like ``ignore_index``: zero loss, zero gradient, not counted in a mean."""
+    return (labels != ignore_index) & (labels >= 0) & (labels < vocab)
+
+
 def softmax_xent_fwd_bwd(logits, labels, gscale=1.0, d_gscale=None, ignore_index=-100, inplace_grad=True):
     """Per-row loss (fp32) and, written **in place over ``logits``** when ``inplace_grad``, the gradient
-    ``(softmax - onehot) * gscale``.  Returns ``(loss_rows, grad_or_None)``.  Not an autograd function:
-    callers (``chunked_linear_xent``) wire the gradient manually."""
+    ``(softmax - onehot) * gscale``.  Rows that :func:`xent_valid` rejects get loss 0 and gradient 0.
+    Returns ``(loss_rows, grad_or_None)``.  Not an autograd function: callers (``chunked_linear_xent``) wire the
+    gradient manually."""
     rows, vocab = logits.shape
     loss = torch.empty(rows, dtype=torch.float32, device=logits.device)
     if logits.is_cuda:
@@ -373,8 +386,8 @@ def softmax_xent_fwd_bwd(logits, labels, gscale=1.0, d_gscale=None, ignore_index
         return loss, grad
     lf = logits.float()
     lse = torch.logsumexp(lf, dim=-1)
-    valid = (labels != ignore_index)
-    safe = labels.clamp(min=0)
+    valid = xent_valid(labels, vocab, ignore_index)
+    safe = torch.where(valid, labels, 0)
     loss = torch.where(valid, lse - lf.gather(1, safe[:, None]).squeeze(1), torch.zeros_like(lse))
     grad = None
     if inplace_grad:
@@ -395,7 +408,7 @@ class _XentFn(torch.autograd.Function):
         work = l2.clone()  # gradient is produced in place on the clone
         lab = labels.reshape(-1).contiguous()
         loss, grad = softmax_xent_fwd_bwd(work, lab, 1.0, None, ignore_index, True)
-        n = (lab != ignore_index).sum().clamp(min=1)
+        n = xent_valid(lab, l2.shape[-1], ignore_index).sum().clamp(min=1)
         ctx.save_for_backward(grad, n)
         ctx.shape = logits.shape
         return loss.sum() / n

@@ -12,7 +12,7 @@
 import torch
 import torch.nn.functional as F
 
-from deepspeed_b200.ops.kernels.transformer_ops import softmax_xent_fwd_bwd
+from deepspeed_b200.ops.kernels.transformer_ops import softmax_xent_fwd_bwd, xent_valid
 
 
 def _zo_of(w):
@@ -214,8 +214,7 @@ class _ChunkedLinearXent(torch.autograd.Function):
     def forward(ctx, h, weight, labels, chunk, ignore_index, assumed_scale):
         from deepspeed_b200.ops import gemm
         T, H = h.shape
-        valid = (labels != ignore_index)
-        n_valid = valid.sum().clamp(min=1).to(torch.float32)
+        n_valid = xent_valid(labels, weight.shape[0], ignore_index).sum().clamp(min=1).to(torch.float32)
         inv_n = (assumed_scale / n_valid).reshape(1)  # device scalar: no host sync
         need_dh = h.requires_grad
         need_dw = weight.requires_grad
@@ -289,7 +288,7 @@ def chunked_linear_xent(h, weight, labels, chunk=2048, ignore_index=-100, assume
     """Mean cross entropy of ``softmax(h W^T)`` vs ``labels`` without materialising the logits."""
     if not torch.is_grad_enabled():
         total = torch.zeros((), dtype=torch.float32, device=h.device)
-        n = (labels != ignore_index).sum().clamp(min=1)
+        n = xent_valid(labels, weight.shape[0], ignore_index).sum().clamp(min=1)
         for s in range(0, h.shape[0], chunk):
             e = min(s + chunk, h.shape[0])
             logits = _gemm(h[s:e], weight)
