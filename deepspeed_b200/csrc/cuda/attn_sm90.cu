@@ -89,12 +89,31 @@ __device__ __forceinline__ void store_acc(const float* acc, __nv_bfloat16* base,
 
 struct FwdParams {
     __nv_bfloat16* o;   // [B*S, ld_o], head h at columns [h*D, (h+1)*D)
-    float* lse;         // [B, Hq, S] natural-log sum-exp of the scaled scores
+    float* lse;         // [B, Hq, S] natural-log sum-exp of the scaled scores (varlen: [Hq, T] by absolute token row)
     int ld_o;
     int S, Hq, Hkv;
     float scale_log2;   // softmax scale * log2(e)
     int causal;
+    const int* cu;      // varlen only: document offsets [n_docs + 1] into the T token rows
+    int T;              // varlen only: token rows
 };
+
+// Packed sequences (varlen): blockIdx.z is a document, not a batch row.  Returns false for a CTA with nothing to do -- its
+// first row is past the document's end, or the offsets are malformed -- so the whole CTA exits before any barrier exists.
+template <bool kVarlen>
+__device__ __forceinline__ bool doc_rows(const int* cu, int T, int S, int b, int first, int& row_base, int& len)
+{
+    if constexpr (kVarlen) {
+        const int start = cu[b], end = cu[b + 1];
+        if (start < 0 || start > end || end > T || first >= end - start) return false;
+        row_base = start;
+        len = end - start;
+    } else {
+        row_base = b * S;
+        len = S;
+    }
+    return true;
+}
 
 namespace kf {  // forward shared-memory plan
 constexpr int KV_STAGES = 3;
@@ -104,11 +123,16 @@ constexpr uint32_t SM_BAR = SM_KV + KV_STAGES * 2 * TILE;
 constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
 }  // namespace kf
 
+template <bool kVarlen>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const FwdParams p)
 {
     using namespace kf;
+    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
+    int row_base, len;  // first token row and length of this sequence
+    if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, q0, row_base, len)) return;
+
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const uint32_t sbase = smem_u32(smem);
@@ -116,10 +140,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     auto kv_full = [&](int s) { return sbase + SM_BAR + 8 * (1 + s); };
     auto kv_empty = [&](int s) { return sbase + SM_BAR + 8 * (1 + KV_STAGES + s); };
 
-    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
     const int kvh = h / (p.Hq / p.Hkv);
-    const int row_base = b * p.S;
-    const int n_blocks = (p.S + BS - 1) / BS;
+    const int n_blocks = (len + BS - 1) / BS;
     const int n_kv = p.causal ? min(n_blocks, (q0 + BQ) / BS) : n_blocks;
 
     if (threadIdx.x == kProducer) {
@@ -185,7 +207,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                         const int key = j * BS + 8 * jj + c_in + e;
                         const int row = qr0 + r_loc + 8 * i;
                         float x = sc[4 * jj + 2 * i + e] * p.scale_log2;
-                        if (key >= p.S || (p.causal && key > row)) x = kNegInf;
+                        if (key >= len || (p.causal && key > row)) x = kNegInf;
                         sc[4 * jj + 2 * i + e] = x;
                         mx[i] = fmaxf(mx[i], x);
                     }
@@ -234,15 +256,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         l_run[i] = quad_sum(l_run[i]);
         inv[i] = l_run[i] > 0.f ? 1.f / l_run[i] : 0.f;
     }
-    const int rows = p.S - qr0;  // rows of this warpgroup inside the sequence
+    const int rows = len - qr0;  // rows of this warpgroup inside the sequence
     store_acc(o, p.o + static_cast<int64_t>(row_base + qr0) * p.ld_o, p.ld_o, r_loc, rows < BS ? rows : BS, h * D, c_in,
               inv[0], inv[1]);
     if (p.lse != nullptr && (lane & 3) == 0) {
+        float* lse = kVarlen ? p.lse + static_cast<int64_t>(h) * p.T + row_base
+                             : p.lse + (static_cast<int64_t>(b) * p.Hq + h) * p.S;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const int row = qr0 + r_loc + 8 * i;
-            if (row < p.S)
-                p.lse[(static_cast<int64_t>(b) * p.Hq + h) * p.S + row] = (m_run[i] + log2f(l_run[i])) * 0.6931471805599453f;
+            if (row < len) lse[row] = (m_run[i] + log2f(l_run[i])) * 0.6931471805599453f;
         }
     }
 }
@@ -261,14 +284,24 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 struct BwdParams {
     __nv_bfloat16 *dq, *dk, *dv;  // outputs, 2-D [B*S, ld]: head h at columns [h*D, +D)
     int ld_dq, ld_dk, ld_dv;
-    const float* lse2;   // [B, Hq, S]  log-sum-exp * log2(e)
-    const float* delta;  // [B, Hq, S]  rowsum(dO * O)
+    const float* lse2;   // [B, Hq, S]  log-sum-exp * log2(e)       (varlen: [Hq, T])
+    const float* delta;  // [B, Hq, S]  rowsum(dO * O)              (varlen: [Hq, T])
     int S, Hq, Hkv;
     float scale, scale_log2;
     int causal;
+    const int* cu;       // varlen only, as in FwdParams
+    int T;
 };
 
-// delta[b,h,s] = sum_d dO * O ; lse2 = lse * log2(e).  One warp per (token, head) row of 128 elements.
+// Per-row statistics (lse2 / delta) of query head h of this sequence, indexed by the row inside the sequence.
+template <bool kVarlen>
+__device__ __forceinline__ int64_t stat_base(const BwdParams& p, int b, int h, int row_base)
+{
+    return kVarlen ? static_cast<int64_t>(h) * p.T + row_base : (static_cast<int64_t>(b) * p.Hq + h) * p.S;
+}
+
+// delta[b,h,s] = sum_d dO * O ; lse2 = lse * log2(e).  One warp per (token, head) row of 128 elements.  The varlen
+// [Hq, T] layout is this kernel's B = 1, S = T.
 __global__ void __launch_bounds__(256)
 attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o, const float* __restrict__ lse,
                      float* __restrict__ delta, float* __restrict__ lse2, int B, int S, int Hq, int ld_o, int ld_do)
@@ -308,6 +341,9 @@ constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
 // ---- (A) dK, dV ---------------------------------------------------------------------------------------------------------------
 // dK and dV both live in registers (128 fp32 per thread), so at the 168 registers a 288-thread CTA can launch with the
 // compiler spills a little and serialises the wgmma issue of this kernel.
+// Varlen: the query blocks cover ceil(len / 64) blocks; queries past `len` (the next document's rows, or TMA zero fill) get
+// P = 0 and dS = 0 explicitly -- the causal mask does not remove them.  Key rows past `len` are computed and never stored.
+template <bool kVarlen>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
@@ -322,9 +358,10 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
 
     const int k0 = blockIdx.x * BQ, kvh = blockIdx.y, b = blockIdx.z;
     const int rep = p.Hq / p.Hkv;
-    const int row_base = b * p.S;
+    int row_base, len;
+    if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, k0, row_base, len)) return;  // before any barrier exists
     const int qb0 = p.causal ? k0 / BS : 0;  // query blocks before the first key of the CTA see none of its keys
-    const int n_qb = p.S / BS;
+    const int n_qb = kVarlen ? (len + BS - 1) / BS : len / BS;
 
     if (threadIdx.x == kProducer) {
         mbar_init(res_full, 1);
@@ -370,8 +407,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
 
     int it = 0;
     for (int qh = kvh * rep; qh < (kvh + 1) * rep; ++qh) {
-        const float* lse2 = p.lse2 + (static_cast<int64_t>(b) * p.Hq + qh) * p.S;
-        const float* delta = p.delta + (static_cast<int64_t>(b) * p.Hq + qh) * p.S;
+        const float* lse2 = p.lse2 + stat_base<kVarlen>(p, b, qh, row_base);
+        const float* delta = p.delta + stat_base<kVarlen>(p, b, qh, row_base);
         for (int qb = qb0; qb < n_qb; ++qb, ++it) {
             const int s = it % STAGES;
             mbar_wait(full(s), (it / STAGES) & 1);
@@ -390,14 +427,15 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int q = qb * BS + 8 * jj + c_in + e;
-                        const float l2 = __ldg(lse2 + q), dl = __ldg(delta + q);
+                        const bool q_in = !kVarlen || q < len;
+                        const float l2 = q_in ? __ldg(lse2 + q) : 0.f, dl = q_in ? __ldg(delta + q) : 0.f;
 #pragma unroll
                         for (int i = 0; i < 2; ++i) {
                             const int key = kr0 + r_loc + 8 * i;
                             const int x = 4 * jj + 2 * i + e;
                             const float pe = (p.causal && q < key) ? 0.f : ex2(fmaf(st[x], p.scale_log2, -l2));
-                            st[x] = pe;
-                            dpt[x] = pe * (dpt[x] - dl) * p.scale;
+                            st[x] = q_in ? pe : 0.f;
+                            dpt[x] = q_in ? pe * (dpt[x] - dl) * p.scale : 0.f;
                         }
                     }
                 uint32_t pf[4][4], df[4][4];
@@ -416,16 +454,23 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         }
     }
     const int64_t r0 = row_base + kr0;
-    store_acc(dk, p.dk + r0 * p.ld_dk, p.ld_dk, r_loc, BS, kvh * D, c_in, 1.f, 1.f);
-    store_acc(dv, p.dv + r0 * p.ld_dv, p.ld_dv, r_loc, BS, kvh * D, c_in, 1.f, 1.f);
+    const int rows = kVarlen ? min(len - kr0, BS) : BS;
+    store_acc(dk, p.dk + r0 * p.ld_dk, p.ld_dk, r_loc, rows, kvh * D, c_in, 1.f, 1.f);
+    store_acc(dv, p.dv + r0 * p.ld_dv, p.ld_dv, r_loc, rows, kvh * D, c_in, 1.f, 1.f);
 }
 
 // ---- (B) dQ -------------------------------------------------------------------------------------------------------------------
+// Varlen: keys past `len` get P = 0 and dS = 0; rows past `len` read no statistics and are never stored.
+template <bool kVarlen>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                    const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
 {
     using namespace kb;
+    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
+    int row_base, len;
+    if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, q0, row_base, len)) return;
+
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const uint32_t sbase = smem_u32(smem);
@@ -433,10 +478,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     auto full = [&](int s) { return sbase + SM_BAR + 8 * (1 + s); };
     auto empty = [&](int s) { return sbase + SM_BAR + 8 * (1 + STAGES + s); };
 
-    const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
     const int kvh = h / (p.Hq / p.Hkv);
-    const int row_base = b * p.S;
-    const int n_kv = p.causal ? (q0 + BQ) / BS : p.S / BS;
+    const int n_blocks = kVarlen ? (len + BS - 1) / BS : len / BS;
+    const int n_kv = p.causal ? (kVarlen ? min(n_blocks, (q0 + BQ) / BS) : (q0 + BQ) / BS) : n_blocks;
 
     if (threadIdx.x == kProducer) {
         mbar_init(res_full, 1);
@@ -473,9 +517,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     const int r_loc = 16 * (warp & 3) + (lane >> 2);
     const int c_in = 2 * (lane & 3);
     const uint32_t sq = sbase + SM_RES + wg * TILE, sdo = sbase + SM_RES + (2 + wg) * TILE;
-    const int64_t stat = (static_cast<int64_t>(b) * p.Hq + h) * p.S + qr0 + r_loc;
-    const float l2[2] = {p.lse2[stat], p.lse2[stat + 8]};
-    const float dl[2] = {p.delta[stat], p.delta[stat + 8]};
+    const int64_t stat = stat_base<kVarlen>(p, b, h, row_base) + qr0 + r_loc;
+    const bool in0 = !kVarlen || qr0 + r_loc < len, in1 = !kVarlen || qr0 + r_loc + 8 < len;
+    const float l2[2] = {in0 ? p.lse2[stat] : 0.f, in1 ? p.lse2[stat + 8] : 0.f};
+    const float dl[2] = {in0 ? p.delta[stat] : 0.f, in1 ? p.delta[stat + 8] : 0.f};
     float dq[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) dq[i] = 0.f;
@@ -504,7 +549,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                         const int row = qr0 + r_loc + 8 * i;
                         const int x = 4 * jj + 2 * i + e;
                         const float pe = (p.causal && key > row) ? 0.f : ex2(fmaf(sc[x], p.scale_log2, -l2[i]));
-                        dp[x] = pe * (dp[x] - dl[i]) * p.scale;
+                        dp[x] = (kVarlen && key >= len) ? 0.f : pe * (dp[x] - dl[i]) * p.scale;
                     }
             uint32_t df[4][4];
             to_frags(dp, df);
@@ -517,7 +562,101 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         __syncwarp();
         if (lane == 0) mbar_arrive(empty(s));
     }
-    store_acc(dq, p.dq + static_cast<int64_t>(row_base + qr0) * p.ld_dq, p.ld_dq, r_loc, BS, h * D, c_in, 1.f, 1.f);
+    store_acc(dq, p.dq + static_cast<int64_t>(row_base + qr0) * p.ld_dq, p.ld_dq, r_loc, kVarlen ? min(len - qr0, BS) : BS,
+              h * D, c_in, 1.f, 1.f);
+}
+
+// ---- launches ------------------------------------------------------------------------------------------------------------------
+// Dense: n_seq = B sequences of S rows, T = B * S.  Varlen: n_seq = n_docs documents at offsets cu[0..n_docs], S = the longest
+// document (it sizes the grid), T = cu[n_docs].  The tensor maps cover all T rows, so a tile that runs past a document reads
+// the next document's rows (masked in the kernels) or TMA zero fill past T.
+template <bool kVarlen>
+int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu, int n_seq, int S, int T, int Hq,
+               int Hkv, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols, int v_cols, float scale, int causal,
+               cudaStream_t stream)
+{
+    CUtensorMap mq, mk, mv;
+    int rc;
+    const uint64_t rows = static_cast<uint64_t>(T);
+    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
+    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
+    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e =
+            cudaFuncSetAttribute(attn_fwd_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize, kf::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    FwdParams p;
+    p.o = static_cast<__nv_bfloat16*>(o);
+    p.lse = lse;
+    p.ld_o = ld_o;
+    p.S = S;
+    p.Hq = Hq;
+    p.Hkv = Hkv;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.causal = causal;
+    p.cu = cu;
+    p.T = T;
+    dim3 grid((S + BQ - 1) / BQ, Hq, n_seq);
+    attn_fwd_kernel<kVarlen><<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+template <bool kVarlen>
+int launch_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse, void* dq,
+               void* dk, void* dv, float* work, const int* cu, int n_seq, int S, int T, int Hq, int Hkv, int ld_q, int ld_k,
+               int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols, int k_cols, int v_cols, float scale,
+               int causal, cudaStream_t stream)
+{
+    CUtensorMap mq, mk, mv, mdo;
+    int rc;
+    const uint64_t rows = static_cast<uint64_t>(T);
+    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
+    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
+    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
+    if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * D, ld_do, BS))) return rc;
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             kb::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        e = cudaFuncSetAttribute(attn_bwd_dq_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    float* delta = work;
+    float* lse2 = work + static_cast<int64_t>(T) * Hq;
+    const int64_t prep_rows = static_cast<int64_t>(T) * Hq;
+    // the varlen [Hq, T] statistics are the dense [B, Hq, S] layout with B = 1, S = T
+    const int prep_b = kVarlen ? 1 : n_seq, prep_s = kVarlen ? T : S;
+    attn_bwd_prep_kernel<<<static_cast<unsigned>((prep_rows * 32 + 255) / 256), 256, 0, stream>>>(
+        static_cast<const __nv_bfloat16*>(o), static_cast<const __nv_bfloat16*>(d_o), lse, delta, lse2, prep_b, prep_s, Hq,
+        ld_o, ld_do);
+    BwdParams p;
+    p.dq = static_cast<__nv_bfloat16*>(dq);
+    p.dk = static_cast<__nv_bfloat16*>(dk);
+    p.dv = static_cast<__nv_bfloat16*>(dv);
+    p.ld_dq = ld_dq;
+    p.ld_dk = ld_dk;
+    p.ld_dv = ld_dv;
+    p.lse2 = lse2;
+    p.delta = delta;
+    p.S = S;
+    p.Hq = Hq;
+    p.Hkv = Hkv;
+    p.scale = scale;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    p.causal = causal;
+    p.cu = cu;
+    p.T = T;
+    const int nx = (S + BQ - 1) / BQ;
+    attn_bwd_dkdv_kernel<kVarlen><<<dim3(nx, Hkv, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    attn_bwd_dq_kernel<kVarlen><<<dim3(nx, Hq, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    DSB_CHECK_LAUNCH();
+    return 0;
 }
 
 }  // namespace attn
@@ -536,31 +675,8 @@ DSB_EXPORT int dsb_attn_fwd_bf16(const void* q, const void* k, const void* v, vo
     if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
          reinterpret_cast<uintptr_t>(o)) & 15)
         return -2;
-    CUtensorMap mq, mk, mv;
-    int rc;
-    const uint64_t rows = static_cast<uint64_t>(B) * S;
-    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
-    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
-    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kf::SM_TOTAL);
-        if (e != cudaSuccess) return static_cast<int>(e);
-        attr = true;
-    }
-    FwdParams p;
-    p.o = static_cast<__nv_bfloat16*>(o);
-    p.lse = lse;
-    p.ld_o = ld_o;
-    p.S = S;
-    p.Hq = Hq;
-    p.Hkv = Hkv;
-    p.scale_log2 = scale * 1.4426950408889634f;
-    p.causal = causal;
-    dim3 grid((S + BQ - 1) / BQ, Hq, B);
-    attn_fwd_kernel<<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
-    DSB_CHECK_LAUNCH();
-    return 0;
+    return launch_fwd<false>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols, v_cols,
+                             scale, causal, stream);
 }
 
 // Backward.  q/k/v as in the forward; o, d_o: [B*S, ld] with head h at h*128; lse from the forward.
@@ -571,43 +687,39 @@ DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, co
                                  int k_cols, int v_cols, float scale, int causal, cudaStream_t stream)
 {
     if (head_dim != D || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
-    CUtensorMap mq, mk, mv, mdo;
-    int rc;
-    const uint64_t rows = static_cast<uint64_t>(B) * S;
-    if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
-    if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
-    if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
-    if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * D, ld_do, BS))) return rc;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
-        if (e != cudaSuccess) return static_cast<int>(e);
-        e = cudaFuncSetAttribute(attn_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
-        if (e != cudaSuccess) return static_cast<int>(e);
-        attr = true;
-    }
-    float* delta = work;
-    float* lse2 = work + static_cast<int64_t>(B) * Hq * S;
-    const int64_t prep_rows = static_cast<int64_t>(B) * S * Hq;
-    attn_bwd_prep_kernel<<<static_cast<unsigned>((prep_rows * 32 + 255) / 256), 256, 0, stream>>>(
-        static_cast<const __nv_bfloat16*>(o), static_cast<const __nv_bfloat16*>(d_o), lse, delta, lse2, B, S, Hq, ld_o, ld_do);
-    BwdParams p;
-    p.dq = static_cast<__nv_bfloat16*>(dq);
-    p.dk = static_cast<__nv_bfloat16*>(dk);
-    p.dv = static_cast<__nv_bfloat16*>(dv);
-    p.ld_dq = ld_dq;
-    p.ld_dk = ld_dk;
-    p.ld_dv = ld_dv;
-    p.lse2 = lse2;
-    p.delta = delta;
-    p.S = S;
-    p.Hq = Hq;
-    p.Hkv = Hkv;
-    p.scale = scale;
-    p.scale_log2 = scale * 1.4426950408889634f;
-    p.causal = causal;
-    attn_bwd_dkdv_kernel<<<dim3(S / BQ, Hkv, B), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
-    attn_bwd_dq_kernel<<<dim3(S / BQ, Hq, B), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
-    DSB_CHECK_LAUNCH();
-    return 0;
+    return launch_bwd<false>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o,
+                             ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, stream);
+}
+
+// Packed sequences (document-masked attention).  q / k / v / o as in dsb_attn_fwd_bf16 over T = cu_seqlens[n_docs] token
+// rows; cu_seqlens: int32 device array of n_docs + 1 non-decreasing offsets from 0 to T (empty documents allowed);
+// max_seqlen: the longest document (or more).  Each token attends only within its document.  lse: fp32 [Hq, T] or null.
+DSB_EXPORT int dsb_attn_varlen_fwd_bf16(const void* q, const void* k, const void* v, void* o, float* lse,
+                                        const int* cu_seqlens, int n_docs, int max_seqlen, int T, int Hq, int Hkv,
+                                        int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
+                                        int v_cols, float scale, int causal, cudaStream_t stream)
+{
+    if (head_dim != D || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
+    if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
+    if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+         reinterpret_cast<uintptr_t>(o)) & 15)
+        return -2;
+    if (T == 0 || n_docs == 0) return 0;
+    return launch_fwd<true>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols,
+                            k_cols, v_cols, scale, causal, stream);
+}
+
+// Backward of dsb_attn_varlen_fwd_bf16 (same cu_seqlens / max_seqlen; lse [Hq, T] from it).  dq / dk / dv may be column
+// ranges of one packed buffer.  work: fp32 scratch of 2 * Hq * T elements.
+DSB_EXPORT int dsb_attn_varlen_bwd_bf16(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+                                        const float* lse, void* dq, void* dk, void* dv, float* work, const int* cu_seqlens,
+                                        int n_docs, int max_seqlen, int T, int Hq, int Hkv, int head_dim, int ld_q, int ld_k,
+                                        int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
+                                        int k_cols, int v_cols, float scale, int causal, cudaStream_t stream)
+{
+    if (head_dim != D || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
+    if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
+    if (T == 0 || n_docs == 0) return 0;
+    return launch_bwd<true>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k,
+                            ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, stream);
 }

@@ -24,7 +24,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from deepspeed_b200.ops.kernels import transformer_ops as T
-from deepspeed_b200.ops.attention import causal_attention
+from deepspeed_b200.ops.attention import causal_attention, check_cu_seqlens, document_positions
 from deepspeed_b200.ops.linear import flat_linear
 
 
@@ -150,12 +150,13 @@ class LlamaAttention(nn.Module):
         self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias)
         self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False)
 
-    def forward(self, x, rope, positions=None):
+    def forward(self, x, rope, positions=None, cu_seqlens=None, max_seqlen=None):
         cfg = self.cfg
         B, S, _ = x.shape
         qkv = self.qkv_proj(x)  # [B, S, (hq + 2 hkv) d]
         out = causal_attention(qkv.view(B * S, -1), B, S, cfg.num_attention_heads, cfg.num_key_value_heads,
-                               cfg.head_dim, rope, positions, backend=cfg.attention_backend)
+                               cfg.head_dim, rope, positions, backend=cfg.attention_backend, cu_seqlens=cu_seqlens,
+                               max_seqlen=max_seqlen)
         return self.o_proj(out.view(B, S, cfg.q_size))
 
 
@@ -186,13 +187,13 @@ class LlamaDecoderLayer(nn.Module):
         self.post_attention_layernorm = RMSNorm(cfg.hidden_size, cfg.rms_norm_eps)
         self.mlp = LlamaMLP(cfg)
 
-    def forward(self, delta, residual, rope, positions=None):
+    def forward(self, delta, residual, rope, positions=None, cu_seqlens=None, max_seqlen=None):
         if residual is None:
             residual = delta
             h = self.input_layernorm(delta)
         else:
             h, residual = self.input_layernorm(delta, residual)
-        attn = self.self_attn(h, rope, positions)
+        attn = self.self_attn(h, rope, positions, cu_seqlens, max_seqlen)
         h, residual = self.post_attention_layernorm(attn, residual)
         return self.mlp(h), residual
 
@@ -214,24 +215,52 @@ class LlamaModel(nn.Module):
                                        self.cfg.rope_scaling)
         return self._rope
 
-    def forward(self, input_ids, positions=None):
+    def forward(self, input_ids, positions=None, cu_seqlens=None, max_seqlen=None):
+        """``cu_seqlens`` / ``max_seqlen``: packed documents, see :meth:`LlamaForCausalLM.forward`."""
         cfg = self.cfg
         h = self.embed_tokens(input_ids)
         rope = self.rope_table(h.device)
+        if cu_seqlens is not None:
+            cu_seqlens, max_seqlen = prepare_packed(cu_seqlens, max_seqlen, input_ids.shape, h.device)
+            if positions is None:
+                positions = document_positions(cu_seqlens, input_ids.numel())
         delta, residual = h, None
         for i, layer in enumerate(self.layers):
             if self.training and i < cfg.checkpoint_layers and torch.is_grad_enabled():
                 from deepspeed_b200.runtime.activation_checkpointing import checkpointing as ckpt
-                delta, residual = ckpt.checkpoint(layer, delta, residual, rope, positions)
+                delta, residual = ckpt.checkpoint(layer, delta, residual, rope, positions, cu_seqlens, max_seqlen)
             else:
-                delta, residual = layer(delta, residual, rope, positions)
+                delta, residual = layer(delta, residual, rope, positions, cu_seqlens, max_seqlen)
         h, _ = self.norm(delta, residual)
         return h
 
 
+def prepare_packed(cu_seqlens, max_seqlen, shape, device):
+    """Check packed-document offsets for a ``[B, S]`` batch and return ``(cu_seqlens on device, max_seqlen)``.  A CPU
+    tensor is checked in full (including that every row start ``b*S`` is a document boundary) and gives ``max_seqlen``;
+    a device tensor is trusted and needs ``max_seqlen``."""
+    B, S = shape
+    max_seqlen = check_cu_seqlens(cu_seqlens, B * S, max_seqlen)
+    if cu_seqlens.device.type == "cpu":
+        row_starts = torch.arange(B, dtype=torch.int32) * S
+        if not bool(torch.isin(row_starts, cu_seqlens).all()):
+            raise ValueError("every row start b*S must be a document boundary in cu_seqlens (documents may not cross rows)")
+        cu_seqlens = cu_seqlens.to(device)
+    return cu_seqlens, max_seqlen
+
+
 class LlamaForCausalLM(nn.Module):
     """``forward(input_ids, labels=None)`` -> loss (if labels) or logits.  Labels are next-token
-    targets aligned with ``input_ids`` (shifted inside, HF convention) unless ``shift_labels=False``."""
+    targets aligned with ``input_ids`` (shifted inside, HF convention) unless ``shift_labels=False``.
+
+    Packed sequences: ``cu_seqlens`` (int32 ``[n_docs + 1]``) gives document offsets into the flattened
+    ``input_ids.view(-1)``; each token then attends only within its document.  Documents may not cross rows: every row
+    start ``b*S`` must be an offset.  A CPU ``cu_seqlens`` (the usual data-loader output) is validated, ``max_seqlen`` is
+    derived from it and it is copied to the device once per forward; a device ``cu_seqlens`` needs ``max_seqlen`` and keeps
+    the step free of host syncs.  ``positions`` defaults to the position inside each document (0 at its first token).
+    With ``shift_labels=True`` the last token of every document gets target -100, so no token learns to predict the
+    next document's first token (ignored targets do not count in the mean).
+"""
 
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
@@ -252,12 +281,19 @@ class LlamaForCausalLM(nn.Module):
             if m.weight.numel():
                 nn.init.normal_(m.weight, mean=0.0, std=std)
 
-    def forward(self, input_ids, labels=None, positions=None, shift_labels=True):
-        h = self.model(input_ids, positions)
+    def forward(self, input_ids, labels=None, positions=None, shift_labels=True, cu_seqlens=None, max_seqlen=None):
+        if cu_seqlens is not None:
+            cu_seqlens, max_seqlen = prepare_packed(cu_seqlens, max_seqlen, input_ids.shape, input_ids.device)
+        h = self.model(input_ids, positions, cu_seqlens, max_seqlen)
         if labels is None:
             return self.lm_head(h)
         if shift_labels:
             labels = torch.cat([labels[:, 1:], torch.full_like(labels[:, :1], -100)], dim=1)
+            if cu_seqlens is not None and labels.numel():
+                # each document's last token: (end - 1) mod T also covers empty documents (their "last token" is the
+                # previous document's, or with end 0 the batch's final token -- both already document ends)
+                ends = (cu_seqlens[1:].long() - 1).remainder(labels.numel())
+                labels = labels.reshape(-1).index_fill(0, ends, -100).view_as(labels)
         return self.lm_head(h, labels=labels, chunk=self.cfg.loss_chunk_tokens, assumed_scale=self.ds_loss_multiplier)
 
     # ---- HF checkpoint interop ---------------------------------------------------------------------

@@ -10,6 +10,9 @@ Attention-core backends (``backend=`` or ``DSB200_ATTN``):
   * ``flash_attn`` -- the flash-attn package;
   * ``native`` -- the framework's own sm_90a kernel (``csrc/cuda/attn_sm90.cu``) when built;
   * ``auto`` -- native if available, else cudnn -> flash -> efficient -> math priority order.
+Packed sequences (``cu_seqlens=``): the ``B*S`` token rows hold several documents at offsets ``cu_seqlens`` and every token
+attends only within its own document (flash-attn's varlen semantics).  ``auto`` / ``native`` run the in-tree varlen
+kernel; any other backend, dtype, head dim or a CPU tensor runs one SDPA call per document.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
 """
@@ -107,8 +110,141 @@ def _native_wins(B, S, hq, hkv, d) -> bool:
     return bool(e and e.get("choice") == "native")
 
 
-def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend="auto"):
+def document_positions(cu_seqlens, T):
+    """int32 ``[T]`` position of every token inside its document (0 at each document start), built on ``cu_seqlens``'
+    device without a host sync."""
+    starts = cu_seqlens[:-1].long()
+    lens = cu_seqlens[1:].long() - starts
+    first = torch.repeat_interleave(starts, lens, output_size=T)
+    return (torch.arange(T, device=cu_seqlens.device) - first).to(torch.int32)
+
+
+def check_cu_seqlens(cu_seqlens, T, max_seqlen=None):
+    """Validate document offsets into ``T`` token rows and return ``max_seqlen``.  A CPU tensor (the usual data-loader
+    output) is checked in full: 1-D int32, starts at 0, ends at ``T``, non-decreasing; ``max_seqlen`` is derived from it
+    when not given.  A device tensor is only checked for shape and dtype (no host sync) and needs ``max_seqlen``."""
+    if not isinstance(cu_seqlens, torch.Tensor) or cu_seqlens.dim() != 1 or cu_seqlens.numel() < 1:
+        raise ValueError("cu_seqlens must be a 1-D tensor of n_docs + 1 offsets")
+    if cu_seqlens.dtype != torch.int32:
+        raise ValueError(f"cu_seqlens must be int32, got {cu_seqlens.dtype}")
+    if cu_seqlens.device.type != "cpu":
+        if max_seqlen is None:
+            raise ValueError("a device cu_seqlens needs max_seqlen (deriving it would sync with the host)")
+        return int(max_seqlen)
+    if int(cu_seqlens[0]) != 0:
+        raise ValueError(f"cu_seqlens must start at 0, got {int(cu_seqlens[0])}")
+    if int(cu_seqlens[-1]) != T:
+        raise ValueError(f"cu_seqlens must end at the token count {T}, got {int(cu_seqlens[-1])}")
+    lens = cu_seqlens[1:] - cu_seqlens[:-1]
+    if bool((lens < 0).any()):
+        raise ValueError("cu_seqlens must be non-decreasing")
+    longest = int(lens.max()) if lens.numel() else 0
+    if max_seqlen is not None and int(max_seqlen) < longest:
+        raise ValueError(f"max_seqlen {int(max_seqlen)} is shorter than the longest document ({longest})")
+    return longest if max_seqlen is None else int(max_seqlen)
+
+
+def _doc_spans(cu_seqlens, T):
+    """Host ``(start, end)`` pairs of the non-empty documents (syncs once for a device tensor)."""
+    cu = cu_seqlens.tolist()
+    if cu[0] != 0 or cu[-1] != T or any(b < a for a, b in zip(cu[:-1], cu[1:])):
+        raise ValueError("cu_seqlens must be non-decreasing offsets from 0 to the token count")
+    return [(a, b) for a, b in zip(cu[:-1], cu[1:]) if b > a]
+
+
+def _split_doc(qkv, s, e, hq, hkv, d):
+    x = qkv[s:e].view(1, e - s, hq + 2 * hkv, d)
+    return x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2), x[:, :, hq + hkv:].transpose(1, 2)
+
+
+class _PackedVarlenCausalAttention(torch.autograd.Function):
+    """Packed documents through one SDPA call per document (the portable path and the reference for the varlen kernel):
+    in-place RoPE with per-token positions, packed ``dqkv`` in the backward, un-rotated in place."""
+
+    @staticmethod
+    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal):
+        T = qkv.shape[0]
+        if rope is not None:
+            rope_qk_inplace(qkv, hq, hkv, d, rope, positions, T, backward=False)
+        out = qkv.new_empty(T, hq * d)
+        graphs = []
+        for s, e in spans:
+            parts = _split_doc(qkv, s, e, hq, hkv, d)  # views taken outside grad mode, like _PackedCausalAttention
+            with torch.enable_grad():
+                qd, kd, vd = (t.detach().requires_grad_(True) for t in parts)
+                o = _sdpa(qd, kd, vd, backend, causal=causal)
+            out[s:e] = o.detach().transpose(1, 2).reshape(e - s, hq * d)
+            graphs.append((s, e, qd, kd, vd, o))
+        ctx.graphs = graphs
+        ctx.meta = (hq, hkv, d, rope, positions)
+        ctx.qkv_shape = qkv.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        hq, hkv, d, rope, positions = ctx.meta
+        graphs, ctx.graphs = ctx.graphs, None
+        T = ctx.qkv_shape[0]
+        dqkv = torch.zeros(ctx.qkv_shape, dtype=dout.dtype, device=dout.device)
+        for s, e, qd, kd, vd, o in graphs:
+            do = dout[s:e].view(1, e - s, hq, d).transpose(1, 2)
+            dq, dk, dv = torch.autograd.grad(o, (qd, kd, vd), do)
+            y = dqkv[s:e].view(1, e - s, hq + 2 * hkv, d)
+            y[:, :, :hq].copy_(dq.transpose(1, 2))
+            y[:, :, hq:hq + hkv].copy_(dk.transpose(1, 2))
+            y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
+        if rope is not None:
+            rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, T, backward=True)
+        return dqkv, None, None, None, None, None, None, None, None
+
+
+def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=None, backend="auto", causal=True):
+    """Per-document SDPA over packed documents (any device / dtype / head dim); ``positions`` as in
+    :func:`causal_attention` (defaults to :func:`document_positions`)."""
+    T = qkv2d.shape[0]
+    if rope is not None and positions is None:
+        positions = document_positions(cu_seqlens, T)
+    if positions is not None:
+        positions = positions.reshape(-1).to(device=qkv2d.device, dtype=torch.int32)
+    spans = _doc_spans(cu_seqlens, T)
+    if torch.is_grad_enabled() and qkv2d.requires_grad:
+        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal)
+    if rope is not None:
+        rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
+    out = qkv2d.new_empty(T, hq * d)
+    for s, e in spans:
+        out[s:e] = _sdpa(*_split_doc(qkv2d, s, e, hq, hkv, d), backend, causal=causal).transpose(1, 2).reshape(e - s, hq * d)
+    return out
+
+
+def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen):
+    max_seqlen = check_cu_seqlens(cu_seqlens, T, max_seqlen)
+    if backend in ("native", "auto") and qkv2d.is_cuda:
+        from deepspeed_b200.ops.kernels import attention_sm100
+        if attention_sm100.supports_varlen(qkv2d, hq, hkv, d):
+            cu = cu_seqlens.to(qkv2d.device, non_blocking=True)
+            if rope is not None:
+                positions = (document_positions(cu, T) if positions is None else positions.reshape(-1).to(
+                    device=qkv2d.device, dtype=torch.int32))
+            if torch.is_grad_enabled() and qkv2d.requires_grad:
+                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions)
+            if rope is not None:
+                rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
+            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv)
+            return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False)[0]
+    if backend == "native":
+        raise RuntimeError("native varlen attention kernel requested but unsupported for this input (needs a CUDA bf16 "
+                           "tensor, head dim 128, 16-byte aligned rows)")
+    return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend)
+
+
+def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend="auto", cu_seqlens=None, max_seqlen=None):
+    """``qkv2d [B*S, (hq + 2 hkv) * d]`` -> ``[B*S, hq*d]``.  With ``cu_seqlens`` (int32 ``[n_docs + 1]`` offsets into the
+    ``B*S`` rows, see :func:`check_cu_seqlens`) attention is masked to each document and ``positions`` defaults to
+    :func:`document_positions`; a device ``cu_seqlens`` needs ``max_seqlen``."""
     backend = _ENV or backend or "auto"
+    if cu_seqlens is not None:
+        return _varlen_causal_attention(qkv2d, B * S, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen)
     if backend == "native" or (backend == "auto" and qkv2d.is_cuda and _native_wins(B, S, hq, hkv, d)):
         from deepspeed_b200.ops.kernels import attention_sm100
         if attention_sm100.supports(qkv2d, hq, hkv, d, S):

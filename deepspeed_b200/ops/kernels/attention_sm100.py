@@ -40,6 +40,38 @@ def fwd(q, k, v, B, S, hq, hkv, causal=True, scale=None, out=None, need_lse=True
     return out, lse
 
 
+def supports_varlen(qkv2d, hq, hkv, d) -> bool:
+    """Packed sequences (:func:`fwd_varlen` / :func:`bwd_varlen`): :func:`supports` without the length rule."""
+    return (qkv2d.is_cuda and qkv2d.dtype == torch.bfloat16 and d == HEAD_DIM and hq % hkv == 0 and qkv2d.stride(-1) == 1
+            and qkv2d.stride(0) % 8 == 0 and qkv2d.data_ptr() % 16 == 0)
+
+
+def _check_cu(cu_seqlens, dev):
+    if not (cu_seqlens.dtype == torch.int32 and cu_seqlens.dim() == 1 and cu_seqlens.numel() >= 1
+            and cu_seqlens.device == dev and cu_seqlens.is_contiguous()):
+        raise ValueError("cu_seqlens must be a contiguous 1-D int32 tensor on the attention's device")
+    return cu_seqlens.numel() - 1
+
+
+def fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, out=None, need_lse=True):
+    """Document-masked attention over packed sequences: ``q [T, hq*128]``, ``k / v [T, hkv*128]`` (2-D views, any row
+    stride), ``cu_seqlens`` int32 ``[n_docs + 1]`` on the device (offsets from 0 to T, non-decreasing, empty documents
+    allowed), ``max_seqlen`` >= the longest document.  Each token attends only to tokens of its own document.
+    Returns ``(o [T, hq*128], lse [hq, T])`` -- the LSE is indexed by absolute token row."""
+    T = q.shape[0]
+    n_docs = _check_cu(cu_seqlens, q.device)
+    if out is None:
+        out = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty(hq, T, dtype=torch.float32, device=q.device) if need_lse else None
+    scale = float(scale) if scale is not None else 1.0 / math.sqrt(HEAD_DIM)
+    rc = N.cuda().dsb_attn_varlen_fwd_bf16(N.ptr(q), N.ptr(k), N.ptr(v), N.ptr(out), N.ptr(lse), N.ptr(cu_seqlens), n_docs,
+                                           int(max_seqlen), T, hq, hkv, HEAD_DIM, q.stride(0), k.stride(0), v.stride(0),
+                                           out.stride(0), q.shape[1], k.shape[1], v.shape[1], N.c_f(scale),
+                                           int(bool(causal)), N.stream())
+    N.check(rc, "attn_varlen_fwd_bf16")
+    return out, lse
+
+
 def split_packed(qkv2d, hq, hkv, d=HEAD_DIM):
     """Column views (no copies) of a packed ``[T, (hq + 2 hkv) * d]`` projection output."""
     return qkv2d[:, :hq * d], qkv2d[:, hq * d:(hq + hkv) * d], qkv2d[:, (hq + hkv) * d:]
@@ -64,6 +96,31 @@ def bwd(d_o, q, k, v, o, lse, B, S, hq, hkv, causal=True, scale=None, dq=None, d
                                     o.stride(0), d_o.stride(0), dq.stride(0), dk.stride(0), dv.stride(0), q.shape[1],
                                     k.shape[1], v.shape[1], N.c_f(scale), int(bool(causal)), N.stream())
     N.check(rc, "attn_bwd_bf16")
+    return dq, dk, dv
+
+
+def bwd_varlen(d_o, q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, dq=None, dk=None, dv=None):
+    """Gradients of :func:`fwd_varlen` (same ``cu_seqlens`` / ``max_seqlen``, ``lse [hq, T]`` from it).  ``dq / dk / dv``
+    may be column views of one packed ``[T, (hq + 2 hkv) * 128]`` buffer."""
+    T = q.shape[0]
+    dev = q.device
+    n_docs = _check_cu(cu_seqlens, dev)
+    if dq is None:
+        dq = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=dev)
+    if dk is None:
+        dk = torch.empty(T, hkv * HEAD_DIM, dtype=torch.bfloat16, device=dev)
+    if dv is None:
+        dv = torch.empty(T, hkv * HEAD_DIM, dtype=torch.bfloat16, device=dev)
+    if d_o.stride(-1) != 1:
+        d_o = d_o.contiguous()
+    work = torch.empty(2 * hq * T, dtype=torch.float32, device=dev)
+    scale = float(scale) if scale is not None else 1.0 / math.sqrt(HEAD_DIM)
+    rc = N.cuda().dsb_attn_varlen_bwd_bf16(N.ptr(q), N.ptr(k), N.ptr(v), N.ptr(o), N.ptr(d_o), N.ptr(lse), N.ptr(dq),
+                                           N.ptr(dk), N.ptr(dv), N.ptr(work), N.ptr(cu_seqlens), n_docs, int(max_seqlen), T,
+                                           hq, hkv, HEAD_DIM, q.stride(0), k.stride(0), v.stride(0), o.stride(0),
+                                           d_o.stride(0), dq.stride(0), dk.stride(0), dv.stride(0), q.shape[1], k.shape[1],
+                                           v.shape[1], N.c_f(scale), int(bool(causal)), N.stream())
+    N.check(rc, "attn_varlen_bwd_bf16")
     return dq, dk, dv
 
 
@@ -99,3 +156,40 @@ class _PackedAttention(torch.autograd.Function):
 def packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None):
     assert d == HEAD_DIM
     return _PackedAttention.apply(qkv2d, B, S, hq, hkv, rope, positions)
+
+
+class _PackedVarlenAttention(torch.autograd.Function):
+    """:class:`_PackedAttention` over packed documents: ``positions`` (int32 ``[T]``, restarting per document) drive the
+    in-place RoPE, ``cu_seqlens`` / ``max_seqlen`` the document masking."""
+
+    @staticmethod
+    def forward(ctx, qkv, cu_seqlens, max_seqlen, hq, hkv, rope, positions):
+        from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
+        T = qkv.shape[0]
+        if rope is not None:
+            rope_qk_inplace(qkv, hq, hkv, HEAD_DIM, rope, positions, T, backward=False)
+        q, k, v = split_packed(qkv, hq, hkv)
+        o, lse = fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True)
+        ctx.save_for_backward(qkv, o, lse, cu_seqlens)
+        ctx.meta = (max_seqlen, hq, hkv, rope, positions)
+        return o
+
+    @staticmethod
+    def backward(ctx, d_o):
+        from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
+        qkv, o, lse, cu_seqlens = ctx.saved_tensors
+        max_seqlen, hq, hkv, rope, positions = ctx.meta
+        T = qkv.shape[0]
+        q, k, v = split_packed(qkv, hq, hkv)
+        dqkv = torch.empty_like(qkv)
+        dq, dk, dv = split_packed(dqkv, hq, hkv)
+        bwd_varlen(d_o.reshape(T, hq * HEAD_DIM), q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, dq=dq,
+                   dk=dk, dv=dv)
+        if rope is not None:
+            rope_qk_inplace(dqkv, hq, hkv, HEAD_DIM, rope, positions, T, backward=True)
+        return dqkv, None, None, None, None, None, None
+
+
+def packed_varlen_attention(qkv2d, cu_seqlens, max_seqlen, hq, hkv, d, rope=None, positions=None):
+    assert d == HEAD_DIM
+    return _PackedVarlenAttention.apply(qkv2d, cu_seqlens, max_seqlen, hq, hkv, rope, positions)
