@@ -96,6 +96,7 @@ struct FwdParams {
     int causal;
     const int* cu;      // varlen only: document offsets [n_docs + 1] into the T token rows
     int T;              // varlen only: token rows
+    int window;         // sliding window only: row i sees keys i - window < j <= i (1 <= window <= S)
 };
 
 // Packed sequences (varlen): blockIdx.z is a document, not a batch row.  Returns false for a CTA with nothing to do -- its
@@ -115,6 +116,14 @@ __device__ __forceinline__ bool doc_rows(const int* cu, int T, int S, int b, int
     return true;
 }
 
+// Sliding window: the first 64-key block a CTA whose first query row is q0 can see.  The producer and the consumers both
+// start there and count ring stages and phases from it.
+template <bool kWindow>
+__device__ __forceinline__ int first_key_block(int q0, int window)
+{
+    return kWindow ? max(0, q0 - window + 1) / BS : 0;
+}
+
 namespace kf {  // forward shared-memory plan
 constexpr int KV_STAGES = 3;
 constexpr uint32_t SM_Q = 0;                              // 2 tiles (one per consumer warpgroup)
@@ -123,7 +132,7 @@ constexpr uint32_t SM_BAR = SM_KV + KV_STAGES * 2 * TILE;
 constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
 }  // namespace kf
 
-template <bool kVarlen>
+template <bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const FwdParams p)
@@ -143,6 +152,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     const int kvh = h / (p.Hq / p.Hkv);
     const int n_blocks = (len + BS - 1) / BS;
     const int n_kv = p.causal ? min(n_blocks, (q0 + BQ) / BS) : n_blocks;
+    const int j0 = first_key_block<kWindow>(q0, p.window);
 
     if (threadIdx.x == kProducer) {
         mbar_init(q_full, 1);
@@ -162,9 +172,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             mbar_expect_tx(q_full, 2 * TILE);
             load_tile(sbase + SM_Q, &map_q, q_full, h * D, row_base + q0);
             load_tile(sbase + SM_Q + TILE, &map_q, q_full, h * D, row_base + q0 + BS);
-            for (int j = 0; j < n_kv; ++j) {
-                const int s = j % KV_STAGES;
-                mbar_wait(kv_empty(s), ((j / KV_STAGES) & 1) ^ 1);
+            for (int j = j0; j < n_kv; ++j) {
+                const int s = (j - j0) % KV_STAGES;
+                mbar_wait(kv_empty(s), (((j - j0) / KV_STAGES) & 1) ^ 1);
                 mbar_expect_tx(kv_full(s), 2 * TILE);
                 const uint32_t dst = sbase + SM_KV + s * 2 * TILE;
                 load_tile(dst, &map_k, kv_full(s), kvh * D, row_base + j * BS);
@@ -186,10 +196,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     float m_run[2] = {kNegInf, kNegInf}, l_run[2] = {0.f, 0.f};
     mbar_wait(q_full, 0);
 
-    for (int j = 0; j < n_kv; ++j) {
-        const int s = j % KV_STAGES;
-        mbar_wait(kv_full(s), (j / KV_STAGES) & 1);
-        if (!(p.causal && j * BS > qr0 + BS - 1)) {  // a block entirely above the diagonal contributes nothing
+    for (int j = j0; j < n_kv; ++j) {
+        const int s = (j - j0) % KV_STAGES;
+        mbar_wait(kv_full(s), ((j - j0) / KV_STAGES) & 1);
+        // a block entirely above the diagonal, or entirely before the window of every row here, contributes nothing
+        if (!(p.causal && j * BS > qr0 + BS - 1) && !(kWindow && j * BS + BS - 1 < qr0 - p.window + 1)) {
             const uint32_t sk = sbase + SM_KV + s * 2 * TILE, sv = sk + TILE;
             float sc[32];
             wgmma_fence();
@@ -207,7 +218,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                         const int key = j * BS + 8 * jj + c_in + e;
                         const int row = qr0 + r_loc + 8 * i;
                         float x = sc[4 * jj + 2 * i + e] * p.scale_log2;
-                        if (key >= len || (p.causal && key > row)) x = kNegInf;
+                        if (key >= len || (p.causal && key > row) || (kWindow && key <= row - p.window)) x = kNegInf;
                         sc[4 * jj + 2 * i + e] = x;
                         mx[i] = fmaxf(mx[i], x);
                     }
@@ -291,6 +302,7 @@ struct BwdParams {
     int causal;
     const int* cu;       // varlen only, as in FwdParams
     int T;
+    int window;          // sliding window only, as in FwdParams
 };
 
 // Per-row statistics (lse2 / delta) of query head h of this sequence, indexed by the row inside the sequence.
@@ -343,7 +355,8 @@ constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
 // compiler spills a little and serialises the wgmma issue of this kernel.
 // Varlen: the query blocks cover ceil(len / 64) blocks; queries past `len` (the next document's rows, or TMA zero fill) get
 // P = 0 and dS = 0 explicitly -- the causal mask does not remove them.  Key rows past `len` are computed and never stored.
-template <bool kVarlen>
+// Sliding window: the query blocks stop after the last query that sees the CTA's last key (k0 + 127 + window - 1).
+template <bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
@@ -361,7 +374,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     int row_base, len;
     if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, k0, row_base, len)) return;  // before any barrier exists
     const int qb0 = p.causal ? k0 / BS : 0;  // query blocks before the first key of the CTA see none of its keys
-    const int n_qb = kVarlen ? (len + BS - 1) / BS : len / BS;
+    const int n_qb_all = kVarlen ? (len + BS - 1) / BS : len / BS;
+    const int n_qb = kWindow ? min(n_qb_all, (k0 + BQ - 1 + p.window - 1) / BS + 1) : n_qb_all;
 
     if (threadIdx.x == kProducer) {
         mbar_init(res_full, 1);
@@ -412,7 +426,7 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         for (int qb = qb0; qb < n_qb; ++qb, ++it) {
             const int s = it % STAGES;
             mbar_wait(full(s), (it / STAGES) & 1);
-            if (!(p.causal && qb * BS + BS - 1 < kr0)) {
+            if (!(p.causal && qb * BS + BS - 1 < kr0) && !(kWindow && qb * BS > kr0 + BS - 1 + p.window - 1)) {
                 const uint32_t sq = sbase + SM_STR + s * 2 * TILE, sdo = sq + TILE;
                 float st[32], dpt[32];
                 wgmma_fence();
@@ -433,7 +447,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                         for (int i = 0; i < 2; ++i) {
                             const int key = kr0 + r_loc + 8 * i;
                             const int x = 4 * jj + 2 * i + e;
-                            const float pe = (p.causal && q < key) ? 0.f : ex2(fmaf(st[x], p.scale_log2, -l2));
+                            const float pe = ((p.causal && q < key) || (kWindow && q - key >= p.window))
+                                                 ? 0.f
+                                                 : ex2(fmaf(st[x], p.scale_log2, -l2));
                             st[x] = q_in ? pe : 0.f;
                             dpt[x] = q_in ? pe * (dpt[x] - dl) * p.scale : 0.f;
                         }
@@ -461,7 +477,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
 
 // ---- (B) dQ -------------------------------------------------------------------------------------------------------------------
 // Varlen: keys past `len` get P = 0 and dS = 0; rows past `len` read no statistics and are never stored.
-template <bool kVarlen>
+// Sliding window: the key blocks start at the forward's first block, keys before a row's window get P = 0 and dS = 0.
+template <bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                    const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
@@ -481,6 +498,7 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     const int kvh = h / (p.Hq / p.Hkv);
     const int n_blocks = kVarlen ? (len + BS - 1) / BS : len / BS;
     const int n_kv = p.causal ? (kVarlen ? min(n_blocks, (q0 + BQ) / BS) : (q0 + BQ) / BS) : n_blocks;
+    const int j0 = first_key_block<kWindow>(q0, p.window);
 
     if (threadIdx.x == kProducer) {
         mbar_init(res_full, 1);
@@ -499,9 +517,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                 load_tile(sbase + SM_RES + w * TILE, &map_q, res_full, h * D, row_base + q0 + w * BS);
                 load_tile(sbase + SM_RES + (2 + w) * TILE, &map_do, res_full, h * D, row_base + q0 + w * BS);
             }
-            for (int j = 0; j < n_kv; ++j) {
-                const int s = j % STAGES;
-                mbar_wait(empty(s), ((j / STAGES) & 1) ^ 1);
+            for (int j = j0; j < n_kv; ++j) {
+                const int s = (j - j0) % STAGES;
+                mbar_wait(empty(s), (((j - j0) / STAGES) & 1) ^ 1);
                 mbar_expect_tx(full(s), 2 * TILE);
                 const uint32_t dst = sbase + SM_STR + s * 2 * TILE;
                 load_tile(dst, &map_k, full(s), kvh * D, row_base + j * BS);
@@ -526,10 +544,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     for (int i = 0; i < 64; ++i) dq[i] = 0.f;
     mbar_wait(res_full, 0);
 
-    for (int j = 0; j < n_kv; ++j) {
-        const int s = j % STAGES;
-        mbar_wait(full(s), (j / STAGES) & 1);
-        if (!(p.causal && j * BS > qr0 + BS - 1)) {
+    for (int j = j0; j < n_kv; ++j) {
+        const int s = (j - j0) % STAGES;
+        mbar_wait(full(s), ((j - j0) / STAGES) & 1);
+        if (!(p.causal && j * BS > qr0 + BS - 1) && !(kWindow && j * BS + BS - 1 < qr0 - p.window + 1)) {
             const uint32_t sk = sbase + SM_STR + s * 2 * TILE, sv = sk + TILE;
             float sc[32], dp[32];
             wgmma_fence();
@@ -548,7 +566,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
                         const int key = j * BS + 8 * jj + c_in + e;
                         const int row = qr0 + r_loc + 8 * i;
                         const int x = 4 * jj + 2 * i + e;
-                        const float pe = (p.causal && key > row) ? 0.f : ex2(fmaf(sc[x], p.scale_log2, -l2[i]));
+                        const float pe = ((p.causal && key > row) || (kWindow && key <= row - p.window))
+                                             ? 0.f
+                                             : ex2(fmaf(sc[x], p.scale_log2, -l2[i]));
                         dp[x] = (kVarlen && key >= len) ? 0.f : pe * (dp[x] - dl[i]) * p.scale;
                     }
             uint32_t df[4][4];
@@ -570,10 +590,10 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 // Dense: n_seq = B sequences of S rows, T = B * S.  Varlen: n_seq = n_docs documents at offsets cu[0..n_docs], S = the longest
 // document (it sizes the grid), T = cu[n_docs].  The tensor maps cover all T rows, so a tile that runs past a document reads
 // the next document's rows (masked in the kernels) or TMA zero fill past T.
-template <bool kVarlen>
+template <bool kVarlen, bool kWindow>
 int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu, int n_seq, int S, int T, int Hq,
                int Hkv, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols, int v_cols, float scale, int causal,
-               cudaStream_t stream)
+               int window, cudaStream_t stream)
 {
     CUtensorMap mq, mk, mv;
     int rc;
@@ -583,8 +603,8 @@ int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
     if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
     static bool attr = false;
     if (!attr) {
-        cudaError_t e =
-            cudaFuncSetAttribute(attn_fwd_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize, kf::SM_TOTAL);
+        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<kVarlen, kWindow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             kf::SM_TOTAL);
         if (e != cudaSuccess) return static_cast<int>(e);
         attr = true;
     }
@@ -599,17 +619,18 @@ int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
     p.causal = causal;
     p.cu = cu;
     p.T = T;
+    p.window = kWindow ? min(window, S) : 0;  // a window of S rows or more masks nothing
     dim3 grid((S + BQ - 1) / BQ, Hq, n_seq);
-    attn_fwd_kernel<kVarlen><<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
+    attn_fwd_kernel<kVarlen, kWindow><<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
     DSB_CHECK_LAUNCH();
     return 0;
 }
 
-template <bool kVarlen>
+template <bool kVarlen, bool kWindow>
 int launch_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse, void* dq,
                void* dk, void* dv, float* work, const int* cu, int n_seq, int S, int T, int Hq, int Hkv, int ld_q, int ld_k,
                int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols, int k_cols, int v_cols, float scale,
-               int causal, cudaStream_t stream)
+               int causal, int window, cudaStream_t stream)
 {
     CUtensorMap mq, mk, mv, mdo;
     int rc;
@@ -620,10 +641,11 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o, const
     if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * D, ld_do, BS))) return rc;
     static bool attr = false;
     if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             kb::SM_TOTAL);
+        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel<kVarlen, kWindow>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
         if (e != cudaSuccess) return static_cast<int>(e);
-        e = cudaFuncSetAttribute(attn_bwd_dq_kernel<kVarlen>, cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
+        e = cudaFuncSetAttribute(attn_bwd_dq_kernel<kVarlen, kWindow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kb::SM_TOTAL);
         if (e != cudaSuccess) return static_cast<int>(e);
         attr = true;
     }
@@ -652,9 +674,10 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o, const
     p.causal = causal;
     p.cu = cu;
     p.T = T;
+    p.window = kWindow ? min(window, S) : 0;  // a window of S rows or more masks nothing
     const int nx = (S + BQ - 1) / BQ;
-    attn_bwd_dkdv_kernel<kVarlen><<<dim3(nx, Hkv, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
-    attn_bwd_dq_kernel<kVarlen><<<dim3(nx, Hq, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    attn_bwd_dkdv_kernel<kVarlen, kWindow><<<dim3(nx, Hkv, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    attn_bwd_dq_kernel<kVarlen, kWindow><<<dim3(nx, Hq, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
     DSB_CHECK_LAUNCH();
     return 0;
 }
@@ -666,60 +689,82 @@ using namespace dsb::attn;
 
 // q / k / v: 2-D bf16 tensors [B*S, *] (row stride ld_*), head `i` at columns [i*128, +128) -- for a packed QKV
 // projection output all three point into the same buffer.  o: [B*S, ld_o] (head h at h*128).  lse: fp32 [B, Hq, S] or null.
+// window > 0: causal sliding-window attention, row i sees keys i - window < j <= i (flash-attn's window_size = (window - 1,
+// 0)); window <= 0: no window.  A window needs causal.
 DSB_EXPORT int dsb_attn_fwd_bf16(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int Hq,
                                  int Hkv, int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
-                                 int v_cols, float scale, int causal, cudaStream_t stream)
+                                 int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
     if (head_dim != D || S <= 0 || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
     if (B > 1 && S % BQ) return -2;  // ragged lengths: one sequence per launch (rows of the next one would be read as keys)
+    if (window > 0 && !causal) return -2;
     if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
          reinterpret_cast<uintptr_t>(o)) & 15)
         return -2;
-    return launch_fwd<false>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols, v_cols,
-                             scale, causal, stream);
+    if (window > 0)
+        return launch_fwd<false, true>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
+                                       v_cols, scale, causal, window, stream);
+    return launch_fwd<false, false>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
+                                    v_cols, scale, causal, 0, stream);
 }
 
 // Backward.  q/k/v as in the forward; o, d_o: [B*S, ld] with head h at h*128; lse from the forward.
 // dq / dk / dv: 2-D outputs (may be column ranges of ONE packed buffer).  work: fp32 scratch of 2 * B * Hq * S elements.
+// window: the forward's.
 DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                                  void* dq, void* dk, void* dv, float* work, int B, int S, int Hq, int Hkv, int head_dim,
                                  int ld_q, int ld_k, int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
-                                 int k_cols, int v_cols, float scale, int causal, cudaStream_t stream)
+                                 int k_cols, int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
     if (head_dim != D || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
-    return launch_bwd<false>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o,
-                             ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, stream);
+    if (window > 0 && !causal) return -2;
+    if (window > 0)
+        return launch_bwd<false, true>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
+                                       ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, window, stream);
+    return launch_bwd<false, false>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
+                                    ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, 0, stream);
 }
 
 // Packed sequences (document-masked attention).  q / k / v / o as in dsb_attn_fwd_bf16 over T = cu_seqlens[n_docs] token
 // rows; cu_seqlens: int32 device array of n_docs + 1 non-decreasing offsets from 0 to T (empty documents allowed);
 // max_seqlen: the longest document (or more).  Each token attends only within its document.  lse: fp32 [Hq, T] or null.
+// window as in dsb_attn_fwd_bf16, measured inside each document.
 DSB_EXPORT int dsb_attn_varlen_fwd_bf16(const void* q, const void* k, const void* v, void* o, float* lse,
                                         const int* cu_seqlens, int n_docs, int max_seqlen, int T, int Hq, int Hkv,
                                         int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
-                                        int v_cols, float scale, int causal, cudaStream_t stream)
+                                        int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
     if (head_dim != D || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
     if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
+    if (window > 0 && !causal) return -2;
     if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
          reinterpret_cast<uintptr_t>(o)) & 15)
         return -2;
     if (T == 0 || n_docs == 0) return 0;
-    return launch_fwd<true>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols,
-                            k_cols, v_cols, scale, causal, stream);
+    if (window > 0)
+        return launch_fwd<true, true>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o,
+                                      q_cols, k_cols, v_cols, scale, causal, window, stream);
+    return launch_fwd<true, false>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols,
+                                   k_cols, v_cols, scale, causal, 0, stream);
 }
 
-// Backward of dsb_attn_varlen_fwd_bf16 (same cu_seqlens / max_seqlen; lse [Hq, T] from it).  dq / dk / dv may be column
-// ranges of one packed buffer.  work: fp32 scratch of 2 * Hq * T elements.
+// Backward of dsb_attn_varlen_fwd_bf16 (same cu_seqlens / max_seqlen / window; lse [Hq, T] from it).  dq / dk / dv may be
+// column ranges of one packed buffer.  work: fp32 scratch of 2 * Hq * T elements.
 DSB_EXPORT int dsb_attn_varlen_bwd_bf16(const void* q, const void* k, const void* v, const void* o, const void* d_o,
                                         const float* lse, void* dq, void* dk, void* dv, float* work, const int* cu_seqlens,
                                         int n_docs, int max_seqlen, int T, int Hq, int Hkv, int head_dim, int ld_q, int ld_k,
                                         int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
-                                        int k_cols, int v_cols, float scale, int causal, cudaStream_t stream)
+                                        int k_cols, int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
     if (head_dim != D || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
     if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
+    if (window > 0 && !causal) return -2;
     if (T == 0 || n_docs == 0) return 0;
-    return launch_bwd<true>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k,
-                            ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, stream);
+    if (window > 0)
+        return launch_bwd<true, true>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
+                                      ld_k, ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal,
+                                      window, stream);
+    return launch_bwd<true, false>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
+                                   ld_k, ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, 0,
+                                   stream);
 }

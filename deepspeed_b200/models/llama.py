@@ -45,6 +45,9 @@ class LlamaConfig:
     hidden_act: str = "silu"
     attention_bias: bool = False
     initializer_range: float = 0.02
+    # causal sliding-window attention (HF ``sliding_window``): token i attends to tokens i - W < j <= i, inside its document
+    # when packed; None attends to the whole causal prefix
+    sliding_window: Optional[int] = None
     # training knobs
     checkpoint_layers: int = 0  # number of decoder layers (from the front) run with activation recompute
     loss_chunk_tokens: int = 2048
@@ -71,10 +74,16 @@ class LlamaConfig:
         return n
 
     def flops_per_token(self, seq_len, causal=True):
-        """Training FLOPs/token (fwd + bwd = 3x fwd matmul FLOPs; attention counted causal)."""
+        """Training FLOPs/token (fwd + bwd = 3x fwd matmul FLOPs; attention counted causal).  With a sliding window
+        shorter than ``seq_len`` the attention term counts the visible (query, key) pairs per token."""
         h, i, L = self.hidden_size, self.intermediate_size, self.num_hidden_layers
         mm = 2 * (h * (self.q_size + 2 * self.kv_size) + self.q_size * h + 3 * h * i) * L + 2 * h * self.vocab_size
-        attn = 4 * seq_len * self.q_size * L * (0.5 if causal else 1.0)
+        W = self.sliding_window
+        if causal and W is not None and W < seq_len:
+            pairs = seq_len * W - W * (W - 1) / 2  # sum over rows of min(row + 1, W)
+            attn = 4 * (pairs / seq_len) * self.q_size * L
+        else:
+            attn = 4 * seq_len * self.q_size * L * (0.5 if causal else 1.0)
         return 3 * (mm + attn)
 
 
@@ -91,8 +100,10 @@ PRESETS = {
                       num_attention_heads=32, num_key_value_heads=32, rope_theta=10000.0, max_position_embeddings=4096),
     "phi3-mini": dict(vocab_size=32064, hidden_size=3072, intermediate_size=8192, num_hidden_layers=32,
                       num_attention_heads=32, num_key_value_heads=32, rope_theta=10000.0, max_position_embeddings=4096),
+    # Mistral-7B v0.1 (rope theta 10 000, 32 000 vocab) was trained with a 4096-token sliding window
     "mistral-7b": dict(vocab_size=32000, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
-                       num_attention_heads=32, num_key_value_heads=8, rope_theta=10000.0, max_position_embeddings=32768),
+                       num_attention_heads=32, num_key_value_heads=8, rope_theta=10000.0, max_position_embeddings=32768,
+                       sliding_window=4096),
     "tiny": dict(vocab_size=512, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=4,
                  num_key_value_heads=2, max_position_embeddings=256, rope_theta=10000.0),
 }
@@ -156,7 +167,7 @@ class LlamaAttention(nn.Module):
         qkv = self.qkv_proj(x)  # [B, S, (hq + 2 hkv) d]
         out = causal_attention(qkv.view(B * S, -1), B, S, cfg.num_attention_heads, cfg.num_key_value_heads,
                                cfg.head_dim, rope, positions, backend=cfg.attention_backend, cu_seqlens=cu_seqlens,
-                               max_seqlen=max_seqlen)
+                               max_seqlen=max_seqlen, sliding_window=cfg.sliding_window)
         return self.o_proj(out.view(B, S, cfg.q_size))
 
 

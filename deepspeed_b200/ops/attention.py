@@ -13,9 +13,15 @@ Attention-core backends (``backend=`` or ``DSB200_ATTN``):
 Packed sequences (``cu_seqlens=``): the ``B*S`` token rows hold several documents at offsets ``cu_seqlens`` and every token
 attends only within its own document (flash-attn's varlen semantics).  ``auto`` / ``native`` run the in-tree varlen
 kernel; any other backend, dtype, head dim or a CPU tensor runs one SDPA call per document.
+Sliding window (``sliding_window=W``, an int >= 1): query row ``i`` attends to key ``j`` only when ``i - W < j <= i`` -- W keys
+counting its own position (HF's ``sliding_window``, flash-attn's ``window_size=(W - 1, 0)``), measured inside each document
+with ``cu_seqlens``.  ``auto`` / ``native`` run the in-tree windowed kernel, which skips the tiles outside the band; every
+other case runs SDPA with an explicit boolean band mask per sequence or document.  A window that covers the whole sequence
+(or the longest document) is dropped, so such a call is exactly the unwindowed one.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
 """
+import numbers
 import os
 
 import torch
@@ -26,7 +32,35 @@ from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
 _ENV = os.environ.get("DSB200_ATTN", "").lower()
 
 
-def _sdpa(q, k, v, backend, causal=True, scale=None):
+def check_sliding_window(sliding_window):
+    """``None`` (no window) or the window as an int >= 1; anything else raises ``ValueError``."""
+    if sliding_window is None:
+        return None
+    if isinstance(sliding_window, bool) or not isinstance(sliding_window, numbers.Integral) or sliding_window < 1:
+        raise ValueError(f"sliding_window must be None or an int >= 1, got {sliding_window!r}")
+    return int(sliding_window)
+
+
+def _sdpa_band(q, k, v, window, scale=None):
+    """Causal sliding-window SDPA through an explicit band mask.  SDPA has no window argument and rejects ``is_causal``
+    together with ``attn_mask``, so causality is folded into the mask.  Flash takes no mask: a CUDA tensor runs one of
+    the memory-efficient, cuDNN or math kernels."""
+    i = torch.arange(q.shape[-2], device=q.device)
+    diff = i[:, None] - i[None, :]
+    mask = (diff >= 0) & (diff < window)  # True where query i may attend key j: i - window < j <= i
+    if q.shape[1] != k.shape[1]:
+        rep = q.shape[1] // k.shape[1]
+        k, v = k.repeat_interleave(rep, dim=1), v.repeat_interleave(rep, dim=1)
+    if not q.is_cuda:
+        return F.scaled_dot_product_attention(q, k, v, attn_mask=mask, scale=scale)
+    from torch.nn.attention import SDPBackend, sdpa_kernel
+    with sdpa_kernel([SDPBackend.EFFICIENT_ATTENTION, SDPBackend.CUDNN_ATTENTION, SDPBackend.MATH]):
+        return F.scaled_dot_product_attention(q, k, v, attn_mask=mask, scale=scale)
+
+
+def _sdpa(q, k, v, backend, causal=True, scale=None, window=None):
+    if window is not None and window < q.shape[-2]:
+        return _sdpa_band(q, k, v, window, scale)
     gqa = q.shape[1] != k.shape[1]
     kw = dict(is_causal=causal, scale=scale)
     if gqa:
@@ -57,7 +91,7 @@ def _sdpa(q, k, v, backend, causal=True, scale=None):
 class _PackedCausalAttention(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, backend):
+    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, backend, window):
         T = B * S
         if rope is not None:
             rope_qk_inplace(qkv, hq, hkv, d, rope, positions, S, backward=False)
@@ -67,7 +101,7 @@ class _PackedCausalAttention(torch.autograd.Function):
         v = x[:, :, hq + hkv:].transpose(1, 2)
         with torch.enable_grad():
             qd, kd, vd = (t.detach().requires_grad_(True) for t in (q, k, v))
-            out = _sdpa(qd, kd, vd, backend)
+            out = _sdpa(qd, kd, vd, backend, window=window)
         ctx.graph = (qd, kd, vd, out)
         ctx.meta = (B, S, hq, hkv, d, rope, positions)
         ctx.qkv_shape = qkv.shape
@@ -87,7 +121,7 @@ class _PackedCausalAttention(torch.autograd.Function):
         y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
         if rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, S, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None, None, None
 
 
 _TABLE = None
@@ -162,7 +196,7 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
     in-place RoPE with per-token positions, packed ``dqkv`` in the backward, un-rotated in place."""
 
     @staticmethod
-    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal):
+    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal, window):
         T = qkv.shape[0]
         if rope is not None:
             rope_qk_inplace(qkv, hq, hkv, d, rope, positions, T, backward=False)
@@ -172,7 +206,7 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
             parts = _split_doc(qkv, s, e, hq, hkv, d)  # views taken outside grad mode, like _PackedCausalAttention
             with torch.enable_grad():
                 qd, kd, vd = (t.detach().requires_grad_(True) for t in parts)
-                o = _sdpa(qd, kd, vd, backend, causal=causal)
+                o = _sdpa(qd, kd, vd, backend, causal=causal, window=window)
             out[s:e] = o.detach().transpose(1, 2).reshape(e - s, hq * d)
             graphs.append((s, e, qd, kd, vd, o))
         ctx.graphs = graphs
@@ -195,12 +229,17 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
             y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
         if rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, T, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None, None, None
 
 
-def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=None, backend="auto", causal=True):
+def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=None, backend="auto", causal=True,
+                          sliding_window=None):
     """Per-document SDPA over packed documents (any device / dtype / head dim); ``positions`` as in
-    :func:`causal_attention` (defaults to :func:`document_positions`)."""
+    :func:`causal_attention` (defaults to :func:`document_positions`).  ``sliding_window`` needs ``causal``; a document
+    longer than the window runs with a boolean band mask."""
+    window = check_sliding_window(sliding_window)
+    if window is not None and not causal:
+        raise ValueError("a sliding window is defined only for causal attention")
     T = qkv2d.shape[0]
     if rope is not None and positions is None:
         positions = document_positions(cu_seqlens, T)
@@ -208,17 +247,20 @@ def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=No
         positions = positions.reshape(-1).to(device=qkv2d.device, dtype=torch.int32)
     spans = _doc_spans(cu_seqlens, T)
     if torch.is_grad_enabled() and qkv2d.requires_grad:
-        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal)
+        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal, window)
     if rope is not None:
         rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
     out = qkv2d.new_empty(T, hq * d)
     for s, e in spans:
-        out[s:e] = _sdpa(*_split_doc(qkv2d, s, e, hq, hkv, d), backend, causal=causal).transpose(1, 2).reshape(e - s, hq * d)
+        o = _sdpa(*_split_doc(qkv2d, s, e, hq, hkv, d), backend, causal=causal, window=window)
+        out[s:e] = o.transpose(1, 2).reshape(e - s, hq * d)
     return out
 
 
-def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen):
+def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window):
     max_seqlen = check_cu_seqlens(cu_seqlens, T, max_seqlen)
+    if window is not None and window >= max_seqlen:
+        window = None  # no document is longer than the window: exactly the unwindowed call
     if backend in ("native", "auto") and qkv2d.is_cuda:
         from deepspeed_b200.ops.kernels import attention_sm100
         if attention_sm100.supports_varlen(qkv2d, hq, hkv, d):
@@ -227,33 +269,41 @@ def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_
                 positions = (document_positions(cu, T) if positions is None else positions.reshape(-1).to(
                     device=qkv2d.device, dtype=torch.int32))
             if torch.is_grad_enabled() and qkv2d.requires_grad:
-                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions)
+                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions, window)
             if rope is not None:
                 rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
             q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv)
-            return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False)[0]
+            return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False,
+                                              window=window)[0]
     if backend == "native":
         raise RuntimeError("native varlen attention kernel requested but unsupported for this input (needs a CUDA bf16 "
                            "tensor, head dim 128, 16-byte aligned rows)")
-    return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend)
+    return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend, sliding_window=window)
 
 
-def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend="auto", cu_seqlens=None, max_seqlen=None):
+def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend="auto", cu_seqlens=None, max_seqlen=None,
+                     sliding_window=None):
     """``qkv2d [B*S, (hq + 2 hkv) * d]`` -> ``[B*S, hq*d]``.  With ``cu_seqlens`` (int32 ``[n_docs + 1]`` offsets into the
     ``B*S`` rows, see :func:`check_cu_seqlens`) attention is masked to each document and ``positions`` defaults to
-    :func:`document_positions`; a device ``cu_seqlens`` needs ``max_seqlen``."""
+    :func:`document_positions`; a device ``cu_seqlens`` needs ``max_seqlen``.  ``sliding_window``: see the module
+    docstring; a value that is not an int >= 1 raises ``ValueError``."""
     backend = _ENV or backend or "auto"
+    window = check_sliding_window(sliding_window)
     if cu_seqlens is not None:
-        return _varlen_causal_attention(qkv2d, B * S, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen)
-    if backend == "native" or (backend == "auto" and qkv2d.is_cuda and _native_wins(B, S, hq, hkv, d)):
+        return _varlen_causal_attention(qkv2d, B * S, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window)
+    if window is not None and window >= S:
+        window = None  # every row sees its whole causal prefix: exactly the unwindowed call
+    # `auto` takes the in-tree kernel for a window whenever it can: it skips the tiles outside the band, the fallback masks
+    if backend == "native" or (backend == "auto" and qkv2d.is_cuda and
+                               (window is not None or _native_wins(B, S, hq, hkv, d))):
         from deepspeed_b200.ops.kernels import attention_sm100
         if attention_sm100.supports(qkv2d, hq, hkv, d, S):
             if torch.is_grad_enabled() and qkv2d.requires_grad:
-                return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions)
+                return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions, window)
             if rope is not None:
                 rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)
             q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv)
-            return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False)[0]
+            return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False, window=window)[0]
         if backend == "native":
             raise RuntimeError("native attention kernel requested but unsupported for this shape (needs bf16, head dim 128, "
                                "sequence length a multiple of 128)")
@@ -262,6 +312,6 @@ def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend
             rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)
         x = qkv2d.view(B, S, hq + 2 * hkv, d)
         out = _sdpa(x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2),
-                    x[:, :, hq + hkv:].transpose(1, 2), backend)
+                    x[:, :, hq + hkv:].transpose(1, 2), backend, window=window)
         return out.transpose(1, 2).reshape(B * S, hq * d)
-    return _PackedCausalAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, backend)
+    return _PackedCausalAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, backend, window)

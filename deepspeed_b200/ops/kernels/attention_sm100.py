@@ -3,6 +3,11 @@
 ``fwd`` / ``bwd`` work on 2-D ``[B*S, heads*128]`` views (row stride free), so the packed QKV projection output is consumed
 in place: Q, K and V are column ranges of ONE buffer and the backward writes dQ | dK | dV into one packed buffer that the
 QKV projection's backward GEMMs read directly (no transposes, no concatenation).
+
+``window`` (every entry point, default ``None``): causal sliding-window attention -- query row ``i`` attends to key ``j``
+only when ``i - window < j <= i`` (``window`` keys counting its own; flash-attn's ``window_size=(window - 1, 0)``), measured
+inside each document for the varlen forms.  The kernels skip the key / query blocks outside the band, so the cost is
+O(S * window) instead of O(S^2).
 """
 import math
 
@@ -19,23 +24,34 @@ def supports(qkv2d, hq, hkv, d, S) -> bool:
             and qkv2d.stride(-1) == 1 and qkv2d.stride(0) % 8 == 0 and qkv2d.data_ptr() % 16 == 0)
 
 
+def _window(window, causal):
+    """The kernels' ``window`` argument: 0 for no window."""
+    from deepspeed_b200.ops.attention import check_sliding_window
+    if window is None:
+        return 0
+    if not causal:
+        raise ValueError("a sliding window is defined only for causal attention")
+    return check_sliding_window(window)
+
+
 def supports_fwd(x2d, hq, hkv, d, B, S) -> bool:
     """Forward-only (inference prefill): any sequence length when one sequence is launched at a time."""
     return (x2d.is_cuda and x2d.dtype == torch.bfloat16 and d == HEAD_DIM and hq % hkv == 0 and x2d.stride(-1) == 1
             and x2d.stride(0) % 8 == 0 and x2d.data_ptr() % 16 == 0 and (B == 1 or S % BLOCK == 0))
 
 
-def fwd(q, k, v, B, S, hq, hkv, causal=True, scale=None, out=None, need_lse=True):
+def fwd(q, k, v, B, S, hq, hkv, causal=True, scale=None, out=None, need_lse=True, window=None):
     """``q [B*S, hq*128]``, ``k / v [B*S, hkv*128]`` (2-D views, any row stride) -> ``(o [B*S, hq*128], lse [B, hq, S])``.
     ``S`` may be any length when ``B == 1`` (a ragged last block is masked inside the kernel)."""
     T = B * S
+    window = _window(window, causal)
     if out is None:
         out = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(B, hq, S, dtype=torch.float32, device=q.device) if need_lse else None
     scale = float(scale) if scale is not None else 1.0 / math.sqrt(HEAD_DIM)
     rc = N.cuda().dsb_attn_fwd_bf16(N.ptr(q), N.ptr(k), N.ptr(v), N.ptr(out), N.ptr(lse), B, S, hq, hkv, HEAD_DIM, q.stride(0),
                                     k.stride(0), v.stride(0), out.stride(0), q.shape[1], k.shape[1], v.shape[1],
-                                    N.c_f(scale), int(bool(causal)), N.stream())
+                                    N.c_f(scale), int(bool(causal)), window, N.stream())
     N.check(rc, "attn_fwd_bf16")
     return out, lse
 
@@ -53,13 +69,14 @@ def _check_cu(cu_seqlens, dev):
     return cu_seqlens.numel() - 1
 
 
-def fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, out=None, need_lse=True):
+def fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, out=None, need_lse=True, window=None):
     """Document-masked attention over packed sequences: ``q [T, hq*128]``, ``k / v [T, hkv*128]`` (2-D views, any row
     stride), ``cu_seqlens`` int32 ``[n_docs + 1]`` on the device (offsets from 0 to T, non-decreasing, empty documents
     allowed), ``max_seqlen`` >= the longest document.  Each token attends only to tokens of its own document.
     Returns ``(o [T, hq*128], lse [hq, T])`` -- the LSE is indexed by absolute token row."""
     T = q.shape[0]
     n_docs = _check_cu(cu_seqlens, q.device)
+    window = _window(window, causal)
     if out is None:
         out = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=q.device)
     lse = torch.empty(hq, T, dtype=torch.float32, device=q.device) if need_lse else None
@@ -67,7 +84,7 @@ def fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None
     rc = N.cuda().dsb_attn_varlen_fwd_bf16(N.ptr(q), N.ptr(k), N.ptr(v), N.ptr(out), N.ptr(lse), N.ptr(cu_seqlens), n_docs,
                                            int(max_seqlen), T, hq, hkv, HEAD_DIM, q.stride(0), k.stride(0), v.stride(0),
                                            out.stride(0), q.shape[1], k.shape[1], v.shape[1], N.c_f(scale),
-                                           int(bool(causal)), N.stream())
+                                           int(bool(causal)), window, N.stream())
     N.check(rc, "attn_varlen_fwd_bf16")
     return out, lse
 
@@ -77,10 +94,12 @@ def split_packed(qkv2d, hq, hkv, d=HEAD_DIM):
     return qkv2d[:, :hq * d], qkv2d[:, hq * d:(hq + hkv) * d], qkv2d[:, (hq + hkv) * d:]
 
 
-def bwd(d_o, q, k, v, o, lse, B, S, hq, hkv, causal=True, scale=None, dq=None, dk=None, dv=None):
-    """Gradients of :func:`fwd`.  ``dq / dk / dv`` may be column views of one packed ``[T, (hq + 2 hkv) * 128]`` buffer."""
+def bwd(d_o, q, k, v, o, lse, B, S, hq, hkv, causal=True, scale=None, dq=None, dk=None, dv=None, window=None):
+    """Gradients of :func:`fwd` (same ``window``).  ``dq / dk / dv`` may be column views of one packed
+    ``[T, (hq + 2 hkv) * 128]`` buffer."""
     T = B * S
     dev = q.device
+    window = _window(window, causal)
     if dq is None:
         dq = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=dev)
     if dk is None:
@@ -94,17 +113,19 @@ def bwd(d_o, q, k, v, o, lse, B, S, hq, hkv, causal=True, scale=None, dq=None, d
     rc = N.cuda().dsb_attn_bwd_bf16(N.ptr(q), N.ptr(k), N.ptr(v), N.ptr(o), N.ptr(d_o), N.ptr(lse), N.ptr(dq), N.ptr(dk),
                                     N.ptr(dv), N.ptr(work), B, S, hq, hkv, HEAD_DIM, q.stride(0), k.stride(0), v.stride(0),
                                     o.stride(0), d_o.stride(0), dq.stride(0), dk.stride(0), dv.stride(0), q.shape[1],
-                                    k.shape[1], v.shape[1], N.c_f(scale), int(bool(causal)), N.stream())
+                                    k.shape[1], v.shape[1], N.c_f(scale), int(bool(causal)), window, N.stream())
     N.check(rc, "attn_bwd_bf16")
     return dq, dk, dv
 
 
-def bwd_varlen(d_o, q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, dq=None, dk=None, dv=None):
-    """Gradients of :func:`fwd_varlen` (same ``cu_seqlens`` / ``max_seqlen``, ``lse [hq, T]`` from it).  ``dq / dk / dv``
-    may be column views of one packed ``[T, (hq + 2 hkv) * 128]`` buffer."""
+def bwd_varlen(d_o, q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, scale=None, dq=None, dk=None, dv=None,
+               window=None):
+    """Gradients of :func:`fwd_varlen` (same ``cu_seqlens`` / ``max_seqlen`` / ``window``, ``lse [hq, T]`` from it).
+    ``dq / dk / dv`` may be column views of one packed ``[T, (hq + 2 hkv) * 128]`` buffer."""
     T = q.shape[0]
     dev = q.device
     n_docs = _check_cu(cu_seqlens, dev)
+    window = _window(window, causal)
     if dq is None:
         dq = torch.empty(T, hq * HEAD_DIM, dtype=torch.bfloat16, device=dev)
     if dk is None:
@@ -119,7 +140,7 @@ def bwd_varlen(d_o, q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=Tru
                                            N.ptr(dk), N.ptr(dv), N.ptr(work), N.ptr(cu_seqlens), n_docs, int(max_seqlen), T,
                                            hq, hkv, HEAD_DIM, q.stride(0), k.stride(0), v.stride(0), o.stride(0),
                                            d_o.stride(0), dq.stride(0), dk.stride(0), dv.stride(0), q.shape[1], k.shape[1],
-                                           v.shape[1], N.c_f(scale), int(bool(causal)), N.stream())
+                                           v.shape[1], N.c_f(scale), int(bool(causal)), window, N.stream())
     N.check(rc, "attn_varlen_bwd_bf16")
     return dq, dk, dv
 
@@ -129,33 +150,34 @@ class _PackedAttention(torch.autograd.Function):
     dQ | dK | dV in ONE packed buffer -- exactly the layout the QKV projection's backward GEMMs consume."""
 
     @staticmethod
-    def forward(ctx, qkv, B, S, hq, hkv, rope, positions):
+    def forward(ctx, qkv, B, S, hq, hkv, rope, positions, window):
         from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
         if rope is not None:
             rope_qk_inplace(qkv, hq, hkv, HEAD_DIM, rope, positions, S, backward=False)
         q, k, v = split_packed(qkv, hq, hkv)
-        o, lse = fwd(q, k, v, B, S, hq, hkv, causal=True)
+        o, lse = fwd(q, k, v, B, S, hq, hkv, causal=True, window=window)
         ctx.save_for_backward(qkv, o, lse)
-        ctx.meta = (B, S, hq, hkv, rope, positions)
+        ctx.meta = (B, S, hq, hkv, rope, positions, window)
         return o
 
     @staticmethod
     def backward(ctx, d_o):
         from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
         qkv, o, lse = ctx.saved_tensors
-        B, S, hq, hkv, rope, positions = ctx.meta
+        B, S, hq, hkv, rope, positions, window = ctx.meta
         q, k, v = split_packed(qkv, hq, hkv)
         dqkv = torch.empty_like(qkv)
         dq, dk, dv = split_packed(dqkv, hq, hkv)
-        bwd(d_o.reshape(B * S, hq * HEAD_DIM), q, k, v, o, lse, B, S, hq, hkv, causal=True, dq=dq, dk=dk, dv=dv)
+        bwd(d_o.reshape(B * S, hq * HEAD_DIM), q, k, v, o, lse, B, S, hq, hkv, causal=True, dq=dq, dk=dk, dv=dv,
+            window=window)
         if rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, HEAD_DIM, rope, positions, S, backward=True)
-        return dqkv, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None
 
 
-def packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None):
+def packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, window=None):
     assert d == HEAD_DIM
-    return _PackedAttention.apply(qkv2d, B, S, hq, hkv, rope, positions)
+    return _PackedAttention.apply(qkv2d, B, S, hq, hkv, rope, positions, window)
 
 
 class _PackedVarlenAttention(torch.autograd.Function):
@@ -163,33 +185,33 @@ class _PackedVarlenAttention(torch.autograd.Function):
     in-place RoPE, ``cu_seqlens`` / ``max_seqlen`` the document masking."""
 
     @staticmethod
-    def forward(ctx, qkv, cu_seqlens, max_seqlen, hq, hkv, rope, positions):
+    def forward(ctx, qkv, cu_seqlens, max_seqlen, hq, hkv, rope, positions, window):
         from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
         T = qkv.shape[0]
         if rope is not None:
             rope_qk_inplace(qkv, hq, hkv, HEAD_DIM, rope, positions, T, backward=False)
         q, k, v = split_packed(qkv, hq, hkv)
-        o, lse = fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True)
+        o, lse = fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, window=window)
         ctx.save_for_backward(qkv, o, lse, cu_seqlens)
-        ctx.meta = (max_seqlen, hq, hkv, rope, positions)
+        ctx.meta = (max_seqlen, hq, hkv, rope, positions, window)
         return o
 
     @staticmethod
     def backward(ctx, d_o):
         from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
         qkv, o, lse, cu_seqlens = ctx.saved_tensors
-        max_seqlen, hq, hkv, rope, positions = ctx.meta
+        max_seqlen, hq, hkv, rope, positions, window = ctx.meta
         T = qkv.shape[0]
         q, k, v = split_packed(qkv, hq, hkv)
         dqkv = torch.empty_like(qkv)
         dq, dk, dv = split_packed(dqkv, hq, hkv)
         bwd_varlen(d_o.reshape(T, hq * HEAD_DIM), q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, dq=dq,
-                   dk=dk, dv=dv)
+                   dk=dk, dv=dv, window=window)
         if rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, HEAD_DIM, rope, positions, T, backward=True)
-        return dqkv, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None
 
 
-def packed_varlen_attention(qkv2d, cu_seqlens, max_seqlen, hq, hkv, d, rope=None, positions=None):
+def packed_varlen_attention(qkv2d, cu_seqlens, max_seqlen, hq, hkv, d, rope=None, positions=None, window=None):
     assert d == HEAD_DIM
-    return _PackedVarlenAttention.apply(qkv2d, cu_seqlens, max_seqlen, hq, hkv, rope, positions)
+    return _PackedVarlenAttention.apply(qkv2d, cu_seqlens, max_seqlen, hq, hkv, rope, positions, window)
