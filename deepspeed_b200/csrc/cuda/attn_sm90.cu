@@ -1,7 +1,9 @@
-// Training attention for sm_90a: causal / full softmax(Q K^T / sqrt(d)) V with grouped-query heads, head dim 128, bf16.
+// Training attention for sm_90a: causal / full softmax(Q K^T / sqrt(d)) V with grouped-query heads, head dim 64 or 128
+// (the template parameter kD of every kernel), bf16.
 //
 // Forward -- one CTA per (128 query rows, query head, batch):
-//   warp 8      TMA producer: Q once, then a 3-stage ring of K and V tiles (64 keys x 128 dims = 16 KiB each)
+//   warp 8      TMA producer: Q once, then a 3-stage ring of K and V tiles (64 keys x kD dims: 16 KiB at kD = 128, 8 KiB
+//               at kD = 64)
 //   warps 0-7   two consumer warpgroups, 64 query rows each: S = Q K_j^T with wgmma (both operands in shared memory,
 //               accumulators in registers), online softmax in the log2 domain (ex2.approx) on the accumulator fragments,
 //               then O += P V_j with P taken straight from registers as the A operand (the m64n64 accumulator layout is the
@@ -19,36 +21,47 @@ namespace dsb {
 namespace attn {
 using namespace dsb::tc;
 
-constexpr int BQ = 128, BS = 64, D = 128;
+constexpr int BQ = 128, BS = 64;
 constexpr int kThreads = 288;                            // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int kProducer = 256;                           // thread index of the producer
-constexpr uint32_t TILE = BS * D * 2;                    // 16 KiB: [64 x 128] bf16 = 2 TMA boxes of [64 x 64]
-constexpr uint32_t HALF = TILE / 2;                      // 8 KiB box (one 128-byte swizzle span of 64 bf16 per row)
+constexpr uint32_t BOX = BS * 64 * 2;                    // 8 KiB TMA box [64 x 64] bf16 (one 128-byte swizzle span per row)
+template <int kD>
+constexpr uint32_t kTile = BS * kD * 2;                  // [64 x kD] bf16 tile of one head = kD / 64 boxes
 constexpr float kNegInf = -__builtin_huge_valf();
 
-// Operand descriptors of a [64 x 128] tile at `t`:
-//   K-major over the 128 columns (S = Q K^T: Q as A, K as B): 16-column step kk in 0..7
-__device__ __forceinline__ uint64_t desc_k(uint32_t t, int kk) { return desc_kmajor_sw128(t + (kk >> 2) * HALF + (kk & 3) * 32); }
-//   MN-major, rows as the reduction dimension, the 128 columns as N (O = P V: V as B): 16-row step kk in 0..3
-__device__ __forceinline__ uint64_t desc_mn(uint32_t t, int kk) { return desc_mnmajor_sw128(t + kk * 2048, HALF); }
+// Operand descriptors of a [64 x kD] tile at `t`:
+//   K-major over the kD columns (S = Q K^T: Q as A, K as B): 16-column step kk in 0..kD/16-1, the second box from kk = 4
+__device__ __forceinline__ uint64_t desc_k(uint32_t t, int kk) { return desc_kmajor_sw128(t + (kk >> 2) * BOX + (kk & 3) * 32); }
+//   MN-major, rows as the reduction dimension, the kD columns as N (O = P V: V as B): 16-row step kk in 0..3.  The LBO
+//   (the distance to the second 64-wide atom) is unused at kD = 64.
+__device__ __forceinline__ uint64_t desc_mn(uint32_t t, int kk) { return desc_mnmajor_sw128(t + kk * 2048, BOX); }
 
+template <int kD>
 __device__ __forceinline__ void load_tile(uint32_t dst, const CUtensorMap* map, uint32_t bar, int col, int row)
 {
+    static_assert(kD == 64 || kD == 128, "head dim 64 or 128");
     tma_load_2d(dst, map, bar, col, row);
-    tma_load_2d(dst + HALF, map, bar, col + 64, row);
+    if constexpr (kD == 128) tma_load_2d(dst + BOX, map, bar, col + 64, row);
 }
 
-// acc = A_tile(64 rows) x B_tile(64 rows)^T over the 128 columns: m64n64, 8 steps
+// acc = A_tile(64 rows) x B_tile(64 rows)^T over the kD columns: m64n64, kD / 16 steps
+template <int kD>
 __device__ __forceinline__ void mma_rows_x_rows(float* acc, uint32_t a, uint32_t b)
 {
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) wgmma_m64n64k16_ss<0, 0>(acc, desc_k(a, kk), desc_k(b, kk), kk > 0 ? 1 : 0);
+    for (int kk = 0; kk < kD / 16; ++kk) wgmma_m64n64k16_ss<0, 0>(acc, desc_k(a, kk), desc_k(b, kk), kk > 0 ? 1 : 0);
 }
-// acc[64 x 128] += P[64 x 64] (register fragments of an m64n64 fp32 block) x tile[64 rows x 128]
+// acc[64 x kD] += P[64 x 64] (register fragments of an m64n64 fp32 block) x tile[64 rows x kD]
+template <int kD>
 __device__ __forceinline__ void mma_regs_x_tile(float* acc, const uint32_t (*frag)[4], uint32_t t)
 {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_m64n128k16_rs<1>(acc, frag[kk], desc_mn(t, kk), 1);
+    for (int kk = 0; kk < 4; ++kk) {
+        if constexpr (kD == 128)
+            wgmma_m64n128k16_rs<1>(acc, frag[kk], desc_mn(t, kk), 1);
+        else
+            wgmma_m64n64k16_rs<1>(acc, frag[kk], desc_mn(t, kk), 1);
+    }
 }
 // m64n64 fp32 accumulator -> bf16 A fragments of four k16 steps
 __device__ __forceinline__ void to_frags(const float* s, uint32_t (*f)[4])
@@ -71,7 +84,8 @@ __device__ __forceinline__ float quad_sum(float v)
     v += __shfl_xor_sync(0xffffffffu, v, 1);
     return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// store a 64 x 128 fp32 accumulator (times `mul`) as bf16 rows `row0 + r` (r < rows) of a [*, ld] matrix at column col0
+// store a 64 x kD fp32 accumulator (times `mul`) as bf16 rows `row0 + r` (r < rows) of a [*, ld] matrix at column col0
+template <int kD>
 __device__ __forceinline__ void store_acc(const float* acc, __nv_bfloat16* base, int64_t ld, int row_local, int rows, int col0,
                                           int c_in, float mul0, float mul1)
 {
@@ -82,7 +96,7 @@ __device__ __forceinline__ void store_acc(const float* acc, __nv_bfloat16* base,
         const float m = i ? mul1 : mul0;
         __nv_bfloat16* dst = base + static_cast<int64_t>(r) * ld + col0 + c_in;
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+        for (int j = 0; j < kD / 8; ++j)
             *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16(acc[4 * j + 2 * i] * m, acc[4 * j + 2 * i + 1] * m);
     }
 }
@@ -124,20 +138,24 @@ __device__ __forceinline__ int first_key_block(int q0, int window)
     return kWindow ? max(0, q0 - window + 1) / BS : 0;
 }
 
-namespace kf {  // forward shared-memory plan
-constexpr int KV_STAGES = 3;
-constexpr uint32_t SM_Q = 0;                              // 2 tiles (one per consumer warpgroup)
-constexpr uint32_t SM_KV = SM_Q + 2 * TILE;               // KV_STAGES x (K tile, V tile)
-constexpr uint32_t SM_BAR = SM_KV + KV_STAGES * 2 * TILE;
-constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
-}  // namespace kf
+template <int kD>
+struct kf {  // forward shared-memory plan
+    static constexpr int KV_STAGES = 3;
+    static constexpr uint32_t TILE = kTile<kD>;
+    static constexpr uint32_t SM_Q = 0;                         // 2 tiles (one per consumer warpgroup)
+    static constexpr uint32_t SM_KV = SM_Q + 2 * TILE;          // KV_STAGES x (K tile, V tile)
+    static constexpr uint32_t SM_BAR = SM_KV + KV_STAGES * 2 * TILE;
+    static constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
+};
 
-template <bool kVarlen, bool kWindow>
+template <int kD, bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                 const __grid_constant__ CUtensorMap map_v, const FwdParams p)
 {
-    using namespace kf;
+    using Plan = kf<kD>;
+    constexpr int KV_STAGES = Plan::KV_STAGES;
+    constexpr uint32_t TILE = Plan::TILE, SM_Q = Plan::SM_Q, SM_KV = Plan::SM_KV, SM_BAR = Plan::SM_BAR;
     const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
     int row_base, len;  // first token row and length of this sequence
     if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, q0, row_base, len)) return;
@@ -170,15 +188,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             prefetch_map(&map_k);
             prefetch_map(&map_v);
             mbar_expect_tx(q_full, 2 * TILE);
-            load_tile(sbase + SM_Q, &map_q, q_full, h * D, row_base + q0);
-            load_tile(sbase + SM_Q + TILE, &map_q, q_full, h * D, row_base + q0 + BS);
+            load_tile<kD>(sbase + SM_Q, &map_q, q_full, h * kD, row_base + q0);
+            load_tile<kD>(sbase + SM_Q + TILE, &map_q, q_full, h * kD, row_base + q0 + BS);
             for (int j = j0; j < n_kv; ++j) {
                 const int s = (j - j0) % KV_STAGES;
                 mbar_wait(kv_empty(s), (((j - j0) / KV_STAGES) & 1) ^ 1);
                 mbar_expect_tx(kv_full(s), 2 * TILE);
                 const uint32_t dst = sbase + SM_KV + s * 2 * TILE;
-                load_tile(dst, &map_k, kv_full(s), kvh * D, row_base + j * BS);
-                load_tile(dst + TILE, &map_v, kv_full(s), kvh * D, row_base + j * BS);
+                load_tile<kD>(dst, &map_k, kv_full(s), kvh * kD, row_base + j * BS);
+                load_tile<kD>(dst + TILE, &map_v, kv_full(s), kvh * kD, row_base + j * BS);
             }
         }
         return;
@@ -190,9 +208,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     const int r_loc = 16 * (warp & 3) + (lane >> 2);          // this thread's rows: qr0 + r_loc (+8)
     const int c_in = 2 * (lane & 3);
     const uint32_t sq = sbase + SM_Q + wg * TILE;
-    float o[64];
+    float o[kD / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
     float m_run[2] = {kNegInf, kNegInf}, l_run[2] = {0.f, 0.f};
     mbar_wait(q_full, 0);
 
@@ -204,7 +222,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             const uint32_t sk = sbase + SM_KV + s * 2 * TILE, sv = sk + TILE;
             float sc[32];
             wgmma_fence();
-            mma_rows_x_rows(sc, sq, sk);
+            mma_rows_x_rows<kD>(sc, sq, sk);
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs<32>(sc);
@@ -232,7 +250,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
                 l_run[i] *= alpha[i];
             }
 #pragma unroll
-            for (int jj = 0; jj < 16; ++jj)
+            for (int jj = 0; jj < kD / 8; ++jj)
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
                     o[4 * jj + 2 * i] *= alpha[i];
@@ -251,10 +269,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
             uint32_t pf[4][4];
             to_frags(sc, pf);
             wgmma_fence();
-            mma_regs_x_tile(o, pf, sv);
+            mma_regs_x_tile<kD>(o, pf, sv);
             wgmma_commit();
             wgmma_wait<0>();
-            fence_regs<64>(o);
+            fence_regs<kD / 2>(o);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(kv_empty(s));
@@ -268,8 +286,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         inv[i] = l_run[i] > 0.f ? 1.f / l_run[i] : 0.f;
     }
     const int rows = len - qr0;  // rows of this warpgroup inside the sequence
-    store_acc(o, p.o + static_cast<int64_t>(row_base + qr0) * p.ld_o, p.ld_o, r_loc, rows < BS ? rows : BS, h * D, c_in,
-              inv[0], inv[1]);
+    store_acc<kD>(o, p.o + static_cast<int64_t>(row_base + qr0) * p.ld_o, p.ld_o, r_loc, rows < BS ? rows : BS, h * kD, c_in,
+                  inv[0], inv[1]);
     if (p.lse != nullptr && (lane & 3) == 0) {
         float* lse = kVarlen ? p.lse + static_cast<int64_t>(h) * p.T + row_base
                              : p.lse + (static_cast<int64_t>(b) * p.Hq + h) * p.S;
@@ -312,8 +330,11 @@ __device__ __forceinline__ int64_t stat_base(const BwdParams& p, int b, int h, i
     return kVarlen ? static_cast<int64_t>(h) * p.T + row_base : (static_cast<int64_t>(b) * p.Hq + h) * p.S;
 }
 
-// delta[b,h,s] = sum_d dO * O ; lse2 = lse * log2(e).  One warp per (token, head) row of 128 elements.  The varlen
-// [Hq, T] layout is this kernel's B = 1, S = T.
+// delta[b,h,s] = sum_d dO * O ; lse2 = lse * log2(e).  One warp per (token, head) row of kD elements, 4 per lane: at
+// kD = 64 lanes 16-31 add zeros, so delta is summed in the order the kD = 128 kernel uses on a head padded with zero
+// columns, and the backward of a d = 64 head is bit-equal to the d = 128 backward of the zero-padded head.
+// The varlen [Hq, T] layout is this kernel's B = 1, S = T.
+template <int kD>
 __global__ void __launch_bounds__(256)
 attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o, const float* __restrict__ lse,
                      float* __restrict__ delta, float* __restrict__ lse2, int B, int S, int Hq, int ld_o, int ld_do)
@@ -324,15 +345,17 @@ attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* _
     if (w >= rows) return;
     const int h = static_cast<int>(w % Hq);
     const int64_t t = w / Hq;  // token row b*S + s
-    const __nv_bfloat16* po = o + t * ld_o + h * D + lane * 4;
-    const __nv_bfloat16* pd = d_o + t * ld_do + h * D + lane * 4;
-    const uint2 a = *reinterpret_cast<const uint2*>(po);
-    const uint2 g = *reinterpret_cast<const uint2*>(pd);
     float acc = 0.f;
-    acc = fmaf(__uint_as_float(a.x << 16), __uint_as_float(g.x << 16), acc);
-    acc = fmaf(__uint_as_float(a.x & 0xffff0000u), __uint_as_float(g.x & 0xffff0000u), acc);
-    acc = fmaf(__uint_as_float(a.y << 16), __uint_as_float(g.y << 16), acc);
-    acc = fmaf(__uint_as_float(a.y & 0xffff0000u), __uint_as_float(g.y & 0xffff0000u), acc);
+    if (kD == 128 || lane < kD / 4) {
+        const __nv_bfloat16* po = o + t * ld_o + h * kD + lane * 4;
+        const __nv_bfloat16* pd = d_o + t * ld_do + h * kD + lane * 4;
+        const uint2 a = *reinterpret_cast<const uint2*>(po);
+        const uint2 g = *reinterpret_cast<const uint2*>(pd);
+        acc = fmaf(__uint_as_float(a.x << 16), __uint_as_float(g.x << 16), acc);
+        acc = fmaf(__uint_as_float(a.x & 0xffff0000u), __uint_as_float(g.x & 0xffff0000u), acc);
+        acc = fmaf(__uint_as_float(a.y << 16), __uint_as_float(g.y << 16), acc);
+        acc = fmaf(__uint_as_float(a.y & 0xffff0000u), __uint_as_float(g.y & 0xffff0000u), acc);
+    }
     acc = warp_reduce<SumOp>(acc);
     if (lane == 0) {
         const int b = static_cast<int>(t / S), s_ = static_cast<int>(t % S);
@@ -342,26 +365,30 @@ attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* _
     }
 }
 
-namespace kb {  // shared-memory plan of both backward kernels: 4 resident tiles + 2 stages x 2 streamed tiles
-constexpr int STAGES = 2;
-constexpr uint32_t SM_RES = 0;                            // [X_wg0, X_wg1, Y_wg0, Y_wg1]
-constexpr uint32_t SM_STR = SM_RES + 4 * TILE;            // STAGES x (X tile, Y tile)
-constexpr uint32_t SM_BAR = SM_STR + STAGES * 2 * TILE;
-constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
-}  // namespace kb
+template <int kD>
+struct kb {  // shared-memory plan of both backward kernels: 4 resident tiles + 2 stages x 2 streamed tiles
+    static constexpr int STAGES = 2;
+    static constexpr uint32_t TILE = kTile<kD>;
+    static constexpr uint32_t SM_RES = 0;                       // [X_wg0, X_wg1, Y_wg0, Y_wg1]
+    static constexpr uint32_t SM_STR = SM_RES + 4 * TILE;       // STAGES x (X tile, Y tile)
+    static constexpr uint32_t SM_BAR = SM_STR + STAGES * 2 * TILE;
+    static constexpr uint32_t SM_TOTAL = SM_BAR + 256 + 1024;
+};
 
 // ---- (A) dK, dV ---------------------------------------------------------------------------------------------------------------
-// dK and dV both live in registers (128 fp32 per thread), so at the 168 registers a 288-thread CTA can launch with the
-// compiler spills a little and serialises the wgmma issue of this kernel.
+// dK and dV both live in registers (kD fp32 per thread), so at kD = 128, at the 168 registers a 288-thread CTA can launch
+// with, the compiler spills a little and serialises the wgmma issue of this kernel.
 // Varlen: the query blocks cover ceil(len / 64) blocks; queries past `len` (the next document's rows, or TMA zero fill) get
 // P = 0 and dS = 0 explicitly -- the causal mask does not remove them.  Key rows past `len` are computed and never stored.
 // Sliding window: the query blocks stop after the last query that sees the CTA's last key (k0 + 127 + window - 1).
-template <bool kVarlen, bool kWindow>
+template <int kD, bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                      const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
 {
-    using namespace kb;
+    using Plan = kb<kD>;
+    constexpr int STAGES = Plan::STAGES;
+    constexpr uint32_t TILE = Plan::TILE, SM_RES = Plan::SM_RES, SM_STR = Plan::SM_STR, SM_BAR = Plan::SM_BAR;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const uint32_t sbase = smem_u32(smem);
@@ -391,8 +418,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
         if (threadIdx.x == kProducer) {
             mbar_expect_tx(res_full, 4 * TILE);
             for (int w = 0; w < 2; ++w) {
-                load_tile(sbase + SM_RES + w * TILE, &map_k, res_full, kvh * D, row_base + k0 + w * BS);
-                load_tile(sbase + SM_RES + (2 + w) * TILE, &map_v, res_full, kvh * D, row_base + k0 + w * BS);
+                load_tile<kD>(sbase + SM_RES + w * TILE, &map_k, res_full, kvh * kD, row_base + k0 + w * BS);
+                load_tile<kD>(sbase + SM_RES + (2 + w) * TILE, &map_v, res_full, kvh * kD, row_base + k0 + w * BS);
             }
             int it = 0;
             for (int qh = kvh * rep; qh < (kvh + 1) * rep; ++qh)
@@ -401,8 +428,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                     mbar_wait(empty(s), ((it / STAGES) & 1) ^ 1);
                     mbar_expect_tx(full(s), 2 * TILE);
                     const uint32_t dst = sbase + SM_STR + s * 2 * TILE;
-                    load_tile(dst, &map_q, full(s), qh * D, row_base + qb * BS);
-                    load_tile(dst + TILE, &map_do, full(s), qh * D, row_base + qb * BS);
+                    load_tile<kD>(dst, &map_q, full(s), qh * kD, row_base + qb * BS);
+                    load_tile<kD>(dst + TILE, &map_do, full(s), qh * kD, row_base + qb * BS);
                 }
         }
         return;
@@ -414,9 +441,9 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     const int r_loc = 16 * (warp & 3) + (lane >> 2);
     const int c_in = 2 * (lane & 3);
     const uint32_t sk = sbase + SM_RES + wg * TILE, sv = sbase + SM_RES + (2 + wg) * TILE;
-    float dk[64], dv[64];
+    float dk[kD / 2], dv[kD / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) dk[i] = dv[i] = 0.f;
+    for (int i = 0; i < kD / 2; ++i) dk[i] = dv[i] = 0.f;
     mbar_wait(res_full, 0);
 
     int it = 0;
@@ -430,8 +457,8 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                 const uint32_t sq = sbase + SM_STR + s * 2 * TILE, sdo = sq + TILE;
                 float st[32], dpt[32];
                 wgmma_fence();
-                mma_rows_x_rows(dpt, sv, sdo);  // dP^T = V dO^T
-                mma_rows_x_rows(st, sk, sq);    // S^T  = K Q^T
+                mma_rows_x_rows<kD>(dpt, sv, sdo);  // dP^T = V dO^T
+                mma_rows_x_rows<kD>(st, sk, sq);    // S^T  = K Q^T
                 wgmma_commit();
                 wgmma_wait<0>();
                 fence_regs<32>(st);
@@ -458,12 +485,12 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
                 to_frags(st, pf);
                 to_frags(dpt, df);
                 wgmma_fence();
-                mma_regs_x_tile(dv, pf, sdo);  // dV += P^T dO
-                mma_regs_x_tile(dk, df, sq);   // dK += dS^T Q
+                mma_regs_x_tile<kD>(dv, pf, sdo);  // dV += P^T dO
+                mma_regs_x_tile<kD>(dk, df, sq);   // dK += dS^T Q
                 wgmma_commit();
                 wgmma_wait<0>();
-                fence_regs<64>(dv);
-                fence_regs<64>(dk);
+                fence_regs<kD / 2>(dv);
+                fence_regs<kD / 2>(dk);
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(empty(s));
@@ -471,19 +498,21 @@ attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_con
     }
     const int64_t r0 = row_base + kr0;
     const int rows = kVarlen ? min(len - kr0, BS) : BS;
-    store_acc(dk, p.dk + r0 * p.ld_dk, p.ld_dk, r_loc, rows, kvh * D, c_in, 1.f, 1.f);
-    store_acc(dv, p.dv + r0 * p.ld_dv, p.ld_dv, r_loc, rows, kvh * D, c_in, 1.f, 1.f);
+    store_acc<kD>(dk, p.dk + r0 * p.ld_dk, p.ld_dk, r_loc, rows, kvh * kD, c_in, 1.f, 1.f);
+    store_acc<kD>(dv, p.dv + r0 * p.ld_dv, p.ld_dv, r_loc, rows, kvh * kD, c_in, 1.f, 1.f);
 }
 
 // ---- (B) dQ -------------------------------------------------------------------------------------------------------------------
 // Varlen: keys past `len` get P = 0 and dS = 0; rows past `len` read no statistics and are never stored.
 // Sliding window: the key blocks start at the forward's first block, keys before a row's window get P = 0 and dS = 0.
-template <bool kVarlen, bool kWindow>
+template <int kD, bool kVarlen, bool kWindow>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
                    const __grid_constant__ CUtensorMap map_v, const __grid_constant__ CUtensorMap map_do, const BwdParams p)
 {
-    using namespace kb;
+    using Plan = kb<kD>;
+    constexpr int STAGES = Plan::STAGES;
+    constexpr uint32_t TILE = Plan::TILE, SM_RES = Plan::SM_RES, SM_STR = Plan::SM_STR, SM_BAR = Plan::SM_BAR;
     const int q0 = blockIdx.x * BQ, h = blockIdx.y, b = blockIdx.z;
     int row_base, len;
     if (!doc_rows<kVarlen>(p.cu, p.T, p.S, b, q0, row_base, len)) return;
@@ -514,16 +543,16 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
         if (threadIdx.x == kProducer) {
             mbar_expect_tx(res_full, 4 * TILE);
             for (int w = 0; w < 2; ++w) {
-                load_tile(sbase + SM_RES + w * TILE, &map_q, res_full, h * D, row_base + q0 + w * BS);
-                load_tile(sbase + SM_RES + (2 + w) * TILE, &map_do, res_full, h * D, row_base + q0 + w * BS);
+                load_tile<kD>(sbase + SM_RES + w * TILE, &map_q, res_full, h * kD, row_base + q0 + w * BS);
+                load_tile<kD>(sbase + SM_RES + (2 + w) * TILE, &map_do, res_full, h * kD, row_base + q0 + w * BS);
             }
             for (int j = j0; j < n_kv; ++j) {
                 const int s = (j - j0) % STAGES;
                 mbar_wait(empty(s), (((j - j0) / STAGES) & 1) ^ 1);
                 mbar_expect_tx(full(s), 2 * TILE);
                 const uint32_t dst = sbase + SM_STR + s * 2 * TILE;
-                load_tile(dst, &map_k, full(s), kvh * D, row_base + j * BS);
-                load_tile(dst + TILE, &map_v, full(s), kvh * D, row_base + j * BS);
+                load_tile<kD>(dst, &map_k, full(s), kvh * kD, row_base + j * BS);
+                load_tile<kD>(dst + TILE, &map_v, full(s), kvh * kD, row_base + j * BS);
             }
         }
         return;
@@ -539,9 +568,9 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
     const bool in0 = !kVarlen || qr0 + r_loc < len, in1 = !kVarlen || qr0 + r_loc + 8 < len;
     const float l2[2] = {in0 ? p.lse2[stat] : 0.f, in1 ? p.lse2[stat + 8] : 0.f};
     const float dl[2] = {in0 ? p.delta[stat] : 0.f, in1 ? p.delta[stat + 8] : 0.f};
-    float dq[64];
+    float dq[kD / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) dq[i] = 0.f;
+    for (int i = 0; i < kD / 2; ++i) dq[i] = 0.f;
     mbar_wait(res_full, 0);
 
     for (int j = j0; j < n_kv; ++j) {
@@ -551,8 +580,8 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             const uint32_t sk = sbase + SM_STR + s * 2 * TILE, sv = sk + TILE;
             float sc[32], dp[32];
             wgmma_fence();
-            mma_rows_x_rows(sc, sq, sk);   // S  = Q K^T
-            mma_rows_x_rows(dp, sdo, sv);  // dP = dO V^T
+            mma_rows_x_rows<kD>(sc, sq, sk);   // S  = Q K^T
+            mma_rows_x_rows<kD>(dp, sdo, sv);  // dP = dO V^T
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs<32>(sc);
@@ -574,26 +603,27 @@ attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
             uint32_t df[4][4];
             to_frags(dp, df);
             wgmma_fence();
-            mma_regs_x_tile(dq, df, sk);  // dQ += dS K
+            mma_regs_x_tile<kD>(dq, df, sk);  // dQ += dS K
             wgmma_commit();
             wgmma_wait<0>();
-            fence_regs<64>(dq);
+            fence_regs<kD / 2>(dq);
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(empty(s));
     }
-    store_acc(dq, p.dq + static_cast<int64_t>(row_base + qr0) * p.ld_dq, p.ld_dq, r_loc, kVarlen ? min(len - qr0, BS) : BS,
-              h * D, c_in, 1.f, 1.f);
+    store_acc<kD>(dq, p.dq + static_cast<int64_t>(row_base + qr0) * p.ld_dq, p.ld_dq, r_loc,
+                  kVarlen ? min(len - qr0, BS) : BS, h * kD, c_in, 1.f, 1.f);
 }
 
 // ---- launches ------------------------------------------------------------------------------------------------------------------
 // Dense: n_seq = B sequences of S rows, T = B * S.  Varlen: n_seq = n_docs documents at offsets cu[0..n_docs], S = the longest
 // document (it sizes the grid), T = cu[n_docs].  The tensor maps cover all T rows, so a tile that runs past a document reads
 // the next document's rows (masked in the kernels) or TMA zero fill past T.
+// head_dim is 64 or 128 (checked by the entry points); it picks the kernel instantiations and their shared-memory plan.
 template <bool kVarlen, bool kWindow>
-int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu, int n_seq, int S, int T, int Hq,
-               int Hkv, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols, int v_cols, float scale, int causal,
-               int window, cudaStream_t stream)
+int launch_fwd(int head_dim, const void* q, const void* k, const void* v, void* o, float* lse, const int* cu, int n_seq, int S,
+               int T, int Hq, int Hkv, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols, int v_cols, float scale,
+               int causal, int window, cudaStream_t stream)
 {
     CUtensorMap mq, mk, mv;
     int rc;
@@ -601,12 +631,14 @@ int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
     if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
     if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
     if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<kVarlen, kWindow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             kf::SM_TOTAL);
+    const bool d64 = head_dim == 64;
+    const auto kernel = d64 ? attn_fwd_kernel<64, kVarlen, kWindow> : attn_fwd_kernel<128, kVarlen, kWindow>;
+    const uint32_t smem = d64 ? kf<64>::SM_TOTAL : kf<128>::SM_TOTAL;
+    static bool attr[2] = {false, false};
+    if (!attr[d64]) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return static_cast<int>(e);
-        attr = true;
+        attr[d64] = true;
     }
     FwdParams p;
     p.o = static_cast<__nv_bfloat16*>(o);
@@ -621,16 +653,16 @@ int launch_fwd(const void* q, const void* k, const void* v, void* o, float* lse,
     p.T = T;
     p.window = kWindow ? min(window, S) : 0;  // a window of S rows or more masks nothing
     dim3 grid((S + BQ - 1) / BQ, Hq, n_seq);
-    attn_fwd_kernel<kVarlen, kWindow><<<grid, kThreads, kf::SM_TOTAL, stream>>>(mq, mk, mv, p);
+    kernel<<<grid, kThreads, smem, stream>>>(mq, mk, mv, p);
     DSB_CHECK_LAUNCH();
     return 0;
 }
 
 template <bool kVarlen, bool kWindow>
-int launch_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse, void* dq,
-               void* dk, void* dv, float* work, const int* cu, int n_seq, int S, int T, int Hq, int Hkv, int ld_q, int ld_k,
-               int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols, int k_cols, int v_cols, float scale,
-               int causal, int window, cudaStream_t stream)
+int launch_bwd(int head_dim, const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+               void* dq, void* dk, void* dv, float* work, const int* cu, int n_seq, int S, int T, int Hq, int Hkv, int ld_q,
+               int ld_k, int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols, int k_cols, int v_cols,
+               float scale, int causal, int window, cudaStream_t stream)
 {
     CUtensorMap mq, mk, mv, mdo;
     int rc;
@@ -638,23 +670,26 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o, const
     if ((rc = make_map(&mq, q, rows, q_cols, ld_q, BS))) return rc;
     if ((rc = make_map(&mk, k, rows, k_cols, ld_k, BS))) return rc;
     if ((rc = make_map(&mv, v, rows, v_cols, ld_v, BS))) return rc;
-    if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * D, ld_do, BS))) return rc;
-    static bool attr = false;
-    if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(attn_bwd_dkdv_kernel<kVarlen, kWindow>,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize, kb::SM_TOTAL);
+    if ((rc = make_map(&mdo, d_o, rows, static_cast<uint64_t>(Hq) * head_dim, ld_do, BS))) return rc;
+    const bool d64 = head_dim == 64;
+    const auto dkdv = d64 ? attn_bwd_dkdv_kernel<64, kVarlen, kWindow> : attn_bwd_dkdv_kernel<128, kVarlen, kWindow>;
+    const auto dq_kernel = d64 ? attn_bwd_dq_kernel<64, kVarlen, kWindow> : attn_bwd_dq_kernel<128, kVarlen, kWindow>;
+    const auto prep = d64 ? attn_bwd_prep_kernel<64> : attn_bwd_prep_kernel<128>;
+    const uint32_t smem = d64 ? kb<64>::SM_TOTAL : kb<128>::SM_TOTAL;
+    static bool attr[2] = {false, false};
+    if (!attr[d64]) {
+        cudaError_t e = cudaFuncSetAttribute(dkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return static_cast<int>(e);
-        e = cudaFuncSetAttribute(attn_bwd_dq_kernel<kVarlen, kWindow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 kb::SM_TOTAL);
+        e = cudaFuncSetAttribute(dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         if (e != cudaSuccess) return static_cast<int>(e);
-        attr = true;
+        attr[d64] = true;
     }
     float* delta = work;
     float* lse2 = work + static_cast<int64_t>(T) * Hq;
     const int64_t prep_rows = static_cast<int64_t>(T) * Hq;
     // the varlen [Hq, T] statistics are the dense [B, Hq, S] layout with B = 1, S = T
     const int prep_b = kVarlen ? 1 : n_seq, prep_s = kVarlen ? T : S;
-    attn_bwd_prep_kernel<<<static_cast<unsigned>((prep_rows * 32 + 255) / 256), 256, 0, stream>>>(
+    prep<<<static_cast<unsigned>((prep_rows * 32 + 255) / 256), 256, 0, stream>>>(
         static_cast<const __nv_bfloat16*>(o), static_cast<const __nv_bfloat16*>(d_o), lse, delta, lse2, prep_b, prep_s, Hq,
         ld_o, ld_do);
     BwdParams p;
@@ -676,8 +711,8 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o, const
     p.T = T;
     p.window = kWindow ? min(window, S) : 0;  // a window of S rows or more masks nothing
     const int nx = (S + BQ - 1) / BQ;
-    attn_bwd_dkdv_kernel<kVarlen, kWindow><<<dim3(nx, Hkv, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
-    attn_bwd_dq_kernel<kVarlen, kWindow><<<dim3(nx, Hq, n_seq), kThreads, kb::SM_TOTAL, stream>>>(mq, mk, mv, mdo, p);
+    dkdv<<<dim3(nx, Hkv, n_seq), kThreads, smem, stream>>>(mq, mk, mv, mdo, p);
+    dq_kernel<<<dim3(nx, Hq, n_seq), kThreads, smem, stream>>>(mq, mk, mv, mdo, p);
     DSB_CHECK_LAUNCH();
     return 0;
 }
@@ -687,28 +722,28 @@ int launch_bwd(const void* q, const void* k, const void* v, const void* o, const
 
 using namespace dsb::attn;
 
-// q / k / v: 2-D bf16 tensors [B*S, *] (row stride ld_*), head `i` at columns [i*128, +128) -- for a packed QKV
-// projection output all three point into the same buffer.  o: [B*S, ld_o] (head h at h*128).  lse: fp32 [B, Hq, S] or null.
+// q / k / v: 2-D bf16 tensors [B*S, *] (row stride ld_*), head `i` at columns [i*head_dim, +head_dim) -- for a packed QKV
+// projection output all three point into the same buffer.  o: [B*S, ld_o] (head h at h*head_dim).  head_dim: 64 or 128.  lse: fp32 [B, Hq, S] or null.
 // window > 0: causal sliding-window attention, row i sees keys i - window < j <= i (flash-attn's window_size = (window - 1,
 // 0)); window <= 0: no window.  A window needs causal.
 DSB_EXPORT int dsb_attn_fwd_bf16(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int Hq,
                                  int Hkv, int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
                                  int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
-    if (head_dim != D || S <= 0 || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
+    if ((head_dim != 64 && head_dim != 128) || S <= 0 || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
     if (B > 1 && S % BQ) return -2;  // ragged lengths: one sequence per launch (rows of the next one would be read as keys)
     if (window > 0 && !causal) return -2;
     if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
          reinterpret_cast<uintptr_t>(o)) & 15)
         return -2;
     if (window > 0)
-        return launch_fwd<false, true>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
+        return launch_fwd<false, true>(head_dim, q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
                                        v_cols, scale, causal, window, stream);
-    return launch_fwd<false, false>(q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
+    return launch_fwd<false, false>(head_dim, q, k, v, o, lse, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols, k_cols,
                                     v_cols, scale, causal, 0, stream);
 }
 
-// Backward.  q/k/v as in the forward; o, d_o: [B*S, ld] with head h at h*128; lse from the forward.
+// Backward.  q/k/v as in the forward; o, d_o: [B*S, ld] with head h at h*head_dim; lse from the forward.
 // dq / dk / dv: 2-D outputs (may be column ranges of ONE packed buffer).  work: fp32 scratch of 2 * B * Hq * S elements.
 // window: the forward's.
 DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
@@ -716,12 +751,12 @@ DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, co
                                  int ld_q, int ld_k, int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
                                  int k_cols, int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
-    if (head_dim != D || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
+    if ((head_dim != 64 && head_dim != 128) || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
     if (window > 0 && !causal) return -2;
     if (window > 0)
-        return launch_bwd<false, true>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
+        return launch_bwd<false, true>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
                                        ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, window, stream);
-    return launch_bwd<false, false>(q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
+    return launch_bwd<false, false>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
                                     ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, 0, stream);
 }
 
@@ -734,7 +769,7 @@ DSB_EXPORT int dsb_attn_varlen_fwd_bf16(const void* q, const void* k, const void
                                         int head_dim, int ld_q, int ld_k, int ld_v, int ld_o, int q_cols, int k_cols,
                                         int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
-    if (head_dim != D || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
+    if ((head_dim != 64 && head_dim != 128) || Hq % Hkv || ld_q % 8 || ld_k % 8 || ld_v % 8 || ld_o % 8) return -2;
     if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
     if (window > 0 && !causal) return -2;
     if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
@@ -742,9 +777,9 @@ DSB_EXPORT int dsb_attn_varlen_fwd_bf16(const void* q, const void* k, const void
         return -2;
     if (T == 0 || n_docs == 0) return 0;
     if (window > 0)
-        return launch_fwd<true, true>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o,
+        return launch_fwd<true, true>(head_dim, q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o,
                                       q_cols, k_cols, v_cols, scale, causal, window, stream);
-    return launch_fwd<true, false>(q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols,
+    return launch_fwd<true, false>(head_dim, q, k, v, o, lse, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q, ld_k, ld_v, ld_o, q_cols,
                                    k_cols, v_cols, scale, causal, 0, stream);
 }
 
@@ -756,15 +791,15 @@ DSB_EXPORT int dsb_attn_varlen_bwd_bf16(const void* q, const void* k, const void
                                         int ld_v, int ld_o, int ld_do, int ld_dq, int ld_dk, int ld_dv, int q_cols,
                                         int k_cols, int v_cols, float scale, int causal, int window, cudaStream_t stream)
 {
-    if (head_dim != D || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
+    if ((head_dim != 64 && head_dim != 128) || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
     if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
     if (window > 0 && !causal) return -2;
     if (T == 0 || n_docs == 0) return 0;
     if (window > 0)
-        return launch_bwd<true, true>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
+        return launch_bwd<true, true>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
                                       ld_k, ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal,
                                       window, stream);
-    return launch_bwd<true, false>(q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
+    return launch_bwd<true, false>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,
                                    ld_k, ld_v, ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, 0,
                                    stream);
 }

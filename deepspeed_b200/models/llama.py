@@ -92,6 +92,12 @@ PRESETS = {
     # state fits one 80 GB card
     "llama3.2-3b": dict(vocab_size=128256, hidden_size=3072, intermediate_size=8192, num_hidden_layers=28,
                         num_attention_heads=24, num_key_value_heads=8, rope_theta=500000.0, max_position_embeddings=8192),
+    # Llama-3.2-1B as published (head dim 64, tied LM head, llama3 RoPE scaling)
+    "llama3.2-1b": dict(vocab_size=128256, hidden_size=2048, intermediate_size=8192, num_hidden_layers=16,
+                        num_attention_heads=32, num_key_value_heads=8, head_dim=64, tie_word_embeddings=True,
+                        rope_theta=500000.0, max_position_embeddings=131072,
+                        rope_scaling={"rope_type": "llama3", "factor": 32.0, "low_freq_factor": 1.0,
+                                      "high_freq_factor": 4.0, "original_max_position_embeddings": 8192}),
     "llama3-8b": dict(vocab_size=128256, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                       num_attention_heads=32, num_key_value_heads=8, rope_theta=500000.0, max_position_embeddings=8192),
     "llama3-70b": dict(vocab_size=128256, hidden_size=8192, intermediate_size=28672, num_hidden_layers=80,

@@ -8,15 +8,15 @@ Attention-core backends (``backend=`` or ``DSB200_ATTN``):
   * ``cudnn`` / ``flash`` / ``efficient`` / ``math`` -- ``torch.nn.functional.scaled_dot_product_attention``
     with that SDPA backend (library path; cuDNN has a Hopper FMHA);
   * ``flash_attn`` -- the flash-attn package;
-  * ``native`` -- the framework's own sm_90a kernel (``csrc/cuda/attn_sm90.cu``) when built;
+  * ``native`` -- the framework's own sm_90a kernel (``csrc/cuda/attn_sm90.cu``, bf16, head dim 64 or 128) when built;
   * ``auto`` -- native if available, else cudnn -> flash -> efficient -> math priority order.
 Packed sequences (``cu_seqlens=``): the ``B*S`` token rows hold several documents at offsets ``cu_seqlens`` and every token
 attends only within its own document (flash-attn's varlen semantics).  ``auto`` / ``native`` run the in-tree varlen
-kernel; any other backend, dtype, head dim or a CPU tensor runs one SDPA call per document.
+kernel; any other backend, dtype, a head dim other than 64 or 128, or a CPU tensor runs one SDPA call per document.
 Sliding window (``sliding_window=W``, an int >= 1): query row ``i`` attends to key ``j`` only when ``i - W < j <= i`` -- W keys
 counting its own position (HF's ``sliding_window``, flash-attn's ``window_size=(W - 1, 0)``), measured inside each document
-with ``cu_seqlens``.  ``auto`` / ``native`` run the in-tree windowed kernel, which skips the tiles outside the band; every
-other case runs SDPA with an explicit boolean band mask per sequence or document.  A window that covers the whole sequence
+with ``cu_seqlens``.  ``auto`` / ``native`` run the in-tree windowed kernel (head dim 64 or 128), which skips the tiles
+outside the band; every other case runs SDPA with an explicit boolean band mask per sequence or document.  A window that covers the whole sequence
 (or the longest document) is dropped, so such a call is exactly the unwindowed one.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
@@ -272,12 +272,12 @@ def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_
                 return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions, window)
             if rope is not None:
                 rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
-            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv)
+            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
             return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False,
-                                              window=window)[0]
+                                              window=window, head_dim=d)[0]
     if backend == "native":
         raise RuntimeError("native varlen attention kernel requested but unsupported for this input (needs a CUDA bf16 "
-                           "tensor, head dim 128, 16-byte aligned rows)")
+                           "tensor, head dim 64 or 128, 16-byte aligned rows)")
     return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend, sliding_window=window)
 
 
@@ -302,11 +302,12 @@ def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend
                 return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions, window)
             if rope is not None:
                 rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)
-            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv)
-            return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False, window=window)[0]
+            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
+            return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False, window=window,
+                                       head_dim=d)[0]
         if backend == "native":
-            raise RuntimeError("native attention kernel requested but unsupported for this shape (needs bf16, head dim 128, "
-                               "sequence length a multiple of 128)")
+            raise RuntimeError("native attention kernel requested but unsupported for this shape (needs bf16, head dim 64 "
+                               "or 128, sequence length a multiple of 128)")
     if not (torch.is_grad_enabled() and qkv2d.requires_grad):
         if rope is not None:
             rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)

@@ -18,9 +18,10 @@ ap.add_argument("--B", type=int, default=2)
 ap.add_argument("--S", type=int, default=4096)
 ap.add_argument("--hq", type=int, default=32)
 ap.add_argument("--hkv", type=int, default=8)
+ap.add_argument("--head-dim", type=int, default=128, choices=(64, 128))
 ap.add_argument("--out", default="gpurun_out/attention_bench.json")
 a = ap.parse_args()
-B, S, hq, hkv, d = a.B, a.S, a.hq, a.hkv, 128
+B, S, hq, hkv, d = a.B, a.S, a.hq, a.hkv, a.head_dim
 bufs = [torch.randn(B * S, (hq + 2 * hkv) * d, device="cuda", dtype=torch.bfloat16) for _ in range(4)]
 flops_fwd = 4.0 * B * hq * S * S * d * 0.5  # causal
 
@@ -39,8 +40,8 @@ def timeit(fn, n=20):
 
 
 def own_fwd(i):
-    q, k, v = A.split_packed(bufs[i % 4], hq, hkv)
-    return A.fwd(q, k, v, B, S, hq, hkv, causal=True)
+    q, k, v = A.split_packed(bufs[i % 4], hq, hkv, d)
+    return A.fwd(q, k, v, B, S, hq, hkv, causal=True, head_dim=d)
 
 
 def lib_fwd(i, backend=SDPBackend.CUDNN_ATTENTION):
@@ -65,10 +66,10 @@ for name, be in (("cudnn", SDPBackend.CUDNN_ATTENTION), ("flash", SDPBackend.FLA
 if hasattr(A, "bwd"):
     try:
         x = bufs[0]
-        q, k, v = A.split_packed(x, hq, hkv)
-        o, lse = A.fwd(q, k, v, B, S, hq, hkv, causal=True)
+        q, k, v = A.split_packed(x, hq, hkv, d)
+        o, lse = A.fwd(q, k, v, B, S, hq, hkv, causal=True, head_dim=d)
         do = torch.randn_like(o)
-        t = timeit(lambda i: A.bwd(do, q, k, v, o, lse, B, S, hq, hkv, causal=True))
+        t = timeit(lambda i: A.bwd(do, q, k, v, o, lse, B, S, hq, hkv, causal=True, head_dim=d))
         res["own_bwd_ms"], res["own_bwd_tflops"] = t, 2.5 * flops_fwd / t / 1e9
     except Exception as ex:  # noqa
         res["own_bwd_ms"] = f"failed: {type(ex).__name__}: {ex}"

@@ -27,6 +27,7 @@ ap.add_argument("--rows", type=int, default=2)
 ap.add_argument("--row-len", type=int, default=4096)
 ap.add_argument("--hq", type=int, default=24)
 ap.add_argument("--hkv", type=int, default=8)
+ap.add_argument("--head-dim", type=int, default=128, choices=(64, 128))
 ap.add_argument("--min-len", type=int, default=16)
 ap.add_argument("--max-len", type=int, default=4096)
 ap.add_argument("--seed", type=int, default=0)
@@ -35,7 +36,7 @@ ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "packed_att
                 help="directory the JSON result is written to")
 a = ap.parse_args()
 
-d = 128
+d = a.head_dim
 hq, hkv = a.hq, a.hkv
 rng = np.random.default_rng(a.seed)
 lens = []
@@ -71,14 +72,14 @@ def timeit(fn, n=a.iters):
 
 
 def native_fwd(i):
-    q, k, v = A.split_packed(bufs[i % 4], hq, hkv)
-    return A.fwd_varlen(q, k, v, cu, max_len, hq, hkv, causal=True)
+    q, k, v = A.split_packed(bufs[i % 4], hq, hkv, d)
+    return A.fwd_varlen(q, k, v, cu, max_len, hq, hkv, causal=True, head_dim=d)
 
 
 def native_fwd_bwd(i):
-    q, k, v = A.split_packed(bufs[i % 4], hq, hkv)
-    o, lse = A.fwd_varlen(q, k, v, cu, max_len, hq, hkv, causal=True)
-    A.bwd_varlen(d_o, q, k, v, o, lse, cu, max_len, hq, hkv, causal=True)
+    q, k, v = A.split_packed(bufs[i % 4], hq, hkv, d)
+    o, lse = A.fwd_varlen(q, k, v, cu, max_len, hq, hkv, causal=True, head_dim=d)
+    A.bwd_varlen(d_o, q, k, v, o, lse, cu, max_len, hq, hkv, causal=True, head_dim=d)
 
 
 def _heads(x2d, rows, S):

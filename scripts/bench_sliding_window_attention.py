@@ -30,12 +30,13 @@ ap.add_argument("--seq", type=int, nargs="+", default=[4096, 8192, 16384, 32768]
 ap.add_argument("--window", type=int, default=4096)
 ap.add_argument("--hq", type=int, default=32)
 ap.add_argument("--hkv", type=int, default=8)
+ap.add_argument("--head-dim", type=int, default=128, choices=(64, 128))
 ap.add_argument("--iters", type=int, default=10)
 ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "sliding_window_attention"),
                 help="directory the JSON result is written to")
 a = ap.parse_args()
 
-d = 128
+d = a.head_dim
 hq, hkv, W = a.hq, a.hkv, a.window
 
 
@@ -75,13 +76,13 @@ def run_shape(S):
     def native(window):
 
         def fwd(i):
-            q, k, v = A.split_packed(bufs[i % 4], hq, hkv)
-            return A.fwd(q, k, v, 1, S, hq, hkv, causal=True, window=window)
+            q, k, v = A.split_packed(bufs[i % 4], hq, hkv, d)
+            return A.fwd(q, k, v, 1, S, hq, hkv, causal=True, window=window, head_dim=d)
 
         def fwd_bwd(i):
-            q, k, v = A.split_packed(bufs[i % 4], hq, hkv)
-            o, lse = A.fwd(q, k, v, 1, S, hq, hkv, causal=True, window=window)
-            A.bwd(d_o, q, k, v, o, lse, 1, S, hq, hkv, causal=True, window=window)
+            q, k, v = A.split_packed(bufs[i % 4], hq, hkv, d)
+            o, lse = A.fwd(q, k, v, 1, S, hq, hkv, causal=True, window=window, head_dim=d)
+            A.bwd(d_o, q, k, v, o, lse, 1, S, hq, hkv, causal=True, window=window, head_dim=d)
 
         return fwd, fwd_bwd
 
