@@ -106,8 +106,9 @@ def _own_available():
 
 
 def _eligible(M, N, K, *tensors):
-    """Own-kernel preconditions: bf16 CUDA row-major operands with 16-byte aligned rows, at least one 256x128 tile."""
-    if _backend == "lib" or M < 256 or N < 128 or K < 64:
+    """Own-kernel preconditions: bf16 CUDA row-major operands with 16-byte aligned rows, N % 8 == 0 (the kernel's
+    16-byte column pairs; ``matmul_nt`` without ``out`` has no tensor whose rows are N long), at least one 256x128 tile."""
+    if _backend == "lib" or M < 256 or N < 128 or K < 64 or N % 8:
         return False
     for t in tensors:
         if t is None:

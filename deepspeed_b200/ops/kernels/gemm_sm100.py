@@ -9,9 +9,11 @@ _checked = None
 
 
 def supports(a, b, nt=True) -> bool:
-    """bf16, 2-D, K-major operands (``a`` [M,K], ``b`` [N,K] when ``nt``), K % 8 == 0, 16-byte aligned rows."""
+    """Whether :func:`matmul_nt` takes these operands: bf16, 2-D, K-major (``a`` [M,K], ``b`` [N,K]), K % 8 == 0,
+    16-byte aligned rows.  Only the NT form is answered here (``nt=False`` is always False); MN-major operands (NN / TN)
+    go through :func:`matmul_2cta`, whose preconditions :func:`supports_2cta` checks."""
     if not nt:
-        return False  # NN / TN use the library path until the MN-major descriptors land
+        return False
     if a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16 or a.dim() != 2 or b.dim() != 2:
         return False
     if a.stride(1) != 1 or b.stride(1) != 1 or a.shape[1] != b.shape[1]:

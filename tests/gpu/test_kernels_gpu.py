@@ -269,29 +269,19 @@ def test_gated_act_fwd_bwd(act, dtype):
 def test_swiglu_raw_at_step_shape(tokens, inter):
     """``gated_act_fwd_raw`` / ``gated_act_bwd`` (the kernels behind the library SwiGLU GEMMs) against float64, per element."""
     from deepspeed_b200.ops.kernels import transformer_ops as T
-    from tests.numerics import U, assert_within, ulp
+    from tests.numerics import assert_within, dswiglu_reference, swiglu_reference
     g = torch.Generator(device="cuda").manual_seed(0)
     gu = (torch.randn(tokens, 2 * inter, generator=g, device="cuda") * 2).bfloat16()
     dout = torch.randn(tokens, inter, generator=g, device="cuda").bfloat16()
     out = T.gated_act_fwd_raw(gu)
     dgu = T.gated_act_bwd(dout, gu)
-    x, u, d = gu[:, :inter].double(), gu[:, inter:].double(), dout.double()
-    s = torch.sigmoid(x)
-    silu = x * s
-    inner = 1 + x * (1 - s)
-    # silu = x / (1 + __expf(-x)): __expf is exact to 2 ulp plus |x| U, the add and the IEEE divide round once each, so
-    # sigmoid and silu carry (|x| + 6) U relative; every further product rounds once
-    s_err = s * (x.abs() + 6) * U
-    ref = silu * u
-    assert_within(out, ref, ulp(ref, torch.bfloat16) + (x.abs() + 8) * U * ref.abs(), "silu(gate) * up")
-    # d(gate) = (d * up) * s * (1 + x * (1 - s)): d * up is exact in fp32; s's error enters through s and 1 - s
-    dact = s * inner
-    dact_err = s_err * (inner.abs() + s * x.abs()) + s * U * (2 * x.abs() * (1 - s).abs() + inner.abs()) + U * dact.abs()
-    dgate = d * u * dact
-    assert_within(dgu[:, :inter], dgate, ulp(dgate, torch.bfloat16) + (d * u).abs() * (dact_err + U * dact.abs()),
-                  "d(gate)")
-    dup = d * silu
-    assert_within(dgu[:, inter:], dup, ulp(dup, torch.bfloat16) + (x.abs() + 8) * U * dup.abs(), "d(up)")
+    ref, bound = swiglu_reference(gu[:, :inter], gu[:, inter:])
+    assert_within(out, ref, bound, "silu(gate) * up")
+    del ref, bound
+    # dout is bf16, so dout * up is exact in fp32
+    dgate, dgate_bound, dup, dup_bound = dswiglu_reference(dout, gu[:, :inter], gu[:, inter:])
+    assert_within(dgu[:, :inter], dgate, dgate_bound, "d(gate)")
+    assert_within(dgu[:, inter:], dup, dup_bound, "d(up)")
 
 
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])

@@ -41,6 +41,163 @@ def assert_within(out, ref, bound, what):
                              f"+- {bound.reshape(-1)[k].item():.3g}")
 
 
+def assert_bits_equal(out, ref, what):
+    """``out`` and ``ref`` (same dtype) hold the same bit patterns, NaN payloads and signed zeros included."""
+    assert out.dtype == ref.dtype and out.shape == ref.shape, (what, out.dtype, ref.dtype, out.shape, ref.shape)
+    view = {2: torch.int16, 4: torch.int32, 8: torch.int64}[out.element_size()]
+    bad = out.contiguous().view(view) != ref.contiguous().view(view)
+    if bool(bad.any()):
+        k = int(bad.reshape(-1).nonzero()[0])
+        idx = tuple(int(i) for i in torch.unravel_index(torch.tensor(k), ref.shape))
+        raise AssertionError(f"{what}: {int(bad.sum())} of {ref.numel()} elements differ; first at {idx}: "
+                             f"got {out.reshape(-1)[k].item()!r}, want {ref.reshape(-1)[k].item()!r}")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# GEMM
+# ---------------------------------------------------------------------------------------------------------------------
+def exact_grid(rows, cols, gen, emin=-12, emax=12, ints=4):
+    """bf16 ``[rows, cols]``: integers in ``[-ints, ints]`` times ``2**e_r``, one exponent per row.  Returns
+    ``(tensor, e)`` with ``e`` the int32 exponents ``[rows]``.
+
+    Used as ``A [M, K]`` and ``B [N, K]`` of ``A @ B^T``, every term of the dot product of row i and column j is an integer
+    times ``2**(e_i + f_j)``.  While ``sum_k |a_ik| |b_jk| < 2**22`` (``16 K < 2**22``: any K up to 262143) every product
+    and every partial sum is exactly representable in fp32, so an fp32 accumulation is exact in any order and the
+    product rounds to bf16 exactly once.  Each row and column of C gets its own scale, so a value written to the wrong
+    row, column or tile cannot match."""
+    dev = gen.device
+    v = torch.randint(-ints, ints + 1, (rows, cols), generator=gen, device=dev, dtype=torch.int32).float()
+    e = torch.randint(emin, emax + 1, (rows, ), generator=gen, device=dev, dtype=torch.int32)
+    return torch.ldexp(v, e[:, None]).bfloat16(), e
+
+
+def exact_addend(e_rows, e_cols, gen, ints=128):
+    """bf16 ``C_old [M, N]`` on the grid of ``A @ B^T`` for row exponents ``e_rows`` of A and ``e_cols`` of B: integers in
+    ``[-ints, ints]`` (exact in bf16 up to 256) times ``2**(e_i + f_j)``, so ``C_old + A @ B^T`` stays exact in fp32."""
+    v = torch.randint(-ints, ints + 1, (e_rows.numel(), e_cols.numel()), generator=gen, device=gen.device,
+                      dtype=torch.int32).float()
+    return torch.ldexp(v, e_rows[:, None] + e_cols[None, :]).bfloat16()
+
+
+def _gemm_blocks(M, N, K, budget=2**24):
+    """Row and column blocks of an [M, N] product whose float64 operand and result blocks hold at most ``budget``
+    (or one 128-row / 128-column strip) elements each: 128 MB in float64, whatever the problem."""
+    cb = min(N, max(128, budget // max(K, 1)))
+    rb = min(M, max(128, min(budget // cb, budget // max(K, 1))))
+    for r in range(0, M, rb):
+        for c in range(0, N, cb):
+            yield slice(r, min(r + rb, M)), slice(c, min(c + cb, N))
+
+
+def gemm_reference(a, b, c_old=None, magnitudes=False):
+    """Float64 ``a @ b^T (+ c_old)`` block by block: yields ``(rows, cols, ref, mag)`` with ``mag = |a| @ |b|^T`` when
+    ``magnitudes`` else None.  ``a`` [M, K] and ``b`` [N, K] may be any strided views (transposes included)."""
+    M, K = a.shape
+    N = b.shape[0]
+    for rs, cs in _gemm_blocks(M, N, K):
+        a64, b64 = a[rs].double(), b[cs].double()
+        ref = a64 @ b64.t()
+        if c_old is not None:
+            ref += c_old[rs, cs].double()
+        mag = a64.abs() @ b64.abs().t() if magnitudes else None
+        del a64, b64
+        yield rs, cs, ref, mag
+
+
+def assert_gemm_exact(c, a, b, c_old=None, what="C"):
+    """``c`` is bit-equal to ``bf16(a @ b^T + c_old)`` rounded once from the exact sum; valid for :func:`exact_grid`
+    operands (and a ``c_old`` on the same grid), where that sum is exactly representable in fp32."""
+    for rs, cs, ref, _ in gemm_reference(a, b, c_old):
+        assert_bits_equal(c[rs, cs], ref.to(torch.bfloat16), f"{what}[{rs.start}:{rs.stop}, {cs.start}:{cs.stop}]")
+
+
+def gemm_accum_error(mag, K):
+    """Error of an fp32 accumulator that sums ``K`` bf16 products of magnitudes ``mag = |A| @ |B|^T``.
+
+    bf16 products are exact in fp32.  Summing K of them in any order, each add rounding to nearest, errs by at most
+    ``K U sum_k |a_k||b_k|`` (``U = 2**-24``); the tensor core's adder may truncate instead of rounding, which at most
+    doubles the per-add error, hence ``2 K U |A| |B|^T``.  An accumulation in any format with fewer than 23 fraction bits
+    cannot meet it."""
+    return 2 * K * U * mag
+
+
+def gemm_bound(ref, mag, K, c_old=None):
+    """Per-element bound on a bf16 GEMM output that accumulates ``K`` products in fp32 (:func:`gemm_accum_error`).
+    ``EPI_ACCUM`` adds ``c_old`` in fp32 (one more rounding, ``U`` times the sum) before the bf16 rounding, which costs
+    at most one :func:`ulp` of the computed value."""
+    acc = gemm_accum_error(mag, K)
+    if c_old is not None:
+        acc = acc + U * (ref.abs() + acc)
+    return ulp(ref.abs() + acc, torch.bfloat16) + acc
+
+
+def assert_gemm_bounded(c, a, b, c_old=None, what="C"):
+    """``|c - (a @ b^T + c_old)| <= gemm_bound`` element by element, in float64."""
+    K = a.shape[1]
+    for rs, cs, ref, mag in gemm_reference(a, b, c_old, magnitudes=True):
+        assert_within(c[rs, cs], ref, gemm_bound(ref, mag, K, c_old), f"{what}[{rs.start}:{rs.stop}, {cs.start}:{cs.stop}]")
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# SwiGLU
+# ---------------------------------------------------------------------------------------------------------------------
+SILU_LIP = 1.1  # max |silu'(x)| = 1.0998...: silu moves by at most 1.1 |dx|
+
+
+def swiglu_reference(g, u, g_err=0.0, u_err=0.0):
+    """Float64 ``act = silu(g) * u`` and its bound for a kernel that forms ``silu(g) = g / (1 + __expf(-g))`` in fp32 from
+    fp32 inputs within ``g_err`` / ``u_err`` of ``g`` / ``u``, multiplies once and rounds to bf16.
+
+    ``__expf`` is exact to 2 ulp plus ``|g| U`` from rounding its scaled argument; the add and the IEEE divide round once
+    each, so silu carries ``(|g| + 6) U`` relative error and the product one more ``U``.  Below ``g = -80`` ``__expf(-g)``
+    may overflow and the kernel writes 0, which is within ``|act|`` of the truth.  An input error moves ``act`` by at most
+    ``1.1 g_err (|u| + u_err) + |silu(g)| u_err``.
+
+    Which ``g`` and ``u`` to pass depends on the path.  The fused GEMM epilogue applies silu to the fp32 accumulators: pass
+    the float64 sums, with the accumulation bound (:func:`gemm_bound` without its final rounding) as the input error, or
+    none on :func:`exact_grid` data, where the accumulators are exact.  The library path applies silu to the gate|up it
+    stored in bf16: pass those bf16 values, which is what it read, without an input error.  Measured against the float64
+    sums instead, the library path would need an extra ``ulp(g) / 2`` and ``ulp(u) / 2`` of input error for that
+    rounding, so its bound is looser than the fused epilogue's."""
+    g, u = g.double(), u.double()
+    silu = g * torch.sigmoid(g)
+    act = silu * u
+    moved = SILU_LIP * g_err * (u.abs() + u_err) + silu.abs() * u_err
+    mag = act.abs() + moved
+    bound = ulp(mag, torch.bfloat16) + moved + (g.abs() + g_err + 8) * U * mag + torch.where(g < -80, mag, 0.0)
+    return act, bound
+
+
+def dswiglu_reference(d, g, u, d_fp32=False, d_err=0.0):
+    """Float64 ``(dgate, dup)`` of ``act = silu(g) * u`` for the upstream gradient ``d``, and their bounds for a kernel
+    that computes ``dgate = (d * u) * s (1 + g (1 - s))`` and ``dup = d * silu(g)`` in fp32 (``s = 1 / (1 + __expf(-g))``,
+    silu as in :func:`swiglu_reference`) from bf16 ``g`` and ``u`` and rounds each to bf16.  Returns
+    ``(dgate, dgate_bound, dup, dup_bound)``.
+
+    With ``d`` in bf16 the product ``d * u`` is exact in fp32 (8 x 8 significant bits).  ``d_fp32=True`` is the dSwiGLU
+    GEMM epilogue, whose ``d`` is an fp32 accumulator: ``d * u`` then rounds once, one more ``U |dgate|``; ``d_err`` is
+    that accumulator's error, which the two products carry as ``|u dsilu(g)| d_err`` and ``|silu(g)| d_err``."""
+    d, g, u = d.double(), g.double(), u.double()
+    s = torch.sigmoid(g)
+    silu = g * s
+    inner = 1 + g * (1 - s)
+    s_err = s * (g.abs() + 6) * U  # sigmoid carries (|g| + 6) U relative, as silu does
+    dact = s * inner
+    # s's error enters through s and 1 - s; the products of s (1 + g (1 - s)) round once each
+    dact_err = s_err * (inner.abs() + s * g.abs()) + s * U * (2 * g.abs() * (1 - s).abs() + inner.abs()) + U * dact.abs()
+    dgate = d * u * dact
+    moved = (u * dact).abs() * d_err
+    mag = dgate.abs() + moved
+    dgate_bound = ulp(mag, torch.bfloat16) + moved + ((d.abs() + d_err) * u.abs()) * (dact_err + U * dact.abs())
+    if d_fp32:
+        dgate_bound = dgate_bound + U * mag
+    dup = d * silu
+    moved = silu.abs() * d_err
+    mag = dup.abs() + moved
+    dup_bound = ulp(mag, torch.bfloat16) + moved + (g.abs() + 8) * U * mag
+    return dgate, dgate_bound, dup, dup_bound
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # softmax cross entropy
 # ---------------------------------------------------------------------------------------------------------------------
