@@ -10,6 +10,8 @@
 //   * fused epilogues: plain store, accumulate into C (dW over micro-batches), SwiGLU (gate and up rows of the same 128
 //     features share one tile), dSwiGLU
 //   * grouped (MoE) form: the tile list is built on the device from the expert offsets (no host synchronisation)
+//   * ragged (dropless MoE training) forms: the grouped form with every epilogue and an MN-major B whose expert offset
+//     lies on K, plus a variable-K weight-gradient form whose tile (expert, m, n) sums only its expert's rows
 //   * OPTIONAL fused all-gather: when `ag` is given, the weight matrix B is being assembled in local memory from the
 //     other ranks' ZeRO shards *by this same kernel*: `ag.comm_ctas` CTAs pull the peers' shard bytes over NVLink
 //     (peer-mapped addresses) chunk by chunk and publish a per-chunk ready flag (st.release.gpu); the producer of each
@@ -178,7 +180,11 @@ static_assert(AG_BUFS * AG_PIECE + 8 * AG_BUFS <= SMEM_TOTAL, "all-gather ring m
 //              dgate = acc * up * silu'(gate) -> C (the [M, I] left half of dgate_up),  dup = acc * silu(gate) -> out2 + I.
 // (cuBLAS cannot express the last two: they remove one full pass over the [tokens, 2I] / [tokens, I] activations each.)
 enum : int { EPI_STORE = 0, EPI_ACCUM = 1, EPI_SWIGLU = 2, EPI_DSWIGLU = 3 };
-enum : int { MODE_PLAIN = 0, MODE_GROUPED = 1, MODE_ALLGATHER = 2 };
+// MODE_GROUPED    m-tiles per expert over expert-sorted rows, K-major B [E, N, K] (inference, offsets trusted)
+// MODE_RAGGED     MODE_GROUPED for training: 64-row aligned segments, checked offsets, SwiGLU / dSwiGLU epilogues and an
+//                 MN-major B [E, K, N] (the expert's slab starts at K coordinate e * K)
+// MODE_RAGGED_K   dW[e] = A_e^T B_e over the rows of expert e only: tiles (e, m, n), k-blocks [off[e] / 64, off[e+1] / 64)
+enum : int { MODE_PLAIN = 0, MODE_GROUPED = 1, MODE_ALLGATHER = 2, MODE_RAGGED = 3, MODE_RAGGED_K = 4 };
 
 struct EpiParams {
     const __nv_bfloat16* aux;  // DSWIGLU: saved gate|up
@@ -222,20 +228,44 @@ __device__ __forceinline__ void st_bf16x2(__nv_bfloat16* p, float lo, float hi)
 }
 
 // Where one tile lives: first row of A / C, rows of C it may write, first B row of each half of the B tile (K-major B:
-// each half is two 64-row boxes), first C column (MN-major B: also the first B column).
+// each half is two 64-row boxes), first C column (MN-major B: also the first B column).  Ragged forms only: k0 is added
+// to the K coordinate of the MN-major operands' loads, nk is the tile's k-block count and crow0 its first C row.
 struct Tile {
     int row0, rows, b0, b1, col0;
+    int k0, nk, crow0;
 };
+
+// Ragged forms: offsets[0..E] must be non-decreasing multiples of 64 inside [0, rows].  Anything else could send a TMA
+// load into another expert's K rows or a store past the output, so the kernel refuses it before it does anything.
+// kPrefix (m-tiled form): the same pass fills prefix[1..E] with the running count of (m-tile x nn n-tiles).
+template <bool kPrefix>
+__device__ __forceinline__ bool ragged_walk(const int* off, int E, int rows, int nn, int* prefix)
+{
+    int prev = off[0];
+    if (prev < 0 || (prev & (BK - 1))) return false;
+    int acc = 0;
+    for (int e = 1; e <= E; ++e) {
+        const int cur = off[e];
+        if (cur < prev || (cur & (BK - 1))) return false;
+        if (kPrefix) {
+            acc += ((cur - prev + BM - 1) / BM) * nn;
+            prefix[e] = acc;
+        }
+        prev = cur;
+    }
+    return prev <= rows;
+}
 
 template <int EPI, int MODE>
 struct Sched {
+    static constexpr bool kGrouped = MODE == MODE_GROUPED || MODE == MODE_RAGGED;  // m-tiles per expert
     static constexpr int TN = (EPI == EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
-    int num_m, num_n, num_tiles, group_m, n_rot, M, N;
+    int num_m, num_n, num_tiles, group_m, n_rot, M, N, K;
     const int* offsets;
     const int* prefix;  // grouped: tile_prefix in shared memory
     int e;              // grouped: current expert (tiles are visited in increasing order)
 
-    __device__ void init(const EpiParams& ep, const AgParams& ag, int M_, int N_, int K, const int* pre)
+    __device__ void init(const EpiParams& ep, const AgParams& ag, int M_, int N_, int K_, const int* pre)
     {
         M = M_;
         N = N_;
@@ -244,10 +274,15 @@ struct Sched {
         prefix = pre;
         e = 0;
         n_rot = 0;
-        if (MODE == MODE_GROUPED) {
+        if (MODE == MODE_RAGGED) K = K_;
+        if (kGrouped) {
             num_m = 0;
             num_tiles = pre[ep.E];
             group_m = 1;
+        } else if (MODE == MODE_RAGGED_K) {
+            num_m = (M + BM - 1) / BM;
+            num_tiles = ep.E * num_m * num_n;
+            group_m = num_m;
         } else {
             num_m = (M + BM - 1) / BM;
             num_tiles = num_m * num_n;
@@ -256,7 +291,7 @@ struct Sched {
         if (MODE == MODE_ALLGATHER) {
             // n-blocks are visited starting at the locally owned rows
             const int64_t own_lo = static_cast<int64_t>(ag.rank) * ag.shard_bytes - ag.b_offset_bytes;
-            int64_t row = own_lo > 0 ? (own_lo + static_cast<int64_t>(K) * 2 - 1) / (static_cast<int64_t>(K) * 2) : 0;
+            int64_t row = own_lo > 0 ? (own_lo + static_cast<int64_t>(K_) * 2 - 1) / (static_cast<int64_t>(K_) * 2) : 0;
             n_rot = static_cast<int>((row + BN - 1) / BN) % num_n;
         }
     }
@@ -264,7 +299,7 @@ struct Sched {
     {
         Tile t;
         int m_blk, n_blk;
-        if (MODE == MODE_GROUPED) {
+        if (kGrouped) {
             while (tile >= prefix[e + 1]) ++e;
             const int lo = offsets[e], cnt = offsets[e + 1] - lo;
             const int nm = (cnt + BM - 1) / BM;
@@ -274,8 +309,29 @@ struct Sched {
             t.row0 = lo + m_blk * BM;
             t.rows = cnt - m_blk * BM;
             t.col0 = n_blk * TN;
-            t.b0 = e * N + t.col0;
-            t.b1 = t.b0 + BN / 2;
+            if (MODE == MODE_RAGGED && EPI == EPI_SWIGLU) {
+                // w13 [E, 2I, K]: the expert's gate rows, then its up rows
+                t.b0 = e * 2 * inter + t.col0;
+                t.b1 = t.b0 + inter;
+            } else {
+                t.b0 = e * N + t.col0;
+                t.b1 = t.b0 + BN / 2;
+            }
+            if (MODE == MODE_RAGGED) t.k0 = e * K;  // MN-major B [E, K, N]
+            return t;
+        }
+        if (MODE == MODE_RAGGED_K) {
+            const int per_e = num_m * num_n;
+            e = tile / per_e;
+            const int local = tile - e * per_e;
+            m_blk = local % num_m;
+            n_blk = local / num_m;
+            t.row0 = m_blk * BM;
+            t.rows = M - t.row0;
+            t.col0 = n_blk * BN;
+            t.crow0 = e * M + t.row0;
+            t.k0 = offsets[e];
+            t.nk = (offsets[e + 1] - t.k0) / BK;
             return t;
         }
         tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
@@ -312,6 +368,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         return;
     }
 
+    if constexpr (MODE == MODE_RAGGED || MODE == MODE_RAGGED_K) {
+        // one pass over the offsets checks them (and, m-tiled, builds the tile prefix); tile_prefix[0] is 0 when they are
+        // well formed, -1 when not -- then the whole CTA leaves before any barrier exists and writes nothing
+        if (threadIdx.x == kConsumerThreads) {
+            const int nn = (N + Sched<EPI, MODE>::TN - 1) / Sched<EPI, MODE>::TN;
+            tile_prefix[0] = ragged_walk<MODE == MODE_RAGGED>(ep.offsets, ep.E, MODE == MODE_RAGGED ? M : K, nn, tile_prefix)
+                                 ? 0
+                                 : -1;
+        }
+        __syncthreads();
+        if (tile_prefix[0] != 0) return;
+    }
+
     if (threadIdx.x == kConsumerThreads) {
         prefetch_map(&map_a);
         prefetch_map(&map_b);
@@ -346,22 +415,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
             for (int tile = blockIdx.x; tile < sch.num_tiles; tile += mma_ctas) {
                 const Tile t = sch.at(tile, ep.inter);
                 if (MODE == MODE_ALLGATHER) ag_wait_rows(ag, t.col0, (N - t.col0) < BN ? (N - t.col0) : BN, K);
-                for (int kb = 0; kb < num_k; ++kb) {
+                const int nk = MODE == MODE_RAGGED_K ? t.nk : num_k;
+                for (int kb = 0; kb < nk; ++kb) {
                     mbar_wait(empty_bar(stage), phase ^ 1);
                     const uint32_t sa = sbase + stage * STAGE_BYTES, sb = sa + 2 * BOX;  // B: 4 boxes of 64 rows
                     const uint32_t fb = full_bar(stage);
                     mbar_expect_tx(fb, STAGE_BYTES);
+                    const int ka = kb * BK + (MODE == MODE_RAGGED_K ? t.k0 : 0);
+                    const int kbb = kb * BK + (MODE == MODE_RAGGED_K || (MODE == MODE_RAGGED && B_MN) ? t.k0 : 0);
                     if (A_MN) {
-                        tma_load_2d(sa, &map_a, fb, t.row0, kb * BK);
-                        tma_load_2d(sa + BOX, &map_a, fb, t.row0 + 64, kb * BK);
+                        tma_load_2d(sa, &map_a, fb, t.row0, ka);
+                        tma_load_2d(sa + BOX, &map_a, fb, t.row0 + 64, ka);
                     } else {
-                        tma_load_2d(sa, &map_a, fb, kb * BK, t.row0);
-                        tma_load_2d(sa + BOX, &map_a, fb, kb * BK, t.row0 + 64);
+                        tma_load_2d(sa, &map_a, fb, ka, t.row0);
+                        tma_load_2d(sa + BOX, &map_a, fb, ka, t.row0 + 64);
                     }
 #pragma unroll
                     for (int i = 0; i < 4; ++i) {
-                        if (B_MN) tma_load_2d(sb + i * BOX, &map_b, fb, t.col0 + 64 * i, kb * BK);
-                        else tma_load_2d(sb + i * BOX, &map_b, fb, kb * BK, (i < 2 ? t.b0 : t.b1) + 64 * (i & 1));
+                        if (B_MN) tma_load_2d(sb + i * BOX, &map_b, fb, t.col0 + 64 * i, kbb);
+                        else tma_load_2d(sb + i * BOX, &map_b, fb, kbb, (i < 2 ? t.b0 : t.b1) + 64 * (i & 1));
                     }
                     if (++stage == STAGES) {
                         stage = 0;
@@ -383,8 +455,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
     float acc[128];
     for (int tile = blockIdx.x; tile < sch.num_tiles; tile += mma_ctas) {
         const Tile t = sch.at(tile, ep.inter);
+        const int nk = MODE == MODE_RAGGED_K ? t.nk : num_k;
         int prev = -1;
-        for (int kb = 0; kb < num_k; ++kb) {
+        for (int kb = 0; kb < nk; ++kb) {
             mbar_wait(full_bar(stage), phase);
             const uint32_t sa = sbase + stage * STAGE_BYTES + wg * BOX, sb = sbase + stage * STAGE_BYTES + 2 * BOX;
             const uint64_t da = A_MN ? desc_mnmajor_sw128(sa, BOX) : desc_kmajor_sw128(sa);
@@ -408,13 +481,24 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         wgmma_wait<0>();
         fence_regs<128>(acc);
         if (prev >= 0 && lane == 0) mbar_arrive(empty_bar(prev));
+        if constexpr (MODE == MODE_RAGGED_K) {
+            // an expert without rows: no wgmma initialised the accumulators; its dW is zero (STORE) or unchanged (ACCUM)
+            if (nk == 0) {
+                if constexpr (EPI == EPI_ACCUM) {
+                    continue;
+                } else {
+#pragma unroll
+                    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+                }
+            }
+        }
 
         // ---- epilogue straight from the accumulators: thread holds rows r_in (+8), column pairs c_in + 8 j ----
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const int lr = r_in + 8 * i;
             if (lr >= t.rows || lr >= BM) continue;
-            const int64_t grow = static_cast<int64_t>(t.row0 + lr);
+            const int64_t grow = static_cast<int64_t>((MODE == MODE_RAGGED_K ? t.crow0 : t.row0) + lr);
             if constexpr (EPI == EPI_SWIGLU) {
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -635,6 +719,99 @@ DSB_EXPORT int dsb_gemm_grouped_nt_bf16(const void* a, const void* w, void* c, c
     const int64_t max_tiles = (static_cast<int64_t>(rows + BM - 1) / BM + E) * ((N + BN - 1) / BN);
     if (grid > max_tiles) grid = static_cast<int>(max_tiles);
     return launch_kernel<false, false, EPI_STORE, MODE_GROUPED>(ma, mb, rows, N, K, grid, ep, ag, stream);
+}
+
+// ---- ragged (dropless MoE training) forms ---------------------------------------------------------------------------
+// Rows are sorted by expert: expert e owns rows [offsets[e], offsets[e+1]) of every [rows, *] operand; offsets is int32
+// [E + 1] ON THE DEVICE (no host synchronisation).  Contract, for both entry points:
+//   * segments are 64-row aligned and zero-padded: every offset is a multiple of 64 and the rows of a segment past its
+//     expert's true token count are zero.  The variable-K form then reads only its expert's rows and the padding adds
+//     exact zeros; the m-tiled forms write the padding rows like any other (SwiGLU(0) = 0, so they stay zero);
+//   * rows outside [offsets[0], offsets[E]) are neither read into a result nor written;
+//   * malformed device offsets -- decreasing, not multiples of 64, negative or past `rows` -- are not launched into: every
+//     CTA checks the whole table first and, if it is malformed, exits before it initialises a barrier, writing nothing;
+//   * host-checked (-2, nothing launched): 1 <= E <= 256, K % 64 == 0, N % 8 == 0 (SwiGLU / dSwiGLU: N = inter and
+//     N % 128 == 0), row strides % 8, 16-byte aligned pointers.
+
+// m-tiled ragged GEMM: for each expert e and its rows r,
+//   b_mn == 0:  b = w [E, Nb, K] (K-major), epi STORE: c[r] = a[r] w[e]^T with Nb = N;
+//               epi SWIGLU: Nb = 2N (gate rows, then up rows), c [rows, N] = silu(gate) * up, out2 = gate|up (nullable)
+//   b_mn == 1:  b = w [E, K, N] (MN-major), epi STORE: c[r] = a[r] w[e];
+//               epi DSWIGLU: aux = saved gate|up [rows, 2N], c = out2 = dgate|dup [rows, 2N] (c the left half)
+// a [rows, K] (lda), c [rows, N] (ldc).
+DSB_EXPORT int dsb_gemm_ragged_bf16(const void* a, const void* b, void* c, const int* offsets, int rows, int E, int N, int K,
+                                    int lda, int ldc, int b_mn, int epi, const void* aux, int ld_aux, void* out2, int ld_out2,
+                                    int sms, cudaStream_t stream)
+{
+    if (rows < 0 || E < 1 || E > kMaxGroups || N <= 0 || K <= 0 || K % BK || N % 8 || lda % 8 || ldc % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
+         reinterpret_cast<uintptr_t>(aux) | reinterpret_cast<uintptr_t>(out2)) & 15)
+        return -2;
+    const bool fused = epi == EPI_SWIGLU || epi == EPI_DSWIGLU;
+    if (epi == EPI_ACCUM || epi < 0 || epi > 3 || (fused && N % (BN / 2))) return -2;
+    if (epi == EPI_SWIGLU && (b_mn || (out2 && ld_out2 % 8))) return -2;
+    if (epi == EPI_DSWIGLU && (!b_mn || !aux || !out2 || ld_aux % 8 || ld_out2 % 8)) return -2;
+    if (offsets == nullptr) return -2;
+    if (rows == 0) return 0;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map(&ma, a, rows, K, lda, 64))) return rc;
+    const uint64_t e = static_cast<uint64_t>(E);
+    if ((rc = b_mn ? make_map(&mb, b, e * K, N, N, 64) : make_map(&mb, b, e * (epi == EPI_SWIGLU ? 2 * N : N), K, K, 64)))
+        return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.aux = static_cast<const __nv_bfloat16*>(aux);
+    ep.out2 = static_cast<__nv_bfloat16*>(out2);
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ld_aux = ld_aux;
+    ep.ld_out2 = ld_out2;
+    ep.ldc = ldc;
+    ep.inter = N;
+    ep.offsets = offsets;
+    ep.E = E;
+    AgParams ag;
+    memset(&ag, 0, sizeof(ag));
+    int grid = sms > 0 ? sms : sm_count();
+    const int tn = epi == EPI_SWIGLU ? BN / 2 : BN;
+    const int64_t max_tiles = (static_cast<int64_t>(rows + BM - 1) / BM + E) * ((N + tn - 1) / tn);
+    if (grid > max_tiles) grid = static_cast<int>(max_tiles);
+    switch (epi) {
+        case EPI_SWIGLU: return launch_kernel<false, false, EPI_SWIGLU, MODE_RAGGED>(ma, mb, rows, N, K, grid, ep, ag, stream);
+        case EPI_DSWIGLU: return launch_kernel<false, true, EPI_DSWIGLU, MODE_RAGGED>(ma, mb, rows, N, K, grid, ep, ag, stream);
+        default:
+            return b_mn ? launch_kernel<false, true, EPI_STORE, MODE_RAGGED>(ma, mb, rows, N, K, grid, ep, ag, stream)
+                        : launch_kernel<false, false, EPI_STORE, MODE_RAGGED>(ma, mb, rows, N, K, grid, ep, ag, stream);
+    }
+}
+
+// Variable-K grouped weight gradient: c[e] (+)= a[rows of e]^T b[rows of e] for every expert, i.e. c [E, M, N] contiguous,
+// a [rows, M] (lda), b [rows, N] (ldb), both MN-major.  One launch of E x ceil(M/128) x ceil(N/256) tiles; a tile sums its
+// expert's k-blocks only.  An expert without rows gets c[e] = 0, or keeps c[e] with `accumulate`.
+// Host-checked (-2): rows >= 1, M % 8 == 0 and N % 8 == 0 besides the contract above.
+DSB_EXPORT int dsb_gemm_ragged_wgrad_bf16(const void* a, const void* b, void* c, const int* offsets, int rows, int E, int M,
+                                          int N, int lda, int ldb, int accumulate, int sms, cudaStream_t stream)
+{
+    if (rows < 1 || E < 1 || E > kMaxGroups || M <= 0 || N <= 0 || M % 8 || N % 8 || lda % 8 || ldb % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) return -2;
+    if (offsets == nullptr) return -2;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map(&ma, a, rows, M, lda, 64))) return rc;
+    if ((rc = make_map(&mb, b, rows, N, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ldc = N;
+    ep.offsets = offsets;
+    ep.E = E;
+    AgParams ag;
+    memset(&ag, 0, sizeof(ag));
+    int grid = sms > 0 ? sms : sm_count();
+    const int64_t tiles = static_cast<int64_t>(E) * ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+    if (grid > tiles) grid = static_cast<int>(tiles);
+    return accumulate ? launch_kernel<true, true, EPI_ACCUM, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream)
+                      : launch_kernel<true, true, EPI_STORE, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream);
 }
 
 DSB_EXPORT int dsb_gemm_tile_m() { return BM; }

@@ -202,9 +202,18 @@ inline int make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t c
     cuuint64_t strides[1] = {ld * 2};
     cuuint32_t box[2] = {64, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    auto encode = [&]() {
+        return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    };
+    CUresult r = encode();
+    if (r == CUDA_ERROR_INVALID_CONTEXT) {
+        // a driver-API call on a thread where the runtime has not made a context current yet (e.g. PyTorch's autograd
+        // worker thread before its first CUDA call): bind the current device's primary context and encode again
+        int dev = 0;
+        if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) r = encode();
+    }
     return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 100;
 }
 

@@ -46,7 +46,14 @@ class GroupedSwiGLUExperts(nn.Module):
             p.group_name = expert_group_name
 
     def forward(self, inputs):
-        """``inputs``: [E_local, tokens, hidden] (capacity-padded dispatch buffer) -> same shape."""
+        """``inputs``: [E_local, tokens, hidden] (capacity-padded dispatch buffer) -> same shape; or ``(rows, offsets)``:
+        expert-sorted rows [R, hidden] where expert ``e`` owns rows ``[offsets[e], offsets[e+1])`` (int32 on the rows'
+        device, 64-row aligned, zero-padded segments: the dropless layout) -> [R, hidden].  Rows outside
+        ``[offsets[0], offsets[E])`` of the result are unspecified (the wgmma path does not write them)."""
+        if isinstance(inputs, tuple):
+            from deepspeed_b200.ops.linear import ragged_swiglu_mlp
+            rows, offsets = inputs
+            return ragged_swiglu_mlp(rows, offsets, self.w13, self.w2, self.act)
         if inputs.is_cuda and inputs.dtype == torch.bfloat16 and self.act == "silu" and inputs.shape[1] >= 256:
             # wgmma path: per expert the fused gate|up GEMM (+) SwiGLU, down GEMM, and in backward the dSwiGLU-fused
             # input-gradient GEMM plus weight-gradient GEMMs written straight into the stacked parameters' flat ZeRO

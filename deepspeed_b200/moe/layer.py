@@ -12,7 +12,10 @@ from .sharded_moe import MOELayer, TopKGate
 
 class MoE(nn.Module):
     """Arguments as in the reference.  ``forward(hidden_states, used_token=None)`` returns
-    ``(output, l_aux, exp_counts)``."""
+    ``(output, l_aux, exp_counts)``.  ``expert`` is a module copied per local expert, or a grouped container (a module
+    with ``num_local_experts``) that takes the ``[E_local, C, hidden]`` dispatch buffer; with ``drop_tokens=False`` and
+    ``ep_size == 1`` the grouped container must be :class:`GroupedSwiGLUExperts`, which takes the dropless
+    ``(rows, offsets)`` layout."""
 
     def __init__(self, hidden_size, expert, num_experts=1, ep_size=1, k=1, capacity_factor=1.0,
                  eval_capacity_factor=1.0, min_capacity=4, use_residual=False, noisy_gate_policy: Optional[str] = None,

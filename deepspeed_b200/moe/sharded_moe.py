@@ -62,7 +62,8 @@ def _capacity(num_tokens, num_experts, capacity_factor, min_capacity, k=1):
 class GateOutput:
     """Routing decision in INDEX form (``[T, k]`` expert ids / slots / weights) -- what the permutation kernels consume.
     Indexing or unpacking it yields the reference's dense 4-tuple ``(l_aux, combine_weights [T, E, C], dispatch_mask
-    [T, E, C], exp_counts)`` (``sharded_moe.py:374``), materialised on demand for code written against that form."""
+    [T, E, C], exp_counts)`` (``sharded_moe.py:374``), materialised on demand for code written against that form.
+    ``capacity`` is an int, except for dropless routing on one expert-parallel rank, where it is a 0-dim device tensor."""
     __slots__ = ("l_aux", "expert_ids", "weights", "positions", "offsets", "counts", "capacity", "k")
 
     def dense(self):
@@ -132,22 +133,27 @@ def topkgating(logits, k, capacity_factor, min_capacity, drop_tokens=True, ep_gr
     out = GateOutput()
     out.l_aux, out.k = l_aux, k
     flat_ids = ids.to(torch.int32).contiguous()
+    # per-expert counts without torch.bincount, which waits for the device to size its output
+    counts = torch.zeros(E, dtype=torch.int32, device=logits.device).scatter_add_(
+        0, ids.reshape(-1), torch.ones(ids.numel(), dtype=torch.int32, device=logits.device))
     if use_rts and k == 1:
         # random token selection: capacity slots go to a random subset instead of the earliest tokens
         perm = torch.randperm(T, device=logits.device)
-        pos_p, counts, offsets = moe_ops.route(flat_ids[perm], E)
+        pos_p, counts, offsets = moe_ops.route(flat_ids[perm], E, counts=counts)
         positions = torch.empty_like(pos_p)
         positions[perm] = pos_p
     else:
-        positions, counts, offsets = moe_ops.route(flat_ids, E)
+        positions, counts, offsets = moe_ops.route(flat_ids, E, counts=counts)
     if drop_tokens:
         cap = _capacity(T, E, capacity_factor, min_capacity, k)
-    else:
+    elif ep_group is not None and dist.get_world_size(ep_group) > 1:
         mx = counts.max().to(torch.int64)
-        if ep_group is not None and dist.get_world_size(ep_group) > 1:
-            dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=ep_group)
-        cap = int(mx.item())
-        cap = max(cap, int(min_capacity))
+        dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=ep_group)
+        cap = max(int(mx.item()), int(min_capacity))
+    else:
+        # dropless on one expert-parallel rank: nothing is sized by the capacity, so it stays on the device (reading it,
+        # e.g. through the dense view, synchronises)
+        cap = counts.max().clamp(min=int(min_capacity))
     if drop_tokens and drop_policy == "probs":
         positions = _keep_most_probable(flat_ids, gates.gather(1, ids), counts, offsets, cap).reshape(positions.shape)
     out.expert_ids, out.weights, out.positions, out.offsets, out.counts, out.capacity = flat_ids, w, positions, offsets, \
@@ -248,24 +254,28 @@ class MOELayer(nn.Module):
         E = self.ep_size * self.num_local_experts
         k = g.k
         if self.ep_size == 1 and not self.gate.drop_tokens:
-            # exact layout: rows sorted by expert, no padding -> ragged per-expert slices
-            rows, slots = moe_ops.scatter(flat, g.expert_ids, g.positions, g.offsets, k, 0, T * k)
-            counts = g.counts.tolist()
-            outs, start = [], 0
-            chunks = rows.split(counts, dim=0)
             experts = self.experts.deepspeed_experts if hasattr(self.experts, "deepspeed_experts") else None
             if experts is not None:
-                for c, ex in zip(chunks, experts):
+                # user expert modules: rows sorted by expert, no padding -> ragged per-expert slices
+                rows, slots = moe_ops.scatter(flat, g.expert_ids, g.positions, g.offsets, k, 0, T * k)
+                outs = []
+                for c, ex in zip(rows.split(g.counts.tolist(), dim=0), experts):
                     o = ex(c) if c.shape[0] else c
                     outs.append(o[0] if isinstance(o, tuple) else o)
                 eo = torch.cat(outs, dim=0)
             else:
-                mx = max(counts) if counts else 0
-                padded = rows.new_zeros(E, mx, H)
-                for e, c in enumerate(chunks):
-                    padded[e, :c.shape[0]] = c
-                po = self.experts(padded)
-                eo = torch.cat([po[e, :n] for e, n in enumerate(counts)], dim=0)
+                from deepspeed_b200.moe.experts import GroupedSwiGLUExperts
+                if not isinstance(self.experts, GroupedSwiGLUExperts):
+                    raise TypeError(f"dropless routing (drop_tokens=False) with ep_size == 1 takes user expert modules "
+                                    f"(wrapped in Experts) or GroupedSwiGLUExperts; {type(self.experts).__name__} is a "
+                                    f"grouped container that does not take the (rows, offsets) layout")
+                # grouped experts: every expert's segment padded to a multiple of 64 rows (zero-filled by the scatter), the
+                # offsets built on the device and the buffer sized by its static bound T*k + E*63 -- no host
+                # synchronisation in forward or backward
+                seg = (g.counts + 63) // 64 * 64
+                offsets = torch.cat([seg.new_zeros(1), torch.cumsum(seg, 0, dtype=torch.int32)])
+                rows, slots = moe_ops.scatter(flat, g.expert_ids, g.positions, offsets, k, 0, T * k + E * 63)
+                eo = self.experts((rows, offsets))
             y = moe_ops.gather(eo, g.weights.to(torch.float32), slots, T, k)
             return y.reshape(x.shape).to(x.dtype)
         C = g.capacity

@@ -58,6 +58,83 @@ def grouped_matmul_nt(x, w, offsets, out=None, sms=0):
     return out
 
 
+RAGGED_ALIGN = 64  # rows per ragged segment granule: every expert offset is a multiple of it
+
+
+def _ragged_rows_ok(t):
+    return (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 8 == 0
+            and t.data_ptr() % 16 == 0 and t.shape[1] % 8 == 0)
+
+
+def supports_ragged(x, w, offsets) -> bool:
+    """Whether the ragged (dropless MoE) entry points take expert-sorted rows ``x [R, K]``, a stacked weight ``w [E, *, *]``
+    (contiguous) and int32 device offsets ``[E + 1]``.  The shape conditions each form adds (``K % 64``, ``I % 128``) are
+    checked by the kernel's host side, which refuses with :class:`NativeOpError`."""
+    return (_ragged_rows_ok(x) and torch.is_tensor(w) and w.is_cuda and w.dtype == torch.bfloat16 and w.dim() == 3
+            and w.is_contiguous() and w.data_ptr() % 16 == 0 and 1 <= w.shape[0] <= 256 and torch.is_tensor(offsets)
+            and offsets.is_cuda and offsets.dtype == torch.int32 and offsets.is_contiguous()
+            and offsets.numel() == w.shape[0] + 1)
+
+
+def ragged_matmul(x, w, offsets, b_mn, out=None, epi=0, aux=None, out2=None, sms=0):
+    """m-tiled ragged GEMM over expert-sorted rows (``dsb_gemm_ragged_bf16``; offsets stay on the device):
+
+    * ``b_mn=False``: ``w [E, N, K]``, ``out[r] = x[r] @ w[e]^T``; with ``epi=EPI_SWIGLU`` ``w`` is ``[E, 2I, K]`` (gate
+      rows, then up rows), ``out [R, I] = silu(gate) * up`` and ``out2`` (optional ``[R, 2I]``) receives gate|up;
+    * ``b_mn=True``: ``w [E, K, N]``, ``out[r] = x[r] @ w[e]``; with ``epi=EPI_DSWIGLU`` ``aux`` is the saved gate|up
+      ``[R, 2N]``, ``out2`` the ``[R, 2N]`` dgate|dup and ``out`` its left half.
+
+    Segments are 64-row aligned and zero-padded (see the entry point); malformed device offsets make the kernel write
+    nothing.  Rows of ``out`` outside ``[offsets[0], offsets[E])`` are not written.  Shapes that do not fit together raise
+    :class:`NativeOpError` before anything is launched (the tensor maps are built from them)."""
+    R, K = x.shape
+    E = w.shape[0]
+    if epi == EPI_SWIGLU:
+        Nn = w.shape[1] // 2
+    else:
+        Nn = w.shape[2] if b_mn else w.shape[1]
+    wk = w.shape[1] if b_mn else w.shape[2]
+    bad = (w.dim() != 3 or wk != K or (epi == EPI_SWIGLU and w.shape[1] != 2 * Nn) or offsets.numel() != E + 1
+           or (out is not None and tuple(out.shape) != (R, Nn)))
+    if epi == EPI_SWIGLU and out2 is not None:
+        bad = bad or tuple(out2.shape) != (R, 2 * Nn)
+    if epi == EPI_DSWIGLU:
+        bad = bad or aux is None or out2 is None or tuple(aux.shape) != (R, 2 * Nn) or tuple(out2.shape) != (R, 2 * Nn)
+    if bad:
+        raise N.NativeOpError(f"gemm_ragged_bf16: x {tuple(x.shape)}, w {tuple(w.shape)}, offsets {tuple(offsets.shape)} "
+                              f"and the outputs do not fit together (b_mn={int(b_mn)}, epi={epi})")
+    if out is None:
+        out = torch.empty(R, Nn, dtype=torch.bfloat16, device=x.device)
+    rc = N.cuda().dsb_gemm_ragged_bf16(N.ptr(x), N.ptr(w), N.ptr(out), N.ptr(offsets), R, E, Nn, K, x.stride(0),
+                                       out.stride(0), int(b_mn), int(epi), N.ptr(aux),
+                                       aux.stride(0) if aux is not None else 0, N.ptr(out2),
+                                       out2.stride(0) if out2 is not None else 0, sms, N.stream())
+    N.check(rc, "gemm_ragged_bf16")
+    return out
+
+
+def ragged_wgrad(a, b, offsets, E, out=None, accumulate=False, sms=0):
+    """Variable-K grouped weight gradient (``dsb_gemm_ragged_wgrad_bf16``): ``out[e] = a[rows of e]^T @ b[rows of e]``
+    (``accumulate``: added to ``out[e]``) for ``a [R, M]``, ``b [R, N]``, ``out [E, M, N]`` contiguous, in one launch.
+    An expert without rows gets zeros (or keeps ``out[e]`` when accumulating)."""
+    R, M = a.shape
+    Nn = b.shape[1]
+    if b.shape[0] != R or offsets.numel() != E + 1:
+        raise N.NativeOpError(f"gemm_ragged_wgrad_bf16: a {tuple(a.shape)}, b {tuple(b.shape)} and offsets "
+                              f"{tuple(offsets.shape)} do not share the rows of {E} experts")
+    if out is None:
+        assert not accumulate
+        out = torch.empty(E, M, Nn, dtype=torch.bfloat16, device=a.device)
+    if not out.is_contiguous() or tuple(out.shape) != (E, M, Nn):
+        raise N.NativeOpError(f"gemm_ragged_wgrad_bf16: out must be a contiguous [{E}, {M}, {Nn}] tensor")
+    if R == 0:
+        return out if accumulate else out.zero_()
+    rc = N.cuda().dsb_gemm_ragged_wgrad_bf16(N.ptr(a), N.ptr(b), N.ptr(out), N.ptr(offsets), R, E, M, Nn, a.stride(0),
+                                             b.stride(0), int(bool(accumulate)), sms, N.stream())
+    N.check(rc, "gemm_ragged_wgrad_bf16")
+    return out
+
+
 def matmul_nt_2cta(a, b, out=None, sms=0):
     """Same contract as :func:`matmul_nt` through the general entry point (grouped tile rasterisation)."""
     M, K = a.shape

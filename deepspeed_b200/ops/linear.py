@@ -208,6 +208,100 @@ def grouped_swiglu_mlp(x, w13, w2):
     return _GroupedSwiGLUFn.apply(x, w13, w2)
 
 
+def _stacked_grad_target(w, dtype):
+    """-> (zo, gradient tensor, accumulate) for a stacked expert weight: its flat ZeRO gradient view when it has one of
+    ``dtype`` (the GEMM epilogue stores or accumulates there), else a fresh tensor returned to autograd."""
+    zo = _zo_of(w)
+    if zo is not None and zo.grad_view_for(w).dtype == dtype:
+        return zo, zo.grad_view_for(w), not zo.grad_is_fresh(w)
+    return None, torch.empty_like(w), False
+
+
+class _RaggedSwiGLUFn(torch.autograd.Function):
+    """Dropless SwiGLU experts on expert-sorted rows ``x [R, H]``: expert ``e`` owns rows ``[offsets[e], offsets[e+1])``
+    (``offsets`` int32 ``[E + 1]`` on the device, segments 64-row aligned and zero-padded -- see
+    ``dsb_gemm_ragged_bf16``), ``w13 [E, 2I, H]``, ``w2 [E, H, I]``.  Every projection is ONE launch over all experts, with
+    no host synchronisation: forward gate|up (+) SwiGLU and down; backward down-dX (+) dSwiGLU, the variable-K dW2 and
+    dW13 and the dX of gate|up.  Weight gradients land in the stacked parameters' flat ZeRO gradient views (accumulated in
+    the epilogue on later micro steps), like :class:`_GroupedSwiGLUFn`."""
+
+    @staticmethod
+    def forward(ctx, x, offsets, w13, w2):
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        R = x.shape[0]
+        I = w2.shape[2]
+        need_grad = any(ctx.needs_input_grad)
+        gu = torch.empty(R, 2 * I, dtype=x.dtype, device=x.device) if need_grad else None
+        act = K.ragged_matmul(x, w13, offsets, False, epi=K.EPI_SWIGLU, out2=gu)
+        y = K.ragged_matmul(act, w2, offsets, False)
+        ctx.w13, ctx.w2 = w13, w2
+        if need_grad:
+            ctx.save_for_backward(x, offsets, gu, act)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        x, offsets, gu, act = ctx.saved_tensors
+        w13, w2 = ctx.w13, ctx.w2
+        E, I = w2.shape[0], w2.shape[2]
+        dy = dy.contiguous()
+        dgu = torch.empty(x.shape[0], 2 * I, dtype=dy.dtype, device=dy.device)
+        K.ragged_matmul(dy, w2, offsets, True, out=dgu[:, :I], epi=K.EPI_DSWIGLU, aux=gu, out2=dgu)
+        # every read of w13 / w2 comes before either weight is marked ready: marking the unit's last gradient ready
+        # reduces it, which under ZeRO-3 releases the gathered weights and with the step fused into backward rewrites them
+        dx = K.ragged_matmul(dgu, w13, offsets, True) if ctx.needs_input_grad[0] else None
+        outs = {}
+        for i, (w, a, b) in ((3, (w2, dy, act)), (2, (w13, dgu, x))):
+            if not ctx.needs_input_grad[i]:
+                outs[i] = None
+                continue
+            zo, g, accumulate = _stacked_grad_target(w, dy.dtype)
+            K.ragged_wgrad(a, b, offsets, E, out=g, accumulate=accumulate)
+            if zo is not None:
+                zo.mark_grad_ready(w)
+                g = None
+            outs[i] = g
+        return dx, None, outs[2], outs[3]
+
+
+def ragged_swiglu_reference(x, offsets, w13, w2, act="silu"):
+    """The per-expert torch loop with the contract of :class:`_RaggedSwiGLUFn` (any device and dtype, autograd through
+    torch).  Rows outside ``[offsets[0], offsets[E])`` come out as zeros here.  Reads the offsets on the host."""
+    from deepspeed_b200.ops.kernels.transformer_ops import gated_act
+    off = offsets.tolist()
+    pieces = [x.new_zeros(off[0], w2.shape[1])]
+    for e in range(w13.shape[0]):
+        xe = x[off[e]:off[e + 1]]
+        pieces.append(gated_act(xe @ w13[e].t(), act) @ w2[e].t() if xe.shape[0] else xe.new_zeros(0, w2.shape[1]))
+    pieces.append(x.new_zeros(x.shape[0] - off[-1], w2.shape[1]))
+    return torch.cat(pieces, dim=0)
+
+
+def ragged_swiglu_native(x, offsets, w13, w2, act="silu") -> bool:
+    """Whether :func:`ragged_swiglu_mlp` runs the wgmma kernels for these operands: CUDA bf16, SwiGLU, ``H % 64 == 0``,
+    ``I % 128 == 0`` and at most 256 experts."""
+    from deepspeed_b200.ops.kernels import gemm_sm100 as K
+    return (act == "silu" and K.supports_ragged(x, w13, offsets) and x.shape[1] % 64 == 0 and w2.shape[2] % 128 == 0
+            and w2.is_contiguous() and w2.dtype == torch.bfloat16)
+
+
+def ragged_swiglu_mlp(x, offsets, w13, w2, act="silu"):
+    """SwiGLU experts over expert-sorted rows ``x [R, H]`` with ``w13 [E, 2I, H]``, ``w2 [E, H, I]`` and ``offsets [E + 1]``:
+    see :class:`_RaggedSwiGLUFn`; other devices, dtypes, activations and shapes take :func:`ragged_swiglu_reference`.
+    Rows outside ``[offsets[0], offsets[E])`` of the result (and of ``x``'s gradient) are unspecified on the wgmma path,
+    which does not write them: callers read only the experts' rows."""
+    E, I = w13.shape[0], w2.shape[-1]
+    H = x.shape[-1]
+    if (x.dim() != 2 or w13.dim() != 3 or tuple(w13.shape) != (E, 2 * I, H) or tuple(w2.shape) != (E, H, I)
+            or offsets.dim() != 1 or offsets.numel() != E + 1):
+        raise ValueError(f"ragged_swiglu_mlp: rows {tuple(x.shape)}, w13 {tuple(w13.shape)}, w2 {tuple(w2.shape)} and "
+                         f"offsets {tuple(offsets.shape)} are not [R, H], [E, 2I, H], [E, H, I] and [E + 1]")
+    if ragged_swiglu_native(x, offsets, w13, w2, act):
+        return _RaggedSwiGLUFn.apply(x, offsets, w13, w2)
+    return ragged_swiglu_reference(x, offsets, w13, w2, act)
+
+
 class _ChunkedLinearXent(torch.autograd.Function):
 
     @staticmethod
