@@ -12,6 +12,8 @@
 //   * grouped (MoE) form: the tile list is built on the device from the expert offsets (no host synchronisation)
 //   * ragged (dropless MoE training) forms: the grouped form with every epilogue and an MN-major B whose expert offset
 //     lies on K, plus a variable-K weight-gradient form whose tile (expert, m, n) sums only its expert's rows
+//   * tensorwise-scaled FP8 form (gemm_fp8_kernel, dsb_gemm_fp8): e4m3 / e5m2 K-major operands, 128 x 128 tiles, every
+//     128-product k-block promoted into an fp32 accumulator, the same epilogues
 //   * OPTIONAL fused all-gather: when `ag` is given, the weight matrix B is being assembled in local memory from the
 //     other ranks' ZeRO shards *by this same kernel*: `ag.comm_ctas` CTAs pull the peers' shard bytes over NVLink
 //     (peer-mapped addresses) chunk by chunk and publish a per-chunk ready flag (st.release.gpu); the producer of each
@@ -538,6 +540,162 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
     }
 }
 
+// ---- FP8 (tensorwise-scaled) GEMM ---------------------------------------------------------------------------------------
+// C[M, N] (bf16) = epi(sa_inv * sb_inv * A[M, K] B[N, K]^T) with A e4m3 / e5m2 and B e4m3, both K-major (fp8 wgmma reads
+// K-major shared operands only).  A stage is [128 rows x 128 B] of A and of B: the same [64 x 128 B] swizzled boxes, the
+// same `desc_kmajor_sw128` and the same 32-byte step per k32 wgmma as the bf16 kernel's.
+// Promoted accumulation: Hopper's fp8 wgmma adds into its accumulator with reduced precision (about 14 bits, aligned to
+// the largest term), so each k-block's four wgmmas (128 K elements) go into a partial accumulator that ordinary FADDs add
+// into the fp32 main accumulator.  The reduced precision then applies to 128 products at a time and never to the running
+// sum: a block partial the tensor core holds exactly (e.g. small integers on a common power-of-two grid) gives an exact
+// result for any K, where an unpromoted accumulation loses the low bits once the sum outgrows 14 bits.  The two 64-float
+// accumulators per thread are why a tile is 128 x 128 (64 x 128 per consumer warpgroup), not the bf16 kernel's 128 x 256.
+constexpr int F8_BN = 128, F8_BK = 128;  // BK in fp8 elements (= bytes)
+constexpr int F8_STAGES = 6;
+constexpr uint32_t F8_BOX = 64 * 128;               // [64 rows x 128 B]
+constexpr uint32_t F8_STAGE_BYTES = 4 * F8_BOX;     // A: 2 boxes, B: 2 boxes
+static_assert(F8_STAGES * F8_STAGE_BYTES <= SMEM_BAR, "the fp8 ring must fit below the barriers");
+
+// EPI_SWIGLU: a tile's 128 B rows are 64 gate rows and the 64 up rows of the same features (N = inter, inter % 64 == 0)
+template <int AE5M2, int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
+                const EpiParams ep, const float* sa_inv, const float* sb_inv)
+{
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    const uint32_t sbase = smem_u32(smem);
+    const uint32_t bar_base = sbase + SMEM_BAR;
+    auto full_bar = [&](int s) { return bar_base + 8 * s; };
+    auto empty_bar = [&](int s) { return bar_base + 8 * (F8_STAGES + s); };
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    constexpr int TN = EPI == EPI_SWIGLU ? F8_BN / 2 : F8_BN;  // output columns per tile
+    const int num_m = (M + BM - 1) / BM, num_n = (N + TN - 1) / TN;
+    const int num_tiles = num_m * num_n;
+    const int group_m = ep.group_m > 0 ? ep.group_m : num_m;
+    const int num_k = (K + F8_BK - 1) / F8_BK;
+
+    if (threadIdx.x == kConsumerThreads) {
+        prefetch_map(&map_a);
+        prefetch_map(&map_b);
+        for (int s = 0; s < F8_STAGES; ++s) {
+            mbar_init(full_bar(s), 1);
+            mbar_init(empty_bar(s), kConsumerThreads / 32);
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (threadIdx.x >= kConsumerThreads) {
+        setmaxnreg_dec<kProducerRegs>();
+        if (threadIdx.x == kConsumerThreads) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                int m_blk, n_blk;
+                tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
+                const int row0 = m_blk * BM, col0 = n_blk * TN;
+                const int b0 = col0, b1 = EPI == EPI_SWIGLU ? ep.inter + col0 : col0 + 64;
+                for (int kb = 0; kb < num_k; ++kb) {
+                    mbar_wait(empty_bar(stage), phase ^ 1);
+                    const uint32_t sa = sbase + stage * F8_STAGE_BYTES, sb = sa + 2 * F8_BOX;
+                    const uint32_t fb = full_bar(stage);
+                    mbar_expect_tx(fb, F8_STAGE_BYTES);
+                    tma_load_2d(sa, &map_a, fb, kb * F8_BK, row0);
+                    tma_load_2d(sa + F8_BOX, &map_a, fb, kb * F8_BK, row0 + 64);
+                    tma_load_2d(sb, &map_b, fb, kb * F8_BK, b0);
+                    tma_load_2d(sb + F8_BOX, &map_b, fb, kb * F8_BK, b1);
+                    if (++stage == F8_STAGES) {
+                        stage = 0;
+                        phase ^= 1;
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = threadIdx.x >> 7;
+    const int r_in = 64 * wg + 16 * (warp & 3) + (lane >> 2);
+    const int c_in = 2 * (lane & 3);
+    // both scales are powers of two, so the product and the rescaling below are exact; a NaN scale makes C NaN
+    const float scale = *sa_inv * *sb_inv;
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[64], part[64];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
+        const int row0 = m_blk * BM, col0 = n_blk * TN;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        for (int kb = 0; kb < num_k; ++kb) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t sa = sbase + stage * F8_STAGE_BYTES + wg * F8_BOX, sb = sbase + stage * F8_STAGE_BYTES + 2 * F8_BOX;
+            const uint64_t da = desc_kmajor_sw128(sa), db = desc_kmajor_sw128(sb);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < F8_BK / 32; ++k) wgmma_m64n128k32_f8_ss<AE5M2>(part, da + 2 * k, db + 2 * k, k > 0 ? 1 : 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs<64>(part);
+            if (lane == 0) mbar_arrive(empty_bar(stage));
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] += part[i];
+            if (++stage == F8_STAGES) {
+                stage = 0;
+                phase ^= 1;
+            }
+        }
+
+        // ---- epilogue from the accumulators: thread holds rows r_in (+8), column pairs c_in + 8 j ----
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int lr = r_in + 8 * i;
+            if (row0 + lr >= M) continue;
+            const int64_t grow = row0 + lr;
+            if constexpr (EPI == EPI_SWIGLU) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int col = col0 + 8 * j + c_in;
+                    if (col >= N) continue;
+                    const float g0 = acc[4 * j + 2 * i] * scale, g1 = acc[4 * j + 2 * i + 1] * scale;
+                    const float u0 = acc[4 * (j + 8) + 2 * i] * scale, u1 = acc[4 * (j + 8) + 2 * i + 1] * scale;
+                    st_bf16x2(ep.c + grow * ep.ldc + col, silu_f(g0) * u0, silu_f(g1) * u1);
+                    if (ep.out2 != nullptr) {
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + col, g0, g1);
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + ep.inter + col, u0, u1);
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int col = col0 + 8 * j + c_in;
+                    if (col >= N) continue;
+                    float v0 = acc[4 * j + 2 * i] * scale, v1 = acc[4 * j + 2 * i + 1] * scale;
+                    __nv_bfloat16* dst = ep.c + grow * ep.ldc + col;
+                    if constexpr (EPI == EPI_ACCUM) {
+                        const float2 o = ld_bf16x2(dst);
+                        v0 += o.x;
+                        v1 += o.y;
+                    }
+                    if constexpr (EPI == EPI_DSWIGLU) {
+                        const float2 g = ld_bf16x2(ep.aux + grow * ep.ld_aux + col);
+                        const float2 u = ld_bf16x2(ep.aux + grow * ep.ld_aux + ep.inter + col);
+                        st_bf16x2(ep.out2 + grow * ep.ld_out2 + ep.inter + col, v0 * silu_f(g.x), v1 * silu_f(g.y));
+                        v0 = v0 * u.x * dsilu_f(g.x);
+                        v1 = v1 * u.y * dsilu_f(g.y);
+                    }
+                    st_bf16x2(dst, v0, v1);
+                }
+            }
+        }
+    }
+}
+
 }  // namespace gemm
 }  // namespace dsb
 
@@ -812,6 +970,80 @@ DSB_EXPORT int dsb_gemm_ragged_wgrad_bf16(const void* a, const void* b, void* c,
     if (grid > tiles) grid = static_cast<int>(tiles);
     return accumulate ? launch_kernel<true, true, EPI_ACCUM, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream)
                       : launch_kernel<true, true, EPI_STORE, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream);
+}
+
+template <int AE5M2, int EPI>
+static int launch_fp8(const CUtensorMap& ma, const CUtensorMap& mb, int M, int N, int K, int grid, const EpiParams& ep,
+                      const float* sa_inv, const float* sb_inv, cudaStream_t stream)
+{
+    static bool attr = false;
+    if (!attr) {
+        cudaError_t e =
+            cudaFuncSetAttribute(gemm_fp8_kernel<AE5M2, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
+        if (e != cudaSuccess) return static_cast<int>(e);
+        attr = true;
+    }
+    gemm_fp8_kernel<AE5M2, EPI><<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, sa_inv, sb_inv);
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+// Tensorwise-scaled FP8 GEMM:  C[M, N] (bf16) = epi(s * A[M, K] B[N, K]^T),  s = *sa_inv * *sb_inv  (device fp32 scalars,
+// read by the kernel: no host synchronisation).  Both operands are row-major and K-major: a [M, K] (lda), b [N, K] (ldb),
+// one byte per element.  a_fmt is the A format, 5 = e4m3 or 6 = e5m2 (the dtype codes of dsb_common.cuh); B is e4m3.
+// Every k-block of 128 products is added into an fp32 accumulator with ordinary FADDs (see the kernel: a block the tensor
+// core sums exactly gives an exact result for any K); the scaled result rounds once to bf16 (ACCUM: C_old + s * sum rounds
+// once).  A NaN scale inverse gives NaN outputs.
+//   epi 0 STORE   C = s AB^T
+//   epi 1 ACCUM   C = C + s AB^T
+//   epi 2 SWIGLU  A e4m3; b = [gate; up] [2N, K]; C [M, N] = silu(g) * u of g|u = s AB^T; out2 (nullable) [M, 2N] = g|u
+//   epi 3 DSWIGLU A e5m2; d = s AB^T [M, N]; aux = saved gate|up [M, 2N]; out2 [M, 2N] = dgate|dup, C its left half
+//                 (c == out2, ldc == ld_out2)
+// group_m: 128-row m-blocks per rasterisation super-group (<= 0: column-major tile order); sms <= 0: all SMs.
+// Host-checked (-2, nothing launched): M, N, K >= 1; K % 16 == 0; N % 8 == 0 (SWIGLU: N % 64 == 0); lda and ldb
+// multiples of 16 and >= K; ldc, ld_aux, ld_out2 multiples of 8 and ldc >= N; a, b, c, aux, out2 16-byte aligned;
+// sa_inv and sb_inv not null; a_fmt 5 or 6 and, for SWIGLU, 5, for DSWIGLU, 6; DSWIGLU with aux and out2; epi in 0..3.
+DSB_EXPORT int dsb_gemm_fp8(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc, int a_fmt,
+                            const float* sa_inv, const float* sb_inv, int epi, const void* aux, int ld_aux, void* out2,
+                            int ld_out2, int group_m, int sms, cudaStream_t stream)
+{
+    if (M <= 0 || N <= 0 || K <= 0 || K % 16 || N % 8) return -2;
+    if (lda % 16 || ldb % 16 || lda < K || ldb < K || ldc % 8 || ldc < N || ld_aux % 8 || ld_out2 % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
+         reinterpret_cast<uintptr_t>(aux) | reinterpret_cast<uintptr_t>(out2)) & 15)
+        return -2;
+    if (!sa_inv || !sb_inv || (a_fmt != dsb::kF8E4M3 && a_fmt != dsb::kF8E5M2) || epi < 0 || epi > 3) return -2;
+    const bool e5m2 = a_fmt == dsb::kF8E5M2;
+    if (epi == EPI_SWIGLU && (e5m2 || N % 64)) return -2;
+    if (epi == EPI_DSWIGLU && (!e5m2 || !aux || !out2)) return -2;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map_fp8(&ma, a, M, K, lda, 64))) return rc;
+    if ((rc = make_map_fp8(&mb, b, epi == EPI_SWIGLU ? 2 * static_cast<uint64_t>(N) : N, K, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.aux = static_cast<const __nv_bfloat16*>(aux);
+    ep.out2 = static_cast<__nv_bfloat16*>(out2);
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ld_aux = ld_aux;
+    ep.ld_out2 = ld_out2;
+    ep.ldc = ldc;
+    ep.inter = N;
+    ep.group_m = group_m;
+    int grid = sms > 0 ? sms : sm_count();
+    const int tn = epi == EPI_SWIGLU ? F8_BN / 2 : F8_BN;
+    const int64_t tiles = static_cast<int64_t>((M + BM - 1) / BM) * ((N + tn - 1) / tn);
+    if (grid > tiles) grid = static_cast<int>(tiles);
+    switch (epi) {
+        case EPI_STORE:
+            return e5m2 ? launch_fp8<1, EPI_STORE>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream)
+                        : launch_fp8<0, EPI_STORE>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+        case EPI_ACCUM:
+            return e5m2 ? launch_fp8<1, EPI_ACCUM>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream)
+                        : launch_fp8<0, EPI_ACCUM>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+        case EPI_SWIGLU: return launch_fp8<0, EPI_SWIGLU>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+        default: return launch_fp8<1, EPI_DSWIGLU>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+    }
 }
 
 DSB_EXPORT int dsb_gemm_tile_m() { return BM; }

@@ -168,6 +168,35 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float* d, const uint32_t* a, 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB));
 }
 
+// FP8 product, both operands K-major in shared memory (fp8 wgmma has no transpose bits): A e4m3 (AE5M2 = 0) or e5m2
+// (AE5M2 = 1), B e4m3.  One k32 step covers 32 bytes of a 128-byte swizzle row, like a bf16 k16 step.
+template <int AE5M2>
+__device__ __forceinline__ void wgmma_m64n128k32_f8_ss(float* d, uint64_t da, uint64_t db, int scale_d)
+{
+#define DSB_WGMMA_F8_OUTS                                                                                                    \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]),           \
+        "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]),           \
+        "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]),           \
+        "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]),           \
+        "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]),           \
+        "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]),           \
+        "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+    if constexpr (AE5M2) {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k32.f32.e5m2.e4m3 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n}\n"
+            : DSB_WGMMA_F8_OUTS
+            : "l"(da), "l"(db), "r"(scale_d));
+    } else {
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+            "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n}\n"
+            : DSB_WGMMA_F8_OUTS
+            : "l"(da), "l"(db), "r"(scale_d));
+    }
+#undef DSB_WGMMA_F8_OUTS
+}
 
 __device__ __forceinline__ float ex2(float x)
 {
@@ -192,20 +221,20 @@ inline EncodeTiledFn encode_fn()
     fn = reinterpret_cast<EncodeTiledFn>(p);
     return fn;
 }
-// Row-major [rows, cols] bf16 matrix with leading dimension `ld` (elements); box [box_rows x 64 cols], 128-byte swizzle.
-// Out-of-bounds rows / columns of a box read as zero.
-inline int make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows)
+// Row-major [rows, cols] matrix with leading dimension `ld` (elements) whose boxes are [box_rows x 128 bytes], 128-byte
+// swizzle.  Out-of-bounds rows / columns of a box read as zero.
+inline int make_map_128b(CUtensorMap* map, CUtensorMapDataType type, uint32_t elem_bytes, const void* ptr, uint64_t rows,
+                         uint64_t cols, uint64_t ld, uint32_t box_rows)
 {
     EncodeTiledFn fn = encode_fn();
     if (!fn) return -3;
     cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {64, box_rows};
+    cuuint64_t strides[1] = {ld * elem_bytes};
+    cuuint32_t box[2] = {128 / elem_bytes, box_rows};
     cuuint32_t estr[2] = {1, 1};
     auto encode = [&]() {
-        return fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        return fn(map, type, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     };
     CUresult r = encode();
     if (r == CUDA_ERROR_INVALID_CONTEXT) {
@@ -215,6 +244,16 @@ inline int make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t c
         if (cudaGetDevice(&dev) == cudaSuccess && cudaSetDevice(dev) == cudaSuccess) r = encode();
     }
     return r == CUDA_SUCCESS ? 0 : -static_cast<int>(r) - 100;
+}
+// bf16 [rows, cols]: box [box_rows x 64 cols]
+inline int make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows)
+{
+    return make_map_128b(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, rows, cols, ld, box_rows);
+}
+// fp8 (e4m3 / e5m2 bytes) [rows, cols]: box [box_rows x 128 cols]
+inline int make_map_fp8(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows)
+{
+    return make_map_128b(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ptr, rows, cols, ld, box_rows);
 }
 
 }  // namespace tc

@@ -48,6 +48,10 @@ class LlamaConfig:
     # causal sliding-window attention (HF ``sliding_window``): token i attends to tokens i - W < j <= i, inside its document
     # when packed; None attends to the whole causal prefix
     sliding_window: Optional[int] = None
+    # FP8 products in the four decoder projections (qkv, o, gate|up with SwiGLU, down), forward and backward, with the
+    # tensorwise power-of-two recipe of ``ops/fp8.py``; weights, optimizer, gradients, attention, norms, embedding and
+    # LM head stay bf16
+    fp8: bool = False
     # training knobs
     checkpoint_layers: int = 0  # number of decoder layers (from the front) run with activation recompute
     loss_chunk_tokens: int = 2048
@@ -135,13 +139,17 @@ class RMSNorm(nn.Module):
 class FlatLinear(nn.Module):
     """``nn.Linear`` whose backward writes dW straight into the ZeRO flat gradient buffer."""
 
-    def __init__(self, in_features, out_features, bias=False):
+    def __init__(self, in_features, out_features, bias=False, fp8=False):
         super().__init__()
         self.in_features, self.out_features = in_features, out_features
         self.weight = nn.Parameter(torch.empty(out_features, in_features))
         self.bias = nn.Parameter(torch.zeros(out_features)) if bias else None
+        self.fp8 = fp8
 
     def forward(self, x):
+        if self.fp8:
+            from deepspeed_b200.ops.linear import fp8_linear
+            return fp8_linear(x, self.weight, self.bias)
         return flat_linear(x, self.weight, self.bias)
 
 
@@ -164,8 +172,8 @@ class LlamaAttention(nn.Module):
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
         self.cfg = cfg
-        self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias)
-        self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False)
+        self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias, fp8=cfg.fp8)
+        self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False, fp8=cfg.fp8)
 
     def forward(self, x, rope, positions=None, cu_seqlens=None, max_seqlen=None):
         cfg = self.cfg
@@ -181,12 +189,16 @@ class LlamaMLP(nn.Module):
 
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
-        self.gate_up_proj = FlatLinear(cfg.hidden_size, 2 * cfg.intermediate_size)
-        self.down_proj = FlatLinear(cfg.intermediate_size, cfg.hidden_size)
+        self.gate_up_proj = FlatLinear(cfg.hidden_size, 2 * cfg.intermediate_size, fp8=cfg.fp8)
+        self.down_proj = FlatLinear(cfg.intermediate_size, cfg.hidden_size, fp8=cfg.fp8)
         self.act = cfg.hidden_act
+        self.fp8 = cfg.fp8
 
     def forward(self, x):
         if self.act == "silu" and self.gate_up_proj.bias is None and self.down_proj.bias is None:
+            if self.fp8:
+                from deepspeed_b200.ops.linear import fp8_swiglu_mlp
+                return fp8_swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight)
             from deepspeed_b200.ops.linear import swiglu_mlp
             return swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight)
         return self.down_proj(T.gated_act(self.gate_up_proj(x), self.act))

@@ -26,6 +26,7 @@ class CudaKernelsBuilder(CUDAOpBuilder):
         "cuda/misc.cu",
         "cuda/symm_coll.cu",
         "cuda/gemm_sm90.cu",
+        "cuda/fp8_cast.cu",
         "cuda/attention.cu",
         "cuda/attn_sm90.cu",
         "cuda/attn_bias.cu",

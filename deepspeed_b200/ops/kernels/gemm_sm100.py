@@ -176,6 +176,47 @@ def matmul_2cta(a, b, a_mn: bool, b_mn: bool, out=None, sms=0, epi=EPI_STORE, au
     return out
 
 
+def fp8_matmul(a, b, sa_inv, sb_inv, out=None, epi=EPI_STORE, aux=None, out2=None, group_m=8, sms=0):
+    """Tensorwise-scaled FP8 GEMM (``dsb_gemm_fp8``): ``out [M, N] (bf16) = epi(sa_inv * sb_inv * a @ b^T)`` for K-major
+    ``a [M, K]`` (``float8_e4m3fn`` or ``float8_e5m2``) and ``b [N, K]`` (``float8_e4m3fn``); ``sa_inv`` / ``sb_inv`` are
+    one-element fp32 device tensors, read by the kernel (no host synchronisation).  Every 128 products are promoted into
+    an fp32 accumulator: the tensor core's reduced-precision accumulation never carries the running sum, so it costs
+    about 2**-14 of a block's magnitudes whatever K is, and nothing where a block sums exactly (small integers on a grid).
+
+    ``epi``: ``EPI_ACCUM`` adds into ``out``; ``EPI_SWIGLU`` (``a`` e4m3) -- ``b`` is ``[2N, K]`` (gate rows, then up rows),
+    ``out [M, N] = silu(g) * u`` and ``out2`` (optional ``[M, 2N]``) receives g|u; ``EPI_DSWIGLU`` (``a`` e5m2) -- ``aux`` is
+    the saved gate|up ``[M, 2N]``, ``out2`` the ``[M, 2N]`` dgate|dup and ``out`` its left half (allocated as a view of
+    ``out2`` when None).  Shapes that do not fit together raise :class:`NativeOpError` before a tensor map is built; the
+    kernel's host side refuses the rest (see the entry point)."""
+    fmt = {torch.float8_e4m3fn: N.F8E4M3, torch.float8_e5m2: N.F8E5M2}.get(a.dtype)
+    M, K = a.shape if a.dim() == 2 else (0, 0)
+    Nn = b.shape[0] // 2 if epi == EPI_SWIGLU else b.shape[0]
+    bad = (fmt is None or b.dtype != torch.float8_e4m3fn or a.dim() != 2 or b.dim() != 2 or b.shape[1] != K
+           or (epi == EPI_SWIGLU and b.shape[0] != 2 * Nn) or a.stride(1) != 1 or b.stride(1) != 1
+           or sa_inv is None or sb_inv is None or sa_inv.dtype != torch.float32 or sb_inv.dtype != torch.float32
+           or sa_inv.numel() != 1 or sb_inv.numel() != 1)
+    if out is not None:
+        bad = bad or tuple(out.shape) != (M, Nn) or out.dtype != torch.bfloat16 or out.stride(1) != 1
+    if out2 is not None:
+        bad = bad or tuple(out2.shape) != (M, 2 * Nn) or out2.dtype != torch.bfloat16 or out2.stride(1) != 1
+    if aux is not None:
+        bad = bad or tuple(aux.shape) != (M, 2 * Nn) or aux.dtype != torch.bfloat16 or aux.stride(1) != 1
+    if epi == EPI_DSWIGLU:
+        bad = bad or aux is None or out2 is None
+    if epi == EPI_ACCUM:
+        bad = bad or out is None
+    if bad:
+        raise N.NativeOpError(f"gemm_fp8: a {tuple(a.shape)} {a.dtype}, b {tuple(b.shape)} {b.dtype}, the scales and the "
+                              f"outputs do not fit together (epi={epi})")
+    if out is None:
+        out = out2[:, :Nn] if epi == EPI_DSWIGLU else torch.empty(M, Nn, dtype=torch.bfloat16, device=a.device)
+    rc = N.cuda().dsb_gemm_fp8(N.ptr(a), N.ptr(b), N.ptr(out), M, Nn, K, a.stride(0), b.stride(0), out.stride(0), fmt,
+                               N.ptr(sa_inv), N.ptr(sb_inv), int(epi), N.ptr(aux), aux.stride(0) if aux is not None else 0,
+                               N.ptr(out2), out2.stride(0) if out2 is not None else 0, int(group_m), sms, N.stream())
+    N.check(rc, "gemm_fp8")
+    return out
+
+
 def supports_2cta(a, b, a_mn, b_mn, out=None) -> bool:
     ok = lambda t: (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 8 == 0
                     and t.data_ptr() % 16 == 0 and t.shape[1] % 8 == 0)

@@ -141,6 +141,157 @@ def swiglu_mlp(x, w_gate_up, w_down):
     return _SwiGLUMLPFn.apply(x, w_gate_up, w_down)
 
 
+def _fp8_native(x2, *ws, inter=None) -> bool:
+    """Whether the FP8 nodes run the wgmma kernels: CUDA bf16 rows ``x2 [T, K]`` and weights, every dimension (and, for
+    the SwiGLU block, ``2 I``) a multiple of 16 -- each is a K of some product or the row count of a transposed cast --
+    and ``I % 64 == 0`` for the SwiGLU epilogue's tile."""
+    ts = (x2, ) + ws
+    if not all(t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 for t in ts):
+        return False
+    if any(d % 16 for t in ts for d in t.shape):
+        return False
+    return inter is None or inter % 64 == 0
+
+
+def _fp8_cast_fn(native):
+    from deepspeed_b200.ops import fp8
+    return fp8.quantize_tensorwise if native else fp8.quantize_reference
+
+
+def _fp8_weight_grad(w, a8t, b8t, sa, sb, native):
+    """dW = sa sb a8t b8t^T (``a8t`` the e5m2 gradient transposed, ``b8t`` the e4m3 input transposed): stored, or
+    accumulated on later micro steps, straight into the ZeRO flat gradient view when there is one (returns None), else
+    returned for autograd."""
+    from deepspeed_b200.ops import fp8
+    zo = _zo_of(w)
+    if zo is None:
+        return fp8.gemm(a8t, b8t, sa, sb, native).to(w.dtype)
+    gv = zo.grad_view_for(w)
+    if gv.dtype == torch.bfloat16:
+        fp8.gemm(a8t, b8t, sa, sb, native, out=gv, accumulate=not zo.grad_is_fresh(w))
+    else:
+        g = fp8.gemm(a8t, b8t, sa, sb, native)
+        gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
+    zo.mark_grad_ready(w)
+    return None
+
+
+class _FP8LinearFn(torch.autograd.Function):
+    """``y = x W^T (+ b)`` in FP8 (the recipe of :mod:`deepspeed_b200.ops.fp8`): forward casts ``x`` to e4m3 (and its
+    transpose, for dW) and ``W`` to e4m3 and saves only the transposed ``x`` and its scale; backward casts ``dY`` (and its
+    transpose) to e5m2 and re-reads the weight (as :class:`_FlatLinearFn`, so ZeRO-3 may release it after forward) to
+    cast ``W^T``.  dW lands in the ZeRO flat gradient view."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        from deepspeed_b200.ops import fp8
+        x2 = x.reshape(-1, x.shape[-1])
+        native = _fp8_native(x2, weight)
+        cast = _fp8_cast_fn(native)
+        x8, x8t, sx = cast(x2, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[1])
+        w8, _, sw = cast(weight, fp8.E4M3)
+        y = fp8.gemm(x8, w8, sx, sw, native).to(x.dtype)
+        if bias is not None:
+            y = y + bias
+        ctx.weight_ref = weight
+        ctx.has_bias = bias is not None
+        ctx.native = native
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.save_for_backward(x8t, sx)
+        return y.view(*x.shape[:-1], weight.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops import fp8
+        x8t, sx = ctx.saved_tensors
+        w, native = ctx.weight_ref, ctx.native
+        cast = _fp8_cast_fn(native)
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        dx = dw = None
+        if need_dx or need_dw:
+            dy8, dy8t, sdy = cast(dy2, fp8.E5M2, rowwise=need_dx, colwise=need_dw)
+            if need_dx:
+                _, w8t, sw = cast(w, fp8.E4M3, rowwise=False, colwise=True)
+                dx = fp8.gemm(dy8, w8t, sdy, sw, native).to(ctx.x_dtype).view(ctx.x_shape)
+            if need_dw:
+                dw = _fp8_weight_grad(w, dy8t, x8t, sdy, sx, native)
+        db = dy2.sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
+        return dx, dw, db
+
+
+def fp8_linear(x, weight, bias=None):
+    """``x W^T (+ b)`` with FP8 products (see :class:`_FP8LinearFn`).  CUDA bf16 operands whose dimensions are multiples
+    of 16 run the wgmma kernels; anything else runs the torch reference of the same recipe (never a bf16 product)."""
+    return _FP8LinearFn.apply(x, weight, bias)
+
+
+class _FP8SwiGLUMLPFn(torch.autograd.Function):
+    """``down(silu(gate(x)) * up(x))`` in FP8, one node like :class:`_SwiGLUMLPFn`:
+
+    forward   x -> e4m3 (+ transposed); gate|up FP8 GEMM with the SwiGLU epilogue (gate|up saved in bf16);
+              act -> e4m3 (+ transposed); FP8 down GEMM;
+    backward  dY -> e5m2 (+ transposed); FP8 ``dY W_down`` GEMM with the dSwiGLU epilogue; dgate|dup -> e5m2 (+ transposed);
+              FP8 dX, dW_down and dW_gate_up, the weight gradients into the ZeRO flat gradient views.
+    Every read of a weight comes before either weight's gradient is marked ready (marking a unit's last gradient reduces
+    it, which under ZeRO-3 releases the gathered weights and with the step fused into backward rewrites them)."""
+
+    @staticmethod
+    def forward(ctx, x, w_gu, w_down):
+        from deepspeed_b200.ops import fp8
+        x2 = x.reshape(-1, x.shape[-1])
+        native = _fp8_native(x2, w_gu, w_down, inter=w_down.shape[1])
+        cast = _fp8_cast_fn(native)
+        need_grad = any(ctx.needs_input_grad)
+        x8, x8t, sx = cast(x2, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[1])
+        wgu8, _, sgu = cast(w_gu, fp8.E4M3)
+        act, gu = fp8.gemm_swiglu(x8, wgu8, sx, sgu, native, save_gate_up=need_grad)
+        act8, act8t, sa = cast(act, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[2])
+        wd8, _, sd = cast(w_down, fp8.E4M3)
+        y = fp8.gemm(act8, wd8, sa, sd, native).to(x.dtype)
+        ctx.w_gu, ctx.w_down, ctx.native = w_gu, w_down, native
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.save_for_backward(x8t, sx, gu, act8t, sa)
+        return y.view(*x.shape[:-1], w_down.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops import fp8
+        x8t, sx, gu, act8t, sa = ctx.saved_tensors
+        w_gu, w_down, native = ctx.w_gu, ctx.w_down, ctx.native
+        cast = _fp8_cast_fn(native)
+        need_dx, need_dgu, need_dd = ctx.needs_input_grad
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        dy8, dy8t, sdy = cast(dy2, fp8.E5M2, rowwise=True, colwise=need_dd)
+        _, wd8t, sd = cast(w_down, fp8.E4M3, rowwise=False, colwise=True)
+        dgu = fp8.gemm_dswiglu(dy8, wd8t, sdy, sd, gu, native)
+        wgu8t = sgu = None
+        if need_dx:
+            _, wgu8t, sgu = cast(w_gu, fp8.E4M3, rowwise=False, colwise=True)
+        dx = dw_gu = dw_down = None
+        if need_dx or need_dgu:
+            dgu8, dgu8t, sg = cast(dgu, fp8.E5M2, rowwise=need_dx, colwise=need_dgu)
+            if need_dx:
+                dx = fp8.gemm(dgu8, wgu8t, sg, sgu, native).to(ctx.x_dtype).view(ctx.x_shape)
+        # weights are not read past this point
+        if need_dd:
+            dw_down = _fp8_weight_grad(w_down, dy8t, act8t, sdy, sa, native)
+        if need_dgu:
+            dw_gu = _fp8_weight_grad(w_gu, dgu8t, x8t, sg, sx, native)
+        return dx, dw_gu, dw_down
+
+
+def fp8_swiglu_mlp(x, w_gate_up, w_down):
+    """SwiGLU MLP block (no biases) with FP8 products: see :class:`_FP8SwiGLUMLPFn`.  CUDA bf16 operands with
+    ``T, H, 2I`` multiples of 16 and ``I % 64 == 0`` run the wgmma kernels; anything else runs the torch reference of the
+    same recipe (never a bf16 product)."""
+    return _FP8SwiGLUMLPFn.apply(x, w_gate_up, w_down)
+
+
 class _GroupedSwiGLUFn(torch.autograd.Function):
     """Stacked SwiGLU experts on a capacity-padded dispatch buffer ``x [E, C, H]`` with ``w13 [E, 2I, H]``, ``w2 [E, H, I]``
     (the MoE training path, reference ``moe/experts.py:13`` + ``sharded_moe.py:586``): per expert the same three fused GEMM
