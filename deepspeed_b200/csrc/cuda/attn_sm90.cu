@@ -722,6 +722,16 @@ int launch_bwd(int head_dim, const void* q, const void* k, const void* v, const 
 
 using namespace dsb::attn;
 
+// The backward's operands must be 16-byte aligned: the tensor maps of q / k / v / d_o need it, the prep pass loads O as
+// 8-byte words and store_acc writes dQ / dK / dV as 4-byte words, so a misaligned view is refused here instead of faulting.
+static bool bwd_misaligned(const void* q, const void* k, const void* v, const void* o, const void* d_o, const void* dq,
+                           const void* dk, const void* dv)
+{
+    return ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+             reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(d_o) | reinterpret_cast<uintptr_t>(dq) |
+             reinterpret_cast<uintptr_t>(dk) | reinterpret_cast<uintptr_t>(dv)) & 15) != 0;
+}
+
 // q / k / v: 2-D bf16 tensors [B*S, *] (row stride ld_*), head `i` at columns [i*head_dim, +head_dim) -- for a packed QKV
 // projection output all three point into the same buffer.  o: [B*S, ld_o] (head h at h*head_dim).  head_dim: 64 or 128.  lse: fp32 [B, Hq, S] or null.
 // window > 0: causal sliding-window attention, row i sees keys i - window < j <= i (flash-attn's window_size = (window - 1,
@@ -753,6 +763,7 @@ DSB_EXPORT int dsb_attn_bwd_bf16(const void* q, const void* k, const void* v, co
 {
     if ((head_dim != 64 && head_dim != 128) || S % BQ || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
     if (window > 0 && !causal) return -2;
+    if (bwd_misaligned(q, k, v, o, d_o, dq, dk, dv)) return -2;
     if (window > 0)
         return launch_bwd<false, true>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, nullptr, B, S, B * S, Hq, Hkv, ld_q, ld_k, ld_v,
                                        ld_o, ld_do, ld_dq, ld_dk, ld_dv, q_cols, k_cols, v_cols, scale, causal, window, stream);
@@ -794,6 +805,7 @@ DSB_EXPORT int dsb_attn_varlen_bwd_bf16(const void* q, const void* k, const void
     if ((head_dim != 64 && head_dim != 128) || Hq % Hkv || (ld_q | ld_k | ld_v | ld_o | ld_do | ld_dq | ld_dk | ld_dv) % 8) return -2;
     if (T < 0 || n_docs < 0 || n_docs > 65535 || (T > 0 && max_seqlen <= 0) || cu_seqlens == nullptr) return -2;
     if (window > 0 && !causal) return -2;
+    if (bwd_misaligned(q, k, v, o, d_o, dq, dk, dv)) return -2;
     if (T == 0 || n_docs == 0) return 0;
     if (window > 0)
         return launch_bwd<true, true>(head_dim, q, k, v, o, d_o, lse, dq, dk, dv, work, cu_seqlens, n_docs, max_seqlen, T, Hq, Hkv, ld_q,

@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.numerics import assert_attention_bounded
+
 pytestmark = pytest.mark.gpu
 
 d = 64
@@ -63,42 +65,16 @@ def _varlen(qkv, d_o, lens, hq, hkv, causal=True, window=None, hd=d, scale=None)
     return o, lse, dqkv
 
 
-def _ref(x, hq, hkv, causal=True, window=None):
-    """float64 reference on one sequence: x [L, (hq + 2 hkv) * d] -> (o [L, hq, d], lse [hq, L]) with autograd."""
-    L = x.shape[0]
-    y = x.view(L, hq + 2 * hkv, d)
-    q, k, v = y[:, :hq], y[:, hq:hq + hkv], y[:, hq + hkv:]
-    rep = hq // hkv
-    k, v = k.repeat_interleave(rep, 1), v.repeat_interleave(rep, 1)
-    s = torch.einsum("qhd,khd->hqk", q, k) / math.sqrt(d)
-    i = torch.arange(L, device=x.device)
-    diff = i[:, None] - i[None, :]
-    if causal:
-        keep = diff >= 0
-        if window is not None:
-            keep = keep & (diff < window)
-        s = s.masked_fill(~keep, float("-inf"))
-    return torch.einsum("hqk,khd->qhd", torch.softmax(s, -1), v), torch.logsumexp(s, -1)
-
-
 def _check_against_ref(qkv, d_o, o, lse_rows, dqkv, hq, hkv, causal=True, window=None, grads=True):
-    """One sequence: o [L, hq*d], lse_rows [hq, L], dqkv [L, (hq + 2 hkv) * d] against the float64 reference."""
+    """One sequence: o [L, hq*d], lse_rows [hq, L], dqkv [L, (hq + 2 hkv) * d] inside the per-element bounds of
+    :func:`tests.numerics.attention_bounds` around the float64 reference."""
     L = qkv.shape[0]
-    x = qkv.double().requires_grad_(grads)
-    ro, rl = _ref(x, hq, hkv, causal, window)
-    assert (o.double().view(L, hq, d) - ro).abs().max().item() < 2e-2
-    assert (lse_rows.double() - rl).abs().max().item() < 2e-2
-    if not grads:
-        return
-    ro.backward(d_o.double().view(L, hq, d))
-    got, ref = dqkv.double(), x.grad
-    for c0, c1 in ((0, hq * d), (hq * d, (hq + hkv) * d), ((hq + hkv) * d, (hq + 2 * hkv) * d)):
-        gg, rr = got[:, c0:c1], ref[:, c0:c1]
-        err, top = (gg - rr).abs().max().item(), rr.abs().max().item()
-        assert err < 3e-2 * top + 2e-2, (c0, err, top)
-        if top > 1e-3 and L > 1:  # with W = 1 (or one row) the softmax is constant: dQ and dK are zero
-            cos = torch.nn.functional.cosine_similarity(gg.flatten(), rr.flatten(), dim=0).item()
-            assert cos > 0.999, (c0, cos)
+    heads = lambda x, n: x.reshape(L, n, d)  # noqa: E731
+    q, k, v = (heads(c, n) for c, n in zip(_cols(qkv, hq, hkv), (hq, hkv, hkv)))
+    got = {"o": heads(o, hq), "lse": lse_rows}
+    if grads:
+        got.update(zip(("dq", "dk", "dv"), (heads(c, n) for c, n in zip(_cols(dqkv, hq, hkv), (hq, hkv, hkv)))))
+    assert_attention_bounded(got, q, k, v, heads(d_o, hq) if grads else None, None, causal, window)
 
 
 # ---- 1. dense against float64 ----------------------------------------------------------------------------------------------

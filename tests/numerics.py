@@ -305,3 +305,294 @@ def chunked_xent_reference(h, w, labels, chunk, ignore_index=-100):
     # row losses are summed in fp32 within a chunk (at most ``chunk`` adds), then chunk by chunk
     loss_bound = (loss_err + (chunk + n_chunks + 2) * U * loss_abs) / n + U * abs(loss)
     return loss, dh, dW, loss_bound, dh_bound, dW_bound
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# training attention (csrc/cuda/attn_sm90.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+LOG2E = 1.0 / math.log(2.0)
+LN2 = math.log(2.0)
+U_BF16 = 2.0**-8  # bf16 unit roundoff: 8 significant bits, round to nearest
+ATTN_BLOCK = 64  # keys per block of the forward and dQ kernels, query rows per block of the dK / dV kernel
+ATTN_ROWS = 1024  # query rows per float64 chunk: a [1024, 4096] float64 matrix is 32 MB
+
+
+def _rel(n):
+    """``|prod (1 + d_k) - 1|`` for ``n`` fp32 roundings ``|d_k| <= U``."""
+    return math.expm1(n * math.log1p(U))
+
+
+def attention_documents(T, cu_seqlens=None):
+    """Non-empty ``(start, end)`` token spans: the documents of ``cu_seqlens`` or one sequence of ``T`` rows."""
+    cu = [0, T] if cu_seqlens is None else [int(c) for c in cu_seqlens]
+    return [(s, e) for s, e in zip(cu[:-1], cu[1:]) if e > s]
+
+
+def attention_visible(L, causal=True, window=None, device=None):
+    """bool ``[L, L]``: query row i sees key j -- ``j <= i`` when causal, and ``i - window < j`` with a window."""
+    i = torch.arange(L, device=device)
+    diff = i[:, None] - i[None, :]
+    vis = diff >= 0 if causal else torch.ones(L, L, dtype=torch.bool, device=device)
+    if window is not None:
+        vis = vis & (diff < window)
+    return vis
+
+
+def _attention(q, k, v, do, cu_seqlens, causal, window, scale, mask, kv_heads, bounds):
+    """Float64 attention one (document, query head, chunk of query rows) at a time, and the bounds of
+    :func:`attention_bounds` when ``bounds``.  Heads outside ``kv_heads`` keep reference 0 and bound inf."""
+    T, Hq, d = q.shape
+    Hkv = k.shape[1]
+    rep = Hq // Hkv
+    c = 1.0 / math.sqrt(d) if scale is None else float(scale)
+    cl = c * LOG2E
+    f64 = dict(dtype=torch.float64, device=q.device)
+    ref = {"o": torch.zeros(T, Hq, d, **f64), "lse": torch.zeros(Hq, T, **f64)}
+    if do is not None:
+        ref.update(dq=torch.zeros(T, Hq, d, **f64), dk=torch.zeros(T, Hkv, d, **f64), dv=torch.zeros(T, Hkv, d, **f64))
+    bnd = {n: torch.full_like(r, math.inf) for n, r in ref.items()} if bounds else None
+    R2, R3, R4 = _rel(2), _rel(3), _rel(4)
+    for s0, e0 in attention_documents(T, cu_seqlens):
+        L = e0 - s0
+        vis = mask[s0:e0, s0:e0] if mask is not None else attention_visible(L, causal, window, q.device)
+        n_b = -(-L // ATTN_BLOCK)  # key blocks (forward, dQ) or query blocks per head (dK / dV) a kernel visits at most
+        for g in (range(Hkv) if kv_heads is None else kv_heads):
+            K, V = k[s0:e0, g].double(), v[s0:e0, g].double()
+            aK, aV = K.abs(), V.abs()
+            if do is not None:
+                dK, dV = torch.zeros(L, d, **f64), torch.zeros(L, d, **f64)
+                if bounds:
+                    eK, mK, eV, mV = (torch.zeros(L, d, **f64) for _ in range(4))
+            for h in range(g * rep, (g + 1) * rep):
+                for r0 in range(0, L, ATTN_ROWS):
+                    r1 = min(r0 + ATTN_ROWS, L)
+                    rows = slice(s0 + r0, s0 + r1)
+                    vm = vis[r0:r1]
+                    Q = q[rows, h].double()
+                    sc = Q @ K.t()
+                    t = (sc * c).masked_fill(~vm, -math.inf)
+                    lse = torch.logsumexp(t, -1)
+                    P = torch.exp(t - lse[:, None]).nan_to_num(0.0)  # a row that sees nothing: P = 0
+                    O = P @ V
+                    ref["o"][rows, h] = O
+                    ref["lse"][h, rows] = lse
+                    if do is not None:
+                        dO = do[rows, h].double()
+                        dP = dO @ V.t()
+                        delta = (dO * O).sum(-1)
+                        dS = P * (dP - delta[:, None]) * c
+                        ref["dq"][rows, h] = dS @ K
+                        dK += dS.t() @ Q
+                        dV += P.t() @ dO
+                    if not bounds:
+                        continue
+                    # ---- forward ----
+                    zero = torch.zeros((), **f64)
+                    e_s = gemm_accum_error(Q.abs() @ aK.t(), d)
+                    err_x = torch.where(vm, cl * (e_s * (1 + R4) + R4 * sc.abs()), zero)
+                    t2 = torch.where(vm, sc * cl, zero)
+                    t2max = torch.where(vm, t2, -math.inf).max(-1).values
+                    emax = err_x.max(-1).values
+                    dist = t2max[:, None] - t2 + err_x + emax[:, None]
+                    span = t2max - torch.where(vm, t2, math.inf).min(-1).values + 2 * emax
+                    lnrel = LN2 * (err_x + U * (dist + span[:, None])) + (5 * n_b + 4) * U
+                    Pe = torch.where(vm, P * torch.expm1(lnrel) + 2.0**-125, zero)
+                    Pw = P + Pe  # bound on |p~| / l
+                    num = (Pe + U_BF16 * Pw) @ aV + gemm_accum_error((Pw * (1 + U_BF16)) @ aV, ATTN_BLOCK * n_b)
+                    rho = Pe.sum(-1) + (16 * n_b + 2) * U * Pw.sum(-1)
+                    e_pre = (num + O.abs() * rho[:, None]) / (1 - rho)[:, None]
+                    e_o = e_pre + R2 * (O.abs() + e_pre)
+                    b_o = ulp(O.abs() + e_o, torch.bfloat16) + e_o
+                    bnd["o"][rows, h] = b_o
+                    a = -torch.log1p(-rho) * LOG2E + 2 * U * torch.log2(vm.sum(-1).double() + 1)
+                    e2 = a + U * (lse.abs() * LOG2E + a)
+                    b_lse = LN2 * e2 + R2 * (lse.abs() + LN2 * e2)
+                    bnd["lse"][h, rows] = b_lse
+                    if do is None:
+                        continue
+                    # ---- backward ----
+                    e_l2 = LOG2E * b_lse * (1 + R2) + R2 * LOG2E * lse.abs()
+                    e_xc = cl * (e_s * (1 + R3) + R3 * sc.abs())
+                    y = (t2 - lse[:, None] * LOG2E).abs()
+                    err_y = e_xc + e_l2[:, None] + U * (y + e_xc + e_l2[:, None])
+                    Pbe = torch.where(vm, P * torch.expm1(LN2 * err_y + 4 * U) + 2.0**-126, zero)
+                    e_dp = gemm_accum_error(dO.abs() @ aV.t(), d)
+                    aOh = O.abs() + b_o
+                    e_delta = (dO.abs() * b_o).sum(-1) + 8 * U * (dO.abs() * aOh).sum(-1)
+                    e_g = e_dp + e_delta[:, None]
+                    gabs = (dP - delta[:, None]).abs()
+                    e_dS = c * (Pbe * (gabs + e_g) + P * e_g) + R4 * c * (P + Pbe) * (dP.abs() + delta.abs()[:, None] + e_g)
+                    e_dS = torch.where(vm, e_dS + U_BF16 * (dS.abs() + e_dS), zero)
+                    aS = dS.abs() + e_dS
+                    e_P = Pbe + U_BF16 * (P + Pbe)
+                    aP = P + e_P
+                    e_q = e_dS @ aK + gemm_accum_error(aS @ aK, ATTN_BLOCK * n_b)
+                    bnd["dq"][rows, h] = ulp(ref["dq"][rows, h].abs() + e_q, torch.bfloat16) + e_q
+                    eK += e_dS.t() @ Q.abs()
+                    mK += aS.t() @ Q.abs()
+                    eV += e_P.t() @ dO.abs()
+                    mV += aP.t() @ dO.abs()
+            if do is None:
+                continue
+            ref["dk"][s0:e0, g] = dK
+            ref["dv"][s0:e0, g] = dV
+            if bounds:
+                K_kv = rep * ATTN_BLOCK * n_b  # products each dK / dV accumulator sums: every query row of every head
+                for name, R, e, m in (("dk", dK, eK, mK), ("dv", dV, eV, mV)):
+                    e = e + gemm_accum_error(m, K_kv)
+                    bnd[name][s0:e0, g] = ulp(R.abs() + e, torch.bfloat16) + e
+    return ref, bnd
+
+
+def attention_reference(q, k, v, do=None, cu_seqlens=None, causal=True, window=None, scale=None, mask=None,
+                        kv_heads=None):
+    """Float64 training attention from explicit formulas.  ``q [T, Hq, d]``, ``k / v [T, Hkv, d]`` and ``do [T, Hq, d]``
+    (any dtype or strides); query head h reads kv head ``h // (Hq / Hkv)``.  Each document of ``cu_seqlens`` (one
+    sequence of T rows when None) is attended on its own; row i of a document sees key j when ``j <= i`` (causal) and
+    ``i - window < j`` (a window).  ``mask`` (bool ``[T, T]``) replaces that rule inside each document.
+
+    With ``t = scale * q k^T`` over the visible keys: ``P = softmax(t)``, ``O = P V``, ``LSE = logsumexp(t)`` (natural
+    log) and for the upstream ``do``: ``dP = do V^T``, ``delta = rowsum(do * O)``, ``dS = P (dP - delta) scale``,
+    ``dQ = dS K``, ``dK = dS^T Q`` and ``dV = P^T do``, with dK and dV summed over the query heads of a group.
+
+    Returns a dict of float64 tensors ``o [T, Hq, d]``, ``lse [Hq, T]`` and, with ``do``, ``dq``, ``dk``, ``dv``.
+    Only the kv heads in ``kv_heads`` (all when None) and their query heads are computed; the rest stay 0."""
+    return _attention(q, k, v, do, cu_seqlens, causal, window, scale, mask, kv_heads, False)[0]
+
+
+def attention_bounds(q, k, v, do=None, cu_seqlens=None, causal=True, window=None, scale=None, kv_heads=None):
+    """``(ref, bound)``: :func:`attention_reference` and per-element bounds on the outputs of ``attn_sm90.cu``, as dicts
+    with the same keys.  Heads left out by ``kv_heads`` get bound inf.  Every term is a magnitude times unit roundoffs
+    (``U = 2**-24`` for fp32, ``U_BF16 = 2**-8`` for bf16); ``n_b = ceil(L / 64)`` blocks bound the keys (or query
+    rows per head) a kernel visits, and ``_rel(n)`` is ``n`` fp32 roundings compounded.
+
+    Forward, per (query row, head), with ``t`` in the log2 domain and ``P`` relative to the kernel's running max:
+
+    1. ``S = Q K^T`` sums d bf16 products in fp32: :func:`gemm_accum_error`.
+    2. ``x = s * scale_log2``: ``scale_log2`` is ``fp32(fp32(scale) * fp32(log2 e))``, three roundings, and the product
+       one more: ``_rel(4) |s|`` on top of the accumulation error.
+    3. ``p = ex2.approx(x - m)``: 2 ulp (``4U`` relative) plus ``ln2 U |x - m|`` from rounding the argument (the model
+       :func:`swiglu_reference` uses for ``__expf``); results below ``2**-126`` flush to zero.  ``|x - m|`` for any
+       running max is at most the row's max minus x.
+    4. Each key block rescales o and l by the same ``alpha = ex2(m_old - m_new)``.  The common factor cancels in
+       ``o / l``, but blocks seen earlier carry more factors than later ones, so per block the ex2's ``4U`` and its
+       argument's ``ln2 U |m_old - m_new|`` weigh p unevenly; the increments of the running max add up to the row's span.
+       The two products round once each per block: ``5U`` per block in all, as a relative error of p.
+    5. l sums the *unrounded* fp32 p: at most ``16 n_b + 2`` adds per thread (16 keys per block, two quad shuffles).
+    6. ``O += P V`` uses p rounded to bf16: ``U_BF16 P |V|``.  This mismatch with l does not cancel and dominates.
+       The fp32 accumulation runs over ``64 n_b`` keys.
+    7. ``1 / l`` (IEEE) and the multiply round once each, then the bf16 rounding of O (one :func:`ulp`).
+    8. ``LSE = (m + log2f(l)) ln2``: l's relative error ``rho`` becomes ``-log2(1 - rho)``; log2f is exact to 1 ulp
+       (``2U |log2 l|``, ``l <= n_visible + 1``), the add rounds once and the product with ``fp32(ln 2)`` twice.
+
+    Backward:
+
+    9. The prep pass forms ``delta`` from the bf16 O the forward wrote: ``|O_bf16 - O| |dO|`` against the float64 delta,
+       plus 8 roundings (three fmaf after an exact first product, five warp-tree adds) of ``|O_bf16| |dO|``.
+    10. ``lse2 = lse * fp32(log2 e)`` rounds twice, on top of the forward's LSE error.
+    11. ``p = ex2(fmaf(s, scale_log2, -lse2))``: the score error as in 1-2 with one fewer rounding (fmaf fuses the
+        product), the lse2 error, the fmaf's rounding of its result, and ex2's ``4U``; an LSE error is a relative
+        error of P.
+    12. ``dP = dO V^T`` sums d products in fp32.
+    13. ``dS = p (dP - delta) scale`` rounds at the subtraction, both products and ``fp32(scale)``: ``_rel(4)`` of
+        ``p (|dP| + |delta|)`` -- the subtraction's rounding scales with its operands, not with ``|dP - delta|``.
+    14. P and dS are rounded to bf16 before their MMAs.
+    15. dV and dK accumulate ``rep * 64 n_b`` products in fp32 (every query row of every head of the group), dQ
+        ``64 n_b`` (every key); each output rounds to bf16 once."""
+    return _attention(q, k, v, do, cu_seqlens, causal, window, scale, None, kv_heads, True)
+
+
+def assert_attention_bounded(got, q, k, v, do=None, cu_seqlens=None, causal=True, window=None, scale=None,
+                             kv_heads=None, what="attention"):
+    """Every output in ``got`` (a dict with any of ``o [T, Hq, d]``, ``lse [Hq, T]``, ``dq``, ``dk``, ``dv``) lies inside
+    :func:`attention_bounds`.  Returns the worst ``err / bound`` per output."""
+    ref, bnd = attention_bounds(q, k, v, do, cu_seqlens, causal, window, scale, kv_heads)
+    worst = {}
+    for name, out in got.items():
+        out = out.to(ref[name].device).double()
+        assert_within(out, ref[name], bnd[name], f"{what}: {name}")
+        worst[name] = float(((out - ref[name]).abs() / bnd[name]).nan_to_num(0.0).max())
+    return worst
+
+
+def attention_emulation(q, k, v, do=None, cu_seqlens=None, causal=True, window=None, scale=None, mask=None):
+    """The kernels' algorithm in torch fp32, with the same arguments and outputs as :func:`attention_reference`: scores
+    in fp32 scaled by the fp32 ``scale * log2 e`` and exponentiated with exp2, P rounded to bf16 before ``P V`` while l
+    sums the fp32 p, ``LSE = (m + log2 l) ln 2``; the backward recomputes P from the LSE, forms delta from the bf16 O,
+    rounds dS and P to bf16 and accumulates in fp32.  O, dQ, dK and dV are bf16, the LSE fp32."""
+    T, Hq, d = q.shape
+    Hkv = k.shape[1]
+    rep = Hq // Hkv
+    c = torch.tensor(1.0 / math.sqrt(d) if scale is None else float(scale), dtype=torch.float32)
+    c2 = c * torch.tensor(LOG2E, dtype=torch.float32)
+    ln2 = torch.tensor(LN2, dtype=torch.float32)
+    l2e = torch.tensor(LOG2E, dtype=torch.float32)
+    f32 = dict(dtype=torch.float32, device=q.device)
+    c, c2, ln2, l2e = (x.to(q.device) for x in (c, c2, ln2, l2e))
+    o = torch.zeros(T, Hq, d, **f32)
+    lse = torch.zeros(Hq, T, **f32)
+    if do is not None:
+        dq = torch.zeros(T, Hq, d, **f32)
+        dk = torch.zeros(T, Hkv, d, **f32)
+        dv = torch.zeros(T, Hkv, d, **f32)
+    bf = lambda x: x.bfloat16().float()  # noqa: E731
+    for s0, e0 in attention_documents(T, cu_seqlens):
+        L = e0 - s0
+        vm = mask[s0:e0, s0:e0] if mask is not None else attention_visible(L, causal, window, q.device)
+        for h in range(Hq):
+            g = h // rep
+            Q, K, V = q[s0:e0, h].float(), k[s0:e0, g].float(), v[s0:e0, g].float()
+            S = Q @ K.t()
+            x = (S * c2).masked_fill(~vm, -math.inf)
+            m = x.max(-1, keepdim=True).values
+            m = torch.where(torch.isfinite(m), m, 0.0)
+            p = torch.exp2(x - m)
+            l = p.sum(-1, keepdim=True)
+            oh = bf((bf(p) @ V) * torch.where(l > 0, 1 / l, 0.0))
+            o[s0:e0, h] = oh
+            lh = ((m + torch.log2(l)) * ln2).squeeze(-1)
+            lse[h, s0:e0] = lh
+            if do is None:
+                continue
+            dO = do[s0:e0, h].float()
+            pb = torch.where(vm, torch.exp2(S * c2 - (lh * l2e)[:, None]), 0.0)
+            dP = dO @ V.t()
+            delta = (oh * dO).sum(-1, keepdim=True)
+            dS = bf(pb * (dP - delta) * c)
+            dq[s0:e0, h] = dS @ K
+            dk[s0:e0, g] += dS.t() @ Q
+            dv[s0:e0, g] += bf(pb).t() @ dO
+    out = {"o": o.bfloat16(), "lse": lse}
+    if do is not None:
+        out.update(dq=dq.bfloat16(), dk=dk.bfloat16(), dv=dv.bfloat16())
+    return out
+
+
+ATTN_FAMILIES = ("diffuse", "peaked", "rescale", "uniform")
+
+
+def attention_data(family, T, hq, hkv, d, gen):
+    """bf16 ``(q [T, hq, d], k / v [T, hkv, d], do [T, hq, d])`` on ``gen``'s device for one data family:
+
+    * ``diffuse``: ``randn * 0.7`` -- logits of std 0.5, a flat softmax;
+    * ``peaked``: q and k ``randn * 2.4`` -- logits of std 5.8, a few keys carry each row;
+    * ``rescale``: column 0 of k rises from -88 to 88 along the rows and q's column 0 is 88, so the scores rise along
+      the keys (about +-1000 in the log2 domain at d = 128), the running max moves in every 64-key block, and the
+      other columns add ``randn * 0.5``;
+    * ``uniform``: K = 0, every visible key weighs the same and O is the mean of the visible V."""
+    dev = gen.device
+    rn = lambda *s: torch.randn(*s, generator=gen, device=dev)  # noqa: E731
+    v, do = rn(T, hkv, d), rn(T, hq, d)
+    if family == "diffuse":
+        q, k, v = rn(T, hq, d) * 0.7, rn(T, hkv, d) * 0.7, v * 0.7
+    elif family == "peaked":
+        q, k = rn(T, hq, d) * 2.4, rn(T, hkv, d) * 2.4
+    elif family == "rescale":
+        q, k = rn(T, hq, d) * 0.5, rn(T, hkv, d) * 0.5
+        q[:, :, 0] = 88.0
+        k[:, :, 0] = torch.linspace(-88.0, 88.0, T, device=dev)[:, None]
+    elif family == "uniform":
+        q, k = rn(T, hq, d), torch.zeros(T, hkv, d, device=dev)
+    else:
+        raise ValueError(family)
+    return tuple(x.bfloat16() for x in (q, k, v, do))
