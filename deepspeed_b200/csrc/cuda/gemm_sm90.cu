@@ -12,8 +12,8 @@
 //   * grouped (MoE) form: the tile list is built on the device from the expert offsets (no host synchronisation)
 //   * ragged (dropless MoE training) forms: the grouped form with every epilogue and an MN-major B whose expert offset
 //     lies on K, plus a variable-K weight-gradient form whose tile (expert, m, n) sums only its expert's rows
-//   * tensorwise-scaled FP8 form (gemm_fp8_kernel, dsb_gemm_fp8): e4m3 / e5m2 K-major operands, 128 x 128 tiles, every
-//     128-product k-block promoted into an fp32 accumulator, the same epilogues
+//   * tensorwise- or blockwise-scaled FP8 form (gemm_fp8_kernel, dsb_gemm_fp8 / dsb_gemm_fp8_block): e4m3 / e5m2 K-major
+//     operands, 128 x 128 tiles, every 128-product k-block promoted into an fp32 accumulator, the same epilogues
 //   * OPTIONAL fused all-gather: when `ag` is given, the weight matrix B is being assembled in local memory from the
 //     other ranks' ZeRO shards *by this same kernel*: `ag.comm_ctas` CTAs pull the peers' shard bytes over NVLink
 //     (peer-mapped addresses) chunk by chunk and publish a per-chunk ready flag (st.release.gpu); the producer of each
@@ -540,7 +540,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
     }
 }
 
-// ---- FP8 (tensorwise-scaled) GEMM ---------------------------------------------------------------------------------------
+// ---- FP8 (tensorwise- or blockwise-scaled) GEMM ---------------------------------------------------------------------------------------
 // C[M, N] (bf16) = epi(sa_inv * sb_inv * A[M, K] B[N, K]^T) with A e4m3 / e5m2 and B e4m3, both K-major (fp8 wgmma reads
 // K-major shared operands only).  A stage is [128 rows x 128 B] of A and of B: the same [64 x 128 B] swizzled boxes, the
 // same `desc_kmajor_sw128` and the same 32-byte step per k32 wgmma as the bf16 kernel's.
@@ -557,10 +557,16 @@ constexpr uint32_t F8_STAGE_BYTES = 4 * F8_BOX;     // A: 2 boxes, B: 2 boxes
 static_assert(F8_STAGES * F8_STAGE_BYTES <= SMEM_BAR, "the fp8 ring must fit below the barriers");
 
 // EPI_SWIGLU: a tile's 128 B rows are 64 gate rows and the 64 up rows of the same features (N = inter, inter % 64 == 0)
-template <int AE5M2, int EPI>
+//
+// BLOCK (blockwise scaling): sa_inv [ceil(K/128), M] (row stride ld_sa) holds one scale per row of A and k-block, sb_inv
+// [ceil(rows of B / 128), ceil(K/128)] (row stride ld_sb) one per 128 x 128 block of B.  The scale granularity is the
+// k-block and the tile the kernel walks anyway, so the promotion's FADD becomes an FFMA with
+// sa_inv[kb, row] * sb_inv[n-block, kb] and the epilogue applies no scale.  A SwiGLU tile's gate and up rows lie in two
+// different 128-row blocks of B (inter % 64 == 0 keeps each 64-row box inside one), so it carries two B scales.
+template <int AE5M2, int EPI, bool BLOCK = false>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
-                const EpiParams ep, const float* sa_inv, const float* sb_inv)
+                const EpiParams ep, const float* sa_inv, const float* sb_inv, int ld_sa = 0, int ld_sb = 0)
 {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -622,7 +628,8 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     const int r_in = 64 * wg + 16 * (warp & 3) + (lane >> 2);
     const int c_in = 2 * (lane & 3);
     // both scales are powers of two, so the product and the rescaling below are exact; a NaN scale makes C NaN
-    const float scale = *sa_inv * *sb_inv;
+    float scale = 1.f;  // BLOCK: the scales are applied in the promotion
+    if constexpr (!BLOCK) scale = *sa_inv * *sb_inv;
     int stage = 0;
     uint32_t phase = 0;
     float acc[64], part[64];
@@ -632,7 +639,28 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
         const int row0 = m_blk * BM, col0 = n_blk * TN;
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+        // BLOCK: the thread's two rows of sa_inv (a row past M reads row M - 1; it is never stored) and the tile's
+        // n-block(s) of sb_inv
+        const float* sa_p = sa_inv;
+        const float* sb_p = sb_inv;
+        int a_off = 0, b_off = 0;
+        if constexpr (BLOCK) {
+            const int ra = min(row0 + r_in, M - 1);
+            sa_p += ra;
+            a_off = min(row0 + r_in + 8, M - 1) - ra;
+            sb_p += static_cast<int64_t>(col0 / F8_BN) * ld_sb;
+            if constexpr (EPI == EPI_SWIGLU) b_off = ((ep.inter + col0) / F8_BN - col0 / F8_BN) * ld_sb;
+        }
         for (int kb = 0; kb < num_k; ++kb) {
+            // s[2 h + i]: the scale of row r_in + 8 i in column half h (the two halves differ for SwiGLU only); loaded
+            // before the wait so the loads are not behind the k-block's wgmmas
+            float s[4];
+            if constexpr (BLOCK) {
+                const float* sa_kb = sa_p + static_cast<int64_t>(kb) * ld_sa;
+                const float a0 = __ldg(sa_kb), a1 = __ldg(sa_kb + a_off);
+                const float b0 = __ldg(sb_p + kb), b1 = EPI == EPI_SWIGLU ? __ldg(sb_p + b_off + kb) : b0;
+                s[0] = a0 * b0, s[1] = a1 * b0, s[2] = a0 * b1, s[3] = a1 * b1;
+            }
             mbar_wait(full_bar(stage), phase);
             const uint32_t sa = sbase + stage * F8_STAGE_BYTES + wg * F8_BOX, sb = sbase + stage * F8_STAGE_BYTES + 2 * F8_BOX;
             const uint64_t da = desc_kmajor_sw128(sa), db = desc_kmajor_sw128(sb);
@@ -643,8 +671,13 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
             wgmma_wait<0>();
             fence_regs<64>(part);
             if (lane == 0) mbar_arrive(empty_bar(stage));
+            if constexpr (BLOCK) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i) acc[i] += part[i];
+                for (int i = 0; i < 64; ++i) acc[i] = fmaf(part[i], s[2 * (i >> 5) + ((i >> 1) & 1)], acc[i]);
+            } else {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc[i] += part[i];
+            }
             if (++stage == F8_STAGES) {
                 stage = 0;
                 phase ^= 1;
@@ -972,40 +1005,27 @@ DSB_EXPORT int dsb_gemm_ragged_wgrad_bf16(const void* a, const void* b, void* c,
                       : launch_kernel<true, true, EPI_STORE, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream);
 }
 
-template <int AE5M2, int EPI>
+template <int AE5M2, int EPI, bool BLOCK>
 static int launch_fp8(const CUtensorMap& ma, const CUtensorMap& mb, int M, int N, int K, int grid, const EpiParams& ep,
-                      const float* sa_inv, const float* sb_inv, cudaStream_t stream)
+                      const float* sa_inv, const float* sb_inv, int ld_sa, int ld_sb, cudaStream_t stream)
 {
     static bool attr = false;
     if (!attr) {
-        cudaError_t e =
-            cudaFuncSetAttribute(gemm_fp8_kernel<AE5M2, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
+        cudaError_t e = cudaFuncSetAttribute(gemm_fp8_kernel<AE5M2, EPI, BLOCK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             SMEM_TOTAL);
         if (e != cudaSuccess) return static_cast<int>(e);
         attr = true;
     }
-    gemm_fp8_kernel<AE5M2, EPI><<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, sa_inv, sb_inv);
+    gemm_fp8_kernel<AE5M2, EPI, BLOCK><<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, sa_inv, sb_inv, ld_sa, ld_sb);
     DSB_CHECK_LAUNCH();
     return 0;
 }
 
-// Tensorwise-scaled FP8 GEMM:  C[M, N] (bf16) = epi(s * A[M, K] B[N, K]^T),  s = *sa_inv * *sb_inv  (device fp32 scalars,
-// read by the kernel: no host synchronisation).  Both operands are row-major and K-major: a [M, K] (lda), b [N, K] (ldb),
-// one byte per element.  a_fmt is the A format, 5 = e4m3 or 6 = e5m2 (the dtype codes of dsb_common.cuh); B is e4m3.
-// Every k-block of 128 products is added into an fp32 accumulator with ordinary FADDs (see the kernel: a block the tensor
-// core sums exactly gives an exact result for any K); the scaled result rounds once to bf16 (ACCUM: C_old + s * sum rounds
-// once).  A NaN scale inverse gives NaN outputs.
-//   epi 0 STORE   C = s AB^T
-//   epi 1 ACCUM   C = C + s AB^T
-//   epi 2 SWIGLU  A e4m3; b = [gate; up] [2N, K]; C [M, N] = silu(g) * u of g|u = s AB^T; out2 (nullable) [M, 2N] = g|u
-//   epi 3 DSWIGLU A e5m2; d = s AB^T [M, N]; aux = saved gate|up [M, 2N]; out2 [M, 2N] = dgate|dup, C its left half
-//                 (c == out2, ldc == ld_out2)
-// group_m: 128-row m-blocks per rasterisation super-group (<= 0: column-major tile order); sms <= 0: all SMs.
-// Host-checked (-2, nothing launched): M, N, K >= 1; K % 16 == 0; N % 8 == 0 (SWIGLU: N % 64 == 0); lda and ldb
-// multiples of 16 and >= K; ldc, ld_aux, ld_out2 multiples of 8 and ldc >= N; a, b, c, aux, out2 16-byte aligned;
-// sa_inv and sb_inv not null; a_fmt 5 or 6 and, for SWIGLU, 5, for DSWIGLU, 6; DSWIGLU with aux and out2; epi in 0..3.
-DSB_EXPORT int dsb_gemm_fp8(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc, int a_fmt,
-                            const float* sa_inv, const float* sb_inv, int epi, const void* aux, int ld_aux, void* out2,
-                            int ld_out2, int group_m, int sms, cudaStream_t stream)
+// The checks and the launch the two FP8 entry points share (their contracts are written at the entry points).
+template <bool BLOCK>
+static int gemm_fp8_host(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc, int a_fmt,
+                         const float* sa_inv, int ld_sa, const float* sb_inv, int ld_sb, int epi, const void* aux, int ld_aux,
+                         void* out2, int ld_out2, int group_m, int sms, cudaStream_t stream)
 {
     if (M <= 0 || N <= 0 || K <= 0 || K % 16 || N % 8) return -2;
     if (lda % 16 || ldb % 16 || lda < K || ldb < K || ldc % 8 || ldc < N || ld_aux % 8 || ld_out2 % 8) return -2;
@@ -1013,6 +1033,7 @@ DSB_EXPORT int dsb_gemm_fp8(const void* a, const void* b, void* c, int M, int N,
          reinterpret_cast<uintptr_t>(aux) | reinterpret_cast<uintptr_t>(out2)) & 15)
         return -2;
     if (!sa_inv || !sb_inv || (a_fmt != dsb::kF8E4M3 && a_fmt != dsb::kF8E5M2) || epi < 0 || epi > 3) return -2;
+    if (BLOCK && (ld_sa < M || ld_sb < (K + F8_BK - 1) / F8_BK)) return -2;
     const bool e5m2 = a_fmt == dsb::kF8E5M2;
     if (epi == EPI_SWIGLU && (e5m2 || N % 64)) return -2;
     if (epi == EPI_DSWIGLU && (!e5m2 || !aux || !out2)) return -2;
@@ -1036,14 +1057,56 @@ DSB_EXPORT int dsb_gemm_fp8(const void* a, const void* b, void* c, int M, int N,
     if (grid > tiles) grid = static_cast<int>(tiles);
     switch (epi) {
         case EPI_STORE:
-            return e5m2 ? launch_fp8<1, EPI_STORE>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream)
-                        : launch_fp8<0, EPI_STORE>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+            return e5m2 ? launch_fp8<1, EPI_STORE, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream)
+                        : launch_fp8<0, EPI_STORE, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream);
         case EPI_ACCUM:
-            return e5m2 ? launch_fp8<1, EPI_ACCUM>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream)
-                        : launch_fp8<0, EPI_ACCUM>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
-        case EPI_SWIGLU: return launch_fp8<0, EPI_SWIGLU>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
-        default: return launch_fp8<1, EPI_DSWIGLU>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, stream);
+            return e5m2 ? launch_fp8<1, EPI_ACCUM, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream)
+                        : launch_fp8<0, EPI_ACCUM, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream);
+        case EPI_SWIGLU: return launch_fp8<0, EPI_SWIGLU, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream);
+        default: return launch_fp8<1, EPI_DSWIGLU, BLOCK>(ma, mb, M, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream);
     }
+}
+
+// Tensorwise-scaled FP8 GEMM:  C[M, N] (bf16) = epi(s * A[M, K] B[N, K]^T),  s = *sa_inv * *sb_inv  (device fp32 scalars,
+// read by the kernel: no host synchronisation).  Both operands are row-major and K-major: a [M, K] (lda), b [N, K] (ldb),
+// one byte per element.  a_fmt is the A format, 5 = e4m3 or 6 = e5m2 (the dtype codes of dsb_common.cuh); B is e4m3.
+// Every k-block of 128 products is added into an fp32 accumulator with ordinary FADDs (see the kernel: a block the tensor
+// core sums exactly gives an exact result for any K); the scaled result rounds once to bf16 (ACCUM: C_old + s * sum rounds
+// once).  A NaN scale inverse gives NaN outputs.
+//   epi 0 STORE   C = s AB^T
+//   epi 1 ACCUM   C = C + s AB^T
+//   epi 2 SWIGLU  A e4m3; b = [gate; up] [2N, K]; C [M, N] = silu(g) * u of g|u = s AB^T; out2 (nullable) [M, 2N] = g|u
+//   epi 3 DSWIGLU A e5m2; d = s AB^T [M, N]; aux = saved gate|up [M, 2N]; out2 [M, 2N] = dgate|dup, C its left half
+//                 (c == out2, ldc == ld_out2)
+// group_m: 128-row m-blocks per rasterisation super-group (<= 0: column-major tile order); sms <= 0: all SMs.
+// Host-checked (-2, nothing launched): M, N, K >= 1; K % 16 == 0; N % 8 == 0 (SWIGLU: N % 64 == 0); lda and ldb
+// multiples of 16 and >= K; ldc, ld_aux, ld_out2 multiples of 8 and ldc >= N; a, b, c, aux, out2 16-byte aligned;
+// sa_inv and sb_inv not null; a_fmt 5 or 6 and, for SWIGLU, 5, for DSWIGLU, 6; DSWIGLU with aux and out2; epi in 0..3.
+DSB_EXPORT int dsb_gemm_fp8(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc, int a_fmt,
+                            const float* sa_inv, const float* sb_inv, int epi, const void* aux, int ld_aux, void* out2,
+                            int ld_out2, int group_m, int sms, cudaStream_t stream)
+{
+    return gemm_fp8_host<false>(a, b, c, M, N, K, lda, ldb, ldc, a_fmt, sa_inv, 0, sb_inv, 0, epi, aux, ld_aux, out2, ld_out2,
+                                group_m, sms, stream);
+}
+
+// Blockwise-scaled FP8 GEMM:  C[M, N] (bf16) = epi(sum over k-blocks kb of sa_inv[kb, m] * sb_inv[n / 128, kb] *
+// A[m, kb-block] B[n, kb-block]^T): dsb_gemm_fp8 with one scale per 1 x 128 strip of A and one per 128 x 128 block of B
+// (device fp32, the layouts dsb_fp8_cast_block writes) in place of the two scalars.
+//   sa_inv [ceil(K/128), M], row stride ld_sa: row kb holds the scale of every row of A for its columns [128 kb, 128 kb + 128)
+//   sb_inv [ceil(rows of b / 128), ceil(K/128)], row stride ld_sb (SWIGLU: b has 2N rows; the gate rows of a tile use
+//          block row col / 128, its up rows block row (N + col) / 128)
+// A k-block's partial sum is multiplied by its scale as it is added to the fp32 accumulator (one FFMA; exact rescaling,
+// the scales being powers of two), so a block the tensor core sums exactly still gives an exact result.  A NaN in sa_inv
+// makes its row of C NaN, a NaN in sb_inv the columns of its n-block.  Operands, formats, epilogues, group_m, sms and the
+// host checks are those of dsb_gemm_fp8, and (-2, nothing launched) ld_sa >= M and ld_sb >= ceil(K/128).
+DSB_EXPORT int dsb_gemm_fp8_block(const void* a, const void* b, void* c, int M, int N, int K, int lda, int ldb, int ldc,
+                                  int a_fmt, const float* sa_inv, int ld_sa, const float* sb_inv, int ld_sb, int epi,
+                                  const void* aux, int ld_aux, void* out2, int ld_out2, int group_m, int sms,
+                                  cudaStream_t stream)
+{
+    return gemm_fp8_host<true>(a, b, c, M, N, K, lda, ldb, ldc, a_fmt, sa_inv, ld_sa, sb_inv, ld_sb, epi, aux, ld_aux, out2,
+                               ld_out2, group_m, sms, stream);
 }
 
 DSB_EXPORT int dsb_gemm_tile_m() { return BM; }

@@ -52,6 +52,9 @@ class LlamaConfig:
     # tensorwise power-of-two recipe of ``ops/fp8.py``; weights, optimizer, gradients, attention, norms, embedding and
     # LM head stay bf16
     fp8: bool = False
+    # scaling granularity when ``fp8`` is on: "tensorwise" (one scale per tensor) or "blockwise" (1 x 128 strips of
+    # activations and gradients, 128 x 128 blocks of weights: an outlier costs precision in its own block only)
+    fp8_recipe: str = "tensorwise"
     # training knobs
     checkpoint_layers: int = 0  # number of decoder layers (from the front) run with activation recompute
     loss_chunk_tokens: int = 2048
@@ -60,6 +63,8 @@ class LlamaConfig:
     def __post_init__(self):
         if self.head_dim is None:
             self.head_dim = self.hidden_size // self.num_attention_heads
+        if self.fp8_recipe not in ("tensorwise", "blockwise"):
+            raise ValueError(f"fp8_recipe must be 'tensorwise' or 'blockwise', got {self.fp8_recipe!r}")
 
     @property
     def q_size(self):
@@ -139,17 +144,17 @@ class RMSNorm(nn.Module):
 class FlatLinear(nn.Module):
     """``nn.Linear`` whose backward writes dW straight into the ZeRO flat gradient buffer."""
 
-    def __init__(self, in_features, out_features, bias=False, fp8=False):
+    def __init__(self, in_features, out_features, bias=False, fp8=False, fp8_recipe="tensorwise"):
         super().__init__()
         self.in_features, self.out_features = in_features, out_features
         self.weight = nn.Parameter(torch.empty(out_features, in_features))
         self.bias = nn.Parameter(torch.zeros(out_features)) if bias else None
-        self.fp8 = fp8
+        self.fp8, self.fp8_recipe = fp8, fp8_recipe
 
     def forward(self, x):
         if self.fp8:
             from deepspeed_b200.ops.linear import fp8_linear
-            return fp8_linear(x, self.weight, self.bias)
+            return fp8_linear(x, self.weight, self.bias, recipe=self.fp8_recipe)
         return flat_linear(x, self.weight, self.bias)
 
 
@@ -172,8 +177,9 @@ class LlamaAttention(nn.Module):
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
         self.cfg = cfg
-        self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias, fp8=cfg.fp8)
-        self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False, fp8=cfg.fp8)
+        self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias, fp8=cfg.fp8,
+                                   fp8_recipe=cfg.fp8_recipe)
+        self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False, fp8=cfg.fp8, fp8_recipe=cfg.fp8_recipe)
 
     def forward(self, x, rope, positions=None, cu_seqlens=None, max_seqlen=None):
         cfg = self.cfg
@@ -189,16 +195,16 @@ class LlamaMLP(nn.Module):
 
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
-        self.gate_up_proj = FlatLinear(cfg.hidden_size, 2 * cfg.intermediate_size, fp8=cfg.fp8)
-        self.down_proj = FlatLinear(cfg.intermediate_size, cfg.hidden_size, fp8=cfg.fp8)
+        self.gate_up_proj = FlatLinear(cfg.hidden_size, 2 * cfg.intermediate_size, fp8=cfg.fp8, fp8_recipe=cfg.fp8_recipe)
+        self.down_proj = FlatLinear(cfg.intermediate_size, cfg.hidden_size, fp8=cfg.fp8, fp8_recipe=cfg.fp8_recipe)
         self.act = cfg.hidden_act
-        self.fp8 = cfg.fp8
+        self.fp8, self.fp8_recipe = cfg.fp8, cfg.fp8_recipe
 
     def forward(self, x):
         if self.act == "silu" and self.gate_up_proj.bias is None and self.down_proj.bias is None:
             if self.fp8:
                 from deepspeed_b200.ops.linear import fp8_swiglu_mlp
-                return fp8_swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight)
+                return fp8_swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight, recipe=self.fp8_recipe)
             from deepspeed_b200.ops.linear import swiglu_mlp
             return swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight)
         return self.down_proj(T.gated_act(self.gate_up_proj(x), self.act))

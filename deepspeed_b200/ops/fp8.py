@@ -1,5 +1,5 @@
-"""FP8 training recipe: tensorwise current scaling with power-of-two scales (torchao's "tensorwise", with Transformer
-Engine's HYBRID formats).
+"""FP8 training recipes: current scaling with power-of-two scales, one scale per tensor (torchao's "tensorwise", with
+Transformer Engine's HYBRID formats) or one per block (below).
 
 * Activations and weights are ``float8_e4m3fn`` (max 448); gradients flowing backward are ``float8_e5m2`` (max 57344).
 * Each tensor gets one fp32 scale computed on the device from its amax when it is cast: no history, no delayed scaling,
@@ -13,6 +13,14 @@ Engine's HYBRID formats).
 The wgmma path is ``csrc/cuda/fp8_cast.cu`` (amax, cast, cast-transpose) and ``dsb_gemm_fp8`` in ``csrc/cuda/gemm_sm90.cu``.
 The ``*_reference`` functions here do the same casts and scales in torch, with an fp32 matmul: they are the path for
 operands the kernels cannot take (CPU tensors, other dtypes and shapes) and the tests' oracle.
+
+Blockwise recipe (DeepSeek-V3's granularity): the same formats, scale rule and cast, with the amax taken per block --
+one scale per 1 x 128 strip along the contraction for the ``A`` operand of a product (activations, gradients), one per
+128 x 128 block for its ``B`` operand (weights; in the weight gradient, the transposed input).  A trailing partial block
+takes its amax over the elements that exist.  ``C = epi(sum_kb sa_inv[kb, m] * sb_inv[n // 128, kb] * (A8[m, kb] @
+B8[n, kb]^T))``: the block partials are scaled and summed in fp32 and rounded once.  An outlier costs the precision of
+its own strip or block only.  ``dsb_fp8_cast_block`` finds the amaxes inside the tile it casts (one pass, no atomics on
+global memory) and ``dsb_gemm_fp8_block`` applies the scales where it promotes each k-block.
 """
 import torch
 
@@ -67,6 +75,81 @@ def matmul_reference(a8, b8, sa_inv, sb_inv):
     return (a8.float() @ b8.float().t()) * (sa_inv * sb_inv)
 
 
+BLOCK = 128
+
+
+def _block_amax(x, rows, cols):
+    """amax of the fp32 matrix ``x [R, C]`` over blocks of ``rows x cols`` (trailing partial blocks over what exists):
+    ``[ceil(R / rows), ceil(C / cols)]``."""
+    R, C = x.shape
+    rb, cb = -(-R // rows), -(-C // cols)
+    a = torch.zeros(rb * rows, cb * cols, dtype=torch.float32, device=x.device)
+    a[:R, :C] = x.abs()
+    return a.view(rb, rows, cb, cols).permute(0, 2, 1, 3).reshape(rb, cb, -1).amax(dim=2)
+
+
+def quantize_blockwise_reference(x, fmt, row="strip", col=None):
+    """Torch implementation of the blockwise cast of the matrix ``x [R, C]``: ``(q, sq, qt, st)``.
+
+    ``row`` scales the row-major copy ``q [R, C]``: ``"strip"`` -- one scale per 1 x 128 strip of a row (``q`` is the ``A``
+    of a product contracting over ``C``), ``sq [ceil(C/128), R]``; ``"block"`` -- one per 128 x 128 block (``q`` is a
+    ``B``), ``sq [ceil(R/128), ceil(C/128)]``; None -- no row-major copy.  ``col`` scales the transposed copy
+    ``qt [C, R]`` the same way, its strips running along ``R``: ``st [ceil(R/128), C]`` or ``[ceil(C/128), ceil(R/128)]``.
+    The scale tensors hold ``scale_inv`` (fp32).  Strip scales are stored k-block-major, the layout the GEMM reads.  A
+    block of ``x`` and the same block of ``qt`` share a scale, so ``row="block", col="block"`` gives ``st == sq.t()`` and
+    ``qt == q.t()``; with any strip scaling the two copies are different casts of ``x``."""
+    xf = x.float()
+    R, C = xf.shape
+
+    def cast(mode, transposed):
+        if mode is None:
+            return None, None
+        if mode == "block":
+            amax = _block_amax(xf, BLOCK, BLOCK)
+        elif transposed:
+            amax = _block_amax(xf, BLOCK, 1)  # [ceil(R/128), C]
+        else:
+            amax = _block_amax(xf, 1, BLOCK)  # [R, ceil(C/128)]
+        scale, scale_inv = scale_from_amax(amax, fmt)
+        full = scale
+        if amax.shape[0] != R:
+            full = full.repeat_interleave(BLOCK, dim=0)[:R]
+        if amax.shape[1] != C:
+            full = full.repeat_interleave(BLOCK, dim=1)[:, :C]
+        q = (xf * full).to(fmt)
+        if transposed:
+            return q.t().contiguous(), (scale_inv.t().contiguous() if mode == "block" else scale_inv)
+        return q, (scale_inv if mode == "block" else scale_inv.t().contiguous())
+
+    q, sq = cast(row, False)
+    qt, st = cast(col, True)
+    return q, sq, qt, st
+
+
+def quantize_blockwise(x, fmt, row="strip", col=None):
+    """Blockwise cast of the matrix ``x`` (see :func:`quantize_blockwise_reference` for the arguments and the result).
+    CUDA bf16 matrices go through the single-pass native kernel (no amax launch, no host synchronisation); anything
+    else through the reference, which is bit-equal."""
+    if native_cast_ok(x, col is not None):
+        from deepspeed_b200.ops.kernels import fp8_ops
+        return fp8_ops.fp8_cast_block(x, fmt, row=row, col=col)
+    return quantize_blockwise_reference(x, fmt, row, col)
+
+
+def matmul_blockwise_reference(a8, b8, sa_inv, sb_inv):
+    """fp32 ``sum_kb sa_inv[kb, m] * sb_inv[n // 128, kb] * (a8[m, kb] @ b8[n, kb]^T)`` (before the bf16 rounding), one
+    k-block of 128 after the other as the kernel promotes them."""
+    M, K = a8.shape
+    Nn = b8.shape[0]
+    a, b = a8.float(), b8.float()
+    acc = torch.zeros(M, Nn, dtype=torch.float32, device=a8.device)
+    for kb in range(-(-K // BLOCK)):
+        k = slice(kb * BLOCK, min(K, (kb + 1) * BLOCK))
+        s = sa_inv[kb][:, None] * sb_inv[:, kb].repeat_interleave(BLOCK)[:Nn][None, :]
+        acc = acc + (a[:, k] @ b[:, k].t()) * s
+    return acc
+
+
 def silu32(g):
     return g / (1 + torch.exp(-g))
 
@@ -77,12 +160,22 @@ def dsilu32(g):
 
 
 # ---- the products of the two training nodes, on the kernels or in torch -------------------------------------------------
-def gemm(a8, b8, sa, sb, native, out=None, accumulate=False):
+# ``block`` selects the blockwise recipe: ``sa`` / ``sb`` are then the strip and block scale tensors.
+def _native_matmul(block):
+    from deepspeed_b200.ops.kernels import gemm_sm100 as K
+    return K, (K.fp8_matmul_block if block else K.fp8_matmul)
+
+
+def _reference_matmul(block):
+    return matmul_blockwise_reference if block else matmul_reference
+
+
+def gemm(a8, b8, sa, sb, native, out=None, accumulate=False, block=False):
     """bf16 ``[M, N]`` = ``sa sb a8 b8^T`` (``accumulate``: added to ``out`` before the one rounding)."""
     if native:
-        from deepspeed_b200.ops.kernels import gemm_sm100 as K
-        return K.fp8_matmul(a8, b8, sa, sb, out=out, epi=K.EPI_ACCUM if accumulate else K.EPI_STORE)
-    c = matmul_reference(a8, b8, sa, sb)
+        K, mm = _native_matmul(block)
+        return mm(a8, b8, sa, sb, out=out, epi=K.EPI_ACCUM if accumulate else K.EPI_STORE)
+    c = _reference_matmul(block)(a8, b8, sa, sb)
     if accumulate:
         c = c + out.float()
     if out is None:
@@ -90,26 +183,26 @@ def gemm(a8, b8, sa, sb, native, out=None, accumulate=False):
     return out.copy_(c)
 
 
-def gemm_swiglu(a8, b8, sa, sb, native, save_gate_up=True):
+def gemm_swiglu(a8, b8, sa, sb, native, save_gate_up=True, block=False):
     """``(act [M, I], gate|up [M, 2I] or None)`` for ``b8 = [gate; up] [2I, K]``: silu applied to the fp32 products."""
     if native:
-        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        K, mm = _native_matmul(block)
         I = b8.shape[0] // 2
         gu = torch.empty(a8.shape[0], 2 * I, dtype=torch.bfloat16, device=a8.device) if save_gate_up else None
-        return K.fp8_matmul(a8, b8, sa, sb, epi=K.EPI_SWIGLU, out2=gu), gu
-    gu = matmul_reference(a8, b8, sa, sb)
+        return mm(a8, b8, sa, sb, epi=K.EPI_SWIGLU, out2=gu), gu
+    gu = _reference_matmul(block)(a8, b8, sa, sb)
     g, u = gu.chunk(2, dim=1)
     return (silu32(g) * u).to(torch.bfloat16), (gu.to(torch.bfloat16) if save_gate_up else None)
 
 
-def gemm_dswiglu(a8, b8, sa, sb, gu, native):
+def gemm_dswiglu(a8, b8, sa, sb, gu, native, block=False):
     """dgate|dup ``[M, 2I]`` (bf16) for the SwiGLU whose gate|up ``gu`` was saved: ``d = sa sb a8 b8^T`` in fp32, then
     ``dgate = d * u * silu'(g)`` and ``dup = d * silu(g)``."""
     if native:
-        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        K, mm = _native_matmul(block)
         out2 = torch.empty(gu.shape, dtype=torch.bfloat16, device=gu.device)
-        K.fp8_matmul(a8, b8, sa, sb, epi=K.EPI_DSWIGLU, aux=gu, out2=out2)
+        mm(a8, b8, sa, sb, epi=K.EPI_DSWIGLU, aux=gu, out2=out2)
         return out2
-    d = matmul_reference(a8, b8, sa, sb)
+    d = _reference_matmul(block)(a8, b8, sa, sb)
     g, u = gu.float().chunk(2, dim=1)
     return torch.cat([d * u * dsilu32(g), d * silu32(g)], dim=1).to(torch.bfloat16)

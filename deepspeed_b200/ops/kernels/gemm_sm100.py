@@ -217,6 +217,44 @@ def fp8_matmul(a, b, sa_inv, sb_inv, out=None, epi=EPI_STORE, aux=None, out2=Non
     return out
 
 
+def fp8_matmul_block(a, b, sa_inv, sb_inv, out=None, epi=EPI_STORE, aux=None, out2=None, group_m=8, sms=0):
+    """Blockwise-scaled FP8 GEMM (``dsb_gemm_fp8_block``): :func:`fp8_matmul` with ``sa_inv [ceil(K/128), M]`` (one scale
+    per row of ``a`` and k-block of 128) and ``sb_inv [ceil(rows of b / 128), ceil(K/128)]`` (one per 128 x 128 block of
+    ``b``) in place of the two scalars; each k-block's partial product is scaled as it is promoted,
+    ``out = epi(sum_kb sa_inv[kb, m] * sb_inv[n // 128, kb] * a[m, kb] @ b[n, kb]^T)``.  Operands, epilogues and outputs
+    are those of :func:`fp8_matmul`."""
+    fmt = {torch.float8_e4m3fn: N.F8E4M3, torch.float8_e5m2: N.F8E5M2}.get(a.dtype)
+    M, K = a.shape if a.dim() == 2 else (0, 0)
+    Nn = b.shape[0] // 2 if epi == EPI_SWIGLU else b.shape[0]
+    kb = -(-K // 128)
+    bad = (fmt is None or b.dtype != torch.float8_e4m3fn or a.dim() != 2 or b.dim() != 2 or b.shape[1] != K
+           or (epi == EPI_SWIGLU and b.shape[0] != 2 * Nn) or a.stride(1) != 1 or b.stride(1) != 1
+           or sa_inv is None or sb_inv is None or sa_inv.dtype != torch.float32 or sb_inv.dtype != torch.float32
+           or tuple(sa_inv.shape) != (kb, M) or tuple(sb_inv.shape) != (-(-b.shape[0] // 128), kb)
+           or sa_inv.stride(1) != 1 or sb_inv.stride(1) != 1)
+    if out is not None:
+        bad = bad or tuple(out.shape) != (M, Nn) or out.dtype != torch.bfloat16 or out.stride(1) != 1
+    if out2 is not None:
+        bad = bad or tuple(out2.shape) != (M, 2 * Nn) or out2.dtype != torch.bfloat16 or out2.stride(1) != 1
+    if aux is not None:
+        bad = bad or tuple(aux.shape) != (M, 2 * Nn) or aux.dtype != torch.bfloat16 or aux.stride(1) != 1
+    if epi == EPI_DSWIGLU:
+        bad = bad or aux is None or out2 is None
+    if epi == EPI_ACCUM:
+        bad = bad or out is None
+    if bad:
+        raise N.NativeOpError(f"gemm_fp8_block: a {tuple(a.shape)} {a.dtype}, b {tuple(b.shape)} {b.dtype}, the scales and "
+                              f"the outputs do not fit together (epi={epi})")
+    if out is None:
+        out = out2[:, :Nn] if epi == EPI_DSWIGLU else torch.empty(M, Nn, dtype=torch.bfloat16, device=a.device)
+    rc = N.cuda().dsb_gemm_fp8_block(N.ptr(a), N.ptr(b), N.ptr(out), M, Nn, K, a.stride(0), b.stride(0), out.stride(0), fmt,
+                                     N.ptr(sa_inv), sa_inv.stride(0), N.ptr(sb_inv), sb_inv.stride(0), int(epi), N.ptr(aux),
+                                     aux.stride(0) if aux is not None else 0, N.ptr(out2),
+                                     out2.stride(0) if out2 is not None else 0, int(group_m), sms, N.stream())
+    N.check(rc, "gemm_fp8_block")
+    return out
+
+
 def supports_2cta(a, b, a_mn, b_mn, out=None) -> bool:
     ok = lambda t: (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 8 == 0
                     and t.data_ptr() % 16 == 0 and t.shape[1] % 8 == 0)

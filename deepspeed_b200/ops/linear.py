@@ -158,19 +158,19 @@ def _fp8_cast_fn(native):
     return fp8.quantize_tensorwise if native else fp8.quantize_reference
 
 
-def _fp8_weight_grad(w, a8t, b8t, sa, sb, native):
-    """dW = sa sb a8t b8t^T (``a8t`` the e5m2 gradient transposed, ``b8t`` the e4m3 input transposed): stored, or
-    accumulated on later micro steps, straight into the ZeRO flat gradient view when there is one (returns None), else
-    returned for autograd."""
+def _fp8_weight_grad(w, a8t, b8t, sa, sb, native, block=False):
+    """dW = sa sb a8t b8t^T (``a8t`` the e5m2 gradient transposed, ``b8t`` the e4m3 input transposed; ``block``: scaled
+    blockwise): stored, or accumulated on later micro steps, straight into the ZeRO flat gradient view when there is one
+    (returns None), else returned for autograd."""
     from deepspeed_b200.ops import fp8
     zo = _zo_of(w)
     if zo is None:
-        return fp8.gemm(a8t, b8t, sa, sb, native).to(w.dtype)
+        return fp8.gemm(a8t, b8t, sa, sb, native, block=block).to(w.dtype)
     gv = zo.grad_view_for(w)
     if gv.dtype == torch.bfloat16:
-        fp8.gemm(a8t, b8t, sa, sb, native, out=gv, accumulate=not zo.grad_is_fresh(w))
+        fp8.gemm(a8t, b8t, sa, sb, native, out=gv, accumulate=not zo.grad_is_fresh(w), block=block)
     else:
-        g = fp8.gemm(a8t, b8t, sa, sb, native)
+        g = fp8.gemm(a8t, b8t, sa, sb, native, block=block)
         gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
     zo.mark_grad_ready(w)
     return None
@@ -222,9 +222,74 @@ class _FP8LinearFn(torch.autograd.Function):
         return dx, dw, db
 
 
-def fp8_linear(x, weight, bias=None):
-    """``x W^T (+ b)`` with FP8 products (see :class:`_FP8LinearFn`).  CUDA bf16 operands whose dimensions are multiples
-    of 16 run the wgmma kernels; anything else runs the torch reference of the same recipe (never a bf16 product)."""
+FP8_RECIPES = ("tensorwise", "blockwise")
+
+
+def _check_recipe(recipe):
+    if recipe not in FP8_RECIPES:
+        raise ValueError(f"fp8 recipe must be one of {FP8_RECIPES}, got {recipe!r}")
+
+
+def _fp8_block_cast_fn(native):
+    from deepspeed_b200.ops import fp8
+    return fp8.quantize_blockwise if native else fp8.quantize_blockwise_reference
+
+
+class _FP8BlockLinearFn(torch.autograd.Function):
+    """:class:`_FP8LinearFn` under the blockwise recipe of :mod:`deepspeed_b200.ops.fp8`.  The ``A`` of each product is
+    scaled in 1 x 128 strips along its contraction, the ``B`` in 128 x 128 blocks:
+
+    forward  ``x`` -> e4m3 strips (and, in the same pass, ``x^T`` in blocks for dW, the only copy saved); ``W`` in blocks;
+    dgrad    ``dY`` -> e5m2 strips along the output features; ``W^T`` in blocks, cast from the re-read weight;
+    wgrad    ``dY^T`` -> e5m2 strips along the tokens (same pass as dgrad's copy, different scales); saved ``x^T``."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias):
+        from deepspeed_b200.ops import fp8
+        x2 = x.reshape(-1, x.shape[-1])
+        native = _fp8_native(x2, weight)
+        cast = _fp8_block_cast_fn(native)
+        x8, sx, x8t, sxt = cast(x2, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[1] else None)
+        w8, sw, _, _ = cast(weight, fp8.E4M3, row="block")
+        y = fp8.gemm(x8, w8, sx, sw, native, block=True).to(x.dtype)
+        if bias is not None:
+            y = y + bias
+        ctx.weight_ref = weight
+        ctx.has_bias = bias is not None
+        ctx.native = native
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.save_for_backward(x8t, sxt)
+        return y.view(*x.shape[:-1], weight.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops import fp8
+        x8t, sxt = ctx.saved_tensors
+        w, native = ctx.weight_ref, ctx.native
+        cast = _fp8_block_cast_fn(native)
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        dx = dw = None
+        if need_dx or need_dw:
+            dy8, sdy, dy8t, sdyt = cast(dy2, fp8.E5M2, row="strip" if need_dx else None, col="strip" if need_dw else None)
+            if need_dx:
+                _, _, w8t, swt = cast(w, fp8.E4M3, row=None, col="block")
+                dx = fp8.gemm(dy8, w8t, sdy, swt, native, block=True).to(ctx.x_dtype).view(ctx.x_shape)
+            if need_dw:
+                dw = _fp8_weight_grad(w, dy8t, x8t, sdyt, sxt, native, block=True)
+        db = dy2.sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
+        return dx, dw, db
+
+
+def fp8_linear(x, weight, bias=None, recipe="tensorwise"):
+    """``x W^T (+ b)`` with FP8 products (see :class:`_FP8LinearFn`; ``recipe="blockwise"``:
+    :class:`_FP8BlockLinearFn`).  CUDA bf16 operands whose dimensions are multiples of 16 run the wgmma kernels; anything
+    else runs the torch reference of the same recipe (never a bf16 product)."""
+    _check_recipe(recipe)
+    if recipe == "blockwise":
+        return _FP8BlockLinearFn.apply(x, weight, bias)
     return _FP8LinearFn.apply(x, weight, bias)
 
 
@@ -285,10 +350,66 @@ class _FP8SwiGLUMLPFn(torch.autograd.Function):
         return dx, dw_gu, dw_down
 
 
-def fp8_swiglu_mlp(x, w_gate_up, w_down):
-    """SwiGLU MLP block (no biases) with FP8 products: see :class:`_FP8SwiGLUMLPFn`.  CUDA bf16 operands with
-    ``T, H, 2I`` multiples of 16 and ``I % 64 == 0`` run the wgmma kernels; anything else runs the torch reference of the
-    same recipe (never a bf16 product)."""
+class _FP8BlockSwiGLUMLPFn(torch.autograd.Function):
+    """:class:`_FP8SwiGLUMLPFn` under the blockwise recipe, operand by operand as in :class:`_FP8BlockLinearFn`: the row-major
+    casts (``x``, ``act``, ``dY``, ``dgate|dup``) are scaled in 1 x 128 strips, the weights and the saved ``x^T`` and
+    ``act^T`` in 128 x 128 blocks, ``dY^T`` and ``dgate|dup^T`` in strips along the tokens.  The same order of weight
+    reads and gradient marks."""
+
+    @staticmethod
+    def forward(ctx, x, w_gu, w_down):
+        from deepspeed_b200.ops import fp8
+        x2 = x.reshape(-1, x.shape[-1])
+        native = _fp8_native(x2, w_gu, w_down, inter=w_down.shape[1])
+        cast = _fp8_block_cast_fn(native)
+        need_grad = any(ctx.needs_input_grad)
+        x8, sx, x8t, sxt = cast(x2, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[1] else None)
+        wgu8, sgu, _, _ = cast(w_gu, fp8.E4M3, row="block")
+        act, gu = fp8.gemm_swiglu(x8, wgu8, sx, sgu, native, save_gate_up=need_grad, block=True)
+        act8, sa, act8t, sat = cast(act, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[2] else None)
+        wd8, sd, _, _ = cast(w_down, fp8.E4M3, row="block")
+        y = fp8.gemm(act8, wd8, sa, sd, native, block=True).to(x.dtype)
+        ctx.w_gu, ctx.w_down, ctx.native = w_gu, w_down, native
+        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
+        ctx.save_for_backward(x8t, sxt, gu, act8t, sat)
+        return y.view(*x.shape[:-1], w_down.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops import fp8
+        x8t, sxt, gu, act8t, sat = ctx.saved_tensors
+        w_gu, w_down, native = ctx.w_gu, ctx.w_down, ctx.native
+        cast = _fp8_block_cast_fn(native)
+        need_dx, need_dgu, need_dd = ctx.needs_input_grad
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        dy8, sdy, dy8t, sdyt = cast(dy2, fp8.E5M2, row="strip", col="strip" if need_dd else None)
+        _, _, wd8t, sdt = cast(w_down, fp8.E4M3, row=None, col="block")
+        dgu = fp8.gemm_dswiglu(dy8, wd8t, sdy, sdt, gu, native, block=True)
+        wgu8t = sgut = None
+        if need_dx:
+            _, _, wgu8t, sgut = cast(w_gu, fp8.E4M3, row=None, col="block")
+        dx = dw_gu = dw_down = None
+        if need_dx or need_dgu:
+            dgu8, sg, dgu8t, sgt = cast(dgu, fp8.E5M2, row="strip" if need_dx else None, col="strip" if need_dgu else None)
+            if need_dx:
+                dx = fp8.gemm(dgu8, wgu8t, sg, sgut, native, block=True).to(ctx.x_dtype).view(ctx.x_shape)
+        # weights are not read past this point
+        if need_dd:
+            dw_down = _fp8_weight_grad(w_down, dy8t, act8t, sdyt, sat, native, block=True)
+        if need_dgu:
+            dw_gu = _fp8_weight_grad(w_gu, dgu8t, x8t, sgt, sxt, native, block=True)
+        return dx, dw_gu, dw_down
+
+
+def fp8_swiglu_mlp(x, w_gate_up, w_down, recipe="tensorwise"):
+    """SwiGLU MLP block (no biases) with FP8 products: see :class:`_FP8SwiGLUMLPFn` (``recipe="blockwise"``:
+    :class:`_FP8BlockSwiGLUMLPFn`).  CUDA bf16 operands with ``T, H, 2I`` multiples of 16 and ``I % 64 == 0`` run the
+    wgmma kernels; anything else runs the torch reference of the same recipe (never a bf16 product)."""
+    _check_recipe(recipe)
+    if recipe == "blockwise":
+        return _FP8BlockSwiGLUMLPFn.apply(x, w_gate_up, w_down)
     return _FP8SwiGLUMLPFn.apply(x, w_gate_up, w_down)
 
 
