@@ -13,7 +13,8 @@
 //   * ragged (dropless MoE training) forms: the grouped form with every epilogue and an MN-major B whose expert offset
 //     lies on K, plus a variable-K weight-gradient form whose tile (expert, m, n) sums only its expert's rows
 //   * tensorwise- or blockwise-scaled FP8 form (gemm_fp8_kernel, dsb_gemm_fp8 / dsb_gemm_fp8_block): e4m3 / e5m2 K-major
-//     operands, 128 x 128 tiles, every 128-product k-block promoted into an fp32 accumulator, the same epilogues
+//     operands, 128 x 128 tiles, every 128-product k-block promoted into an fp32 accumulator, the same epilogues; and
+//     its ragged forms (dsb_gemm_fp8_ragged / dsb_gemm_fp8_ragged_wgrad) on the same tile walk, with 128-row segments
 //   * OPTIONAL fused all-gather: when `ag` is given, the weight matrix B is being assembled in local memory from the
 //     other ranks' ZeRO shards *by this same kernel*: `ag.comm_ctas` CTAs pull the peers' shard bytes over NVLink
 //     (peer-mapped addresses) chunk by chunk and publish a per-chunk ready flag (st.release.gpu); the producer of each
@@ -237,18 +238,19 @@ struct Tile {
     int k0, nk, crow0;
 };
 
-// Ragged forms: offsets[0..E] must be non-decreasing multiples of 64 inside [0, rows].  Anything else could send a TMA
-// load into another expert's K rows or a store past the output, so the kernel refuses it before it does anything.
+// Ragged forms: offsets[0..E] must be non-decreasing multiples of the segment granule GRAN (the kernel's k-block: 64 rows
+// bf16, 128 rows FP8) inside [0, rows].  Anything else could send a TMA load into another expert's K rows or a store
+// past the output, so the kernel refuses it before it does anything.
 // kPrefix (m-tiled form): the same pass fills prefix[1..E] with the running count of (m-tile x nn n-tiles).
-template <bool kPrefix>
+template <bool kPrefix, int GRAN>
 __device__ __forceinline__ bool ragged_walk(const int* off, int E, int rows, int nn, int* prefix)
 {
     int prev = off[0];
-    if (prev < 0 || (prev & (BK - 1))) return false;
+    if (prev < 0 || (prev & (GRAN - 1))) return false;
     int acc = 0;
     for (int e = 1; e <= E; ++e) {
         const int cur = off[e];
-        if (cur < prev || (cur & (BK - 1))) return false;
+        if (cur < prev || (cur & (GRAN - 1))) return false;
         if (kPrefix) {
             acc += ((cur - prev + BM - 1) / BM) * nn;
             prefix[e] = acc;
@@ -258,10 +260,11 @@ __device__ __forceinline__ bool ragged_walk(const int* off, int E, int rows, int
     return prev <= rows;
 }
 
-template <int EPI, int MODE>
+// TBN: B rows per tile (256 bf16, 128 FP8); KB: rows per k-block of the variable-K form (= the segment granule).
+template <int EPI, int MODE, int TBN = BN, int KB = BK>
 struct Sched {
     static constexpr bool kGrouped = MODE == MODE_GROUPED || MODE == MODE_RAGGED;  // m-tiles per expert
-    static constexpr int TN = (EPI == EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
+    static constexpr int TN = (EPI == EPI_SWIGLU) ? TBN / 2 : TBN;  // output columns per tile
     int num_m, num_n, num_tiles, group_m, n_rot, M, N, K;
     const int* offsets;
     const int* prefix;  // grouped: tile_prefix in shared memory
@@ -317,7 +320,7 @@ struct Sched {
                 t.b1 = t.b0 + inter;
             } else {
                 t.b0 = e * N + t.col0;
-                t.b1 = t.b0 + BN / 2;
+                t.b1 = t.b0 + TBN / 2;
             }
             if (MODE == MODE_RAGGED) t.k0 = e * K;  // MN-major B [E, K, N]
             return t;
@@ -330,10 +333,10 @@ struct Sched {
             n_blk = local / num_m;
             t.row0 = m_blk * BM;
             t.rows = M - t.row0;
-            t.col0 = n_blk * BN;
+            t.col0 = n_blk * TBN;
             t.crow0 = e * M + t.row0;
             t.k0 = offsets[e];
-            t.nk = (offsets[e + 1] - t.k0) / BK;
+            t.nk = (offsets[e + 1] - t.k0) / KB;
             return t;
         }
         tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
@@ -342,7 +345,7 @@ struct Sched {
         t.rows = M - t.row0;
         t.col0 = n_blk * TN;
         t.b0 = t.col0;
-        t.b1 = (EPI == EPI_SWIGLU) ? inter + t.col0 : t.col0 + BN / 2;
+        t.b1 = (EPI == EPI_SWIGLU) ? inter + t.col0 : t.col0 + TBN / 2;
         return t;
     }
 };
@@ -375,7 +378,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ C
         // well formed, -1 when not -- then the whole CTA leaves before any barrier exists and writes nothing
         if (threadIdx.x == kConsumerThreads) {
             const int nn = (N + Sched<EPI, MODE>::TN - 1) / Sched<EPI, MODE>::TN;
-            tile_prefix[0] = ragged_walk<MODE == MODE_RAGGED>(ep.offsets, ep.E, MODE == MODE_RAGGED ? M : K, nn, tile_prefix)
+            tile_prefix[0] = ragged_walk<MODE == MODE_RAGGED, BK>(ep.offsets, ep.E, MODE == MODE_RAGGED ? M : K, nn,
+                                                                  tile_prefix)
                                  ? 0
                                  : -1;
         }
@@ -563,7 +567,17 @@ static_assert(F8_STAGES * F8_STAGE_BYTES <= SMEM_BAR, "the fp8 ring must fit bel
 // k-block and the tile the kernel walks anyway, so the promotion's FADD becomes an FFMA with
 // sa_inv[kb, row] * sb_inv[n-block, kb] and the epilogue applies no scale.  A SwiGLU tile's gate and up rows lie in two
 // different 128-row blocks of B (inter % 64 == 0 keeps each 64-row box inside one), so it carries two B scales.
-template <int AE5M2, int EPI, bool BLOCK = false>
+//
+// MODE (the dropless MoE forms; segments are 128-row aligned, so no k-block, strip or block straddles two experts):
+//   MODE_PLAIN      one [M, N] product
+//   MODE_RAGGED     m-tiles per expert over expert-sorted rows A [M, K].  The A format picks the B addressing: e4m3
+//                   (forward) B is the stacked weight viewed [E * Nb, K] and expert e's rows start at e * Nb (SwiGLU:
+//                   gate rows at e * 2I + col0, up rows at e * 2I + I + col0); e5m2 (dgrad) B is the transposed cast of
+//                   that view, [N, E * K], and expert e's W^T is the column slab at K coordinate e * K.  Blockwise B
+//                   scales are indexed the same way: block row (e * Nb + col0) / 128, or block column e * K / 128 + kb.
+//   MODE_RAGGED_K   dW[e] = A_e B_e^T over expert e's rows only: A [M, R] and B [N, R] (the transposed casts), tiles
+//                   (e, m, n), k-blocks [off[e] / 128, off[e+1] / 128); strip row and block column off[e] / 128 + kb.
+template <int AE5M2, int EPI, bool BLOCK = false, int MODE = MODE_PLAIN>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int M, int N, int K,
                 const EpiParams ep, const float* sa_inv, const float* sb_inv, int ld_sa = 0, int ld_sb = 0)
@@ -574,14 +588,25 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     const uint32_t bar_base = sbase + SMEM_BAR;
     auto full_bar = [&](int s) { return bar_base + 8 * s; };
     auto empty_bar = [&](int s) { return bar_base + 8 * (F8_STAGES + s); };
+    int* tile_prefix = reinterpret_cast<int*>(smem + SMEM_GRP);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    constexpr int TN = EPI == EPI_SWIGLU ? F8_BN / 2 : F8_BN;  // output columns per tile
-    const int num_m = (M + BM - 1) / BM, num_n = (N + TN - 1) / TN;
-    const int num_tiles = num_m * num_n;
-    const int group_m = ep.group_m > 0 ? ep.group_m : num_m;
-    const int num_k = (K + F8_BK - 1) / F8_BK;
+    using S = Sched<EPI, MODE, F8_BN, F8_BK>;
+    constexpr bool kOff = MODE == MODE_RAGGED && AE5M2;  // dgrad: the expert offset lies on B's K coordinate
+    constexpr bool kVarK = MODE == MODE_RAGGED_K;
+
+    if constexpr (MODE == MODE_RAGGED || MODE == MODE_RAGGED_K) {
+        // as in gemm_kernel: malformed offsets make every CTA leave before any barrier exists, writing nothing
+        if (threadIdx.x == kConsumerThreads) {
+            const int nn = (N + S::TN - 1) / S::TN;
+            tile_prefix[0] = ragged_walk<MODE == MODE_RAGGED, F8_BK>(ep.offsets, ep.E, kVarK ? K : M, nn, tile_prefix)
+                                 ? 0
+                                 : -1;
+        }
+        __syncthreads();
+        if (tile_prefix[0] != 0) return;
+    }
 
     if (threadIdx.x == kConsumerThreads) {
         prefetch_map(&map_a);
@@ -594,25 +619,30 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     }
     __syncthreads();
 
+    const AgParams no_ag{};
+    S sch;
+    sch.init(ep, no_ag, M, N, K, tile_prefix);
+    const int num_k = (K + F8_BK - 1) / F8_BK;
+
     if (threadIdx.x >= kConsumerThreads) {
         setmaxnreg_dec<kProducerRegs>();
         if (threadIdx.x == kConsumerThreads) {
             int stage = 0;
             uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                int m_blk, n_blk;
-                tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
-                const int row0 = m_blk * BM, col0 = n_blk * TN;
-                const int b0 = col0, b1 = EPI == EPI_SWIGLU ? ep.inter + col0 : col0 + 64;
-                for (int kb = 0; kb < num_k; ++kb) {
+            for (int tile = blockIdx.x; tile < sch.num_tiles; tile += gridDim.x) {
+                const Tile t = sch.at(tile, ep.inter);
+                const int b0 = kOff || kVarK ? t.col0 : t.b0, b1 = kOff || kVarK ? t.col0 + 64 : t.b1;
+                const int ka0 = kVarK ? t.k0 : 0, kb0 = kOff || kVarK ? t.k0 : 0;
+                const int nk = kVarK ? t.nk : num_k;
+                for (int kb = 0; kb < nk; ++kb) {
                     mbar_wait(empty_bar(stage), phase ^ 1);
                     const uint32_t sa = sbase + stage * F8_STAGE_BYTES, sb = sa + 2 * F8_BOX;
                     const uint32_t fb = full_bar(stage);
                     mbar_expect_tx(fb, F8_STAGE_BYTES);
-                    tma_load_2d(sa, &map_a, fb, kb * F8_BK, row0);
-                    tma_load_2d(sa + F8_BOX, &map_a, fb, kb * F8_BK, row0 + 64);
-                    tma_load_2d(sb, &map_b, fb, kb * F8_BK, b0);
-                    tma_load_2d(sb + F8_BOX, &map_b, fb, kb * F8_BK, b1);
+                    tma_load_2d(sa, &map_a, fb, ka0 + kb * F8_BK, t.row0);
+                    tma_load_2d(sa + F8_BOX, &map_a, fb, ka0 + kb * F8_BK, t.row0 + 64);
+                    tma_load_2d(sb, &map_b, fb, kb0 + kb * F8_BK, b0);
+                    tma_load_2d(sb + F8_BOX, &map_b, fb, kb0 + kb * F8_BK, b1);
                     if (++stage == F8_STAGES) {
                         stage = 0;
                         phase ^= 1;
@@ -633,10 +663,9 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
     int stage = 0;
     uint32_t phase = 0;
     float acc[64], part[64];
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_blk, n_blk;
-        tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
-        const int row0 = m_blk * BM, col0 = n_blk * TN;
+    for (int tile = blockIdx.x; tile < sch.num_tiles; tile += gridDim.x) {
+        const Tile t = sch.at(tile, ep.inter);
+        const int nk = kVarK ? t.nk : num_k;
 #pragma unroll
         for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         // BLOCK: the thread's two rows of sa_inv (a row past M reads row M - 1; it is never stored) and the tile's
@@ -645,13 +674,16 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
         const float* sb_p = sb_inv;
         int a_off = 0, b_off = 0;
         if constexpr (BLOCK) {
-            const int ra = min(row0 + r_in, M - 1);
+            const int ra = min(t.row0 + r_in, M - 1);
             sa_p += ra;
-            a_off = min(row0 + r_in + 8, M - 1) - ra;
-            sb_p += static_cast<int64_t>(col0 / F8_BN) * ld_sb;
-            if constexpr (EPI == EPI_SWIGLU) b_off = ((ep.inter + col0) / F8_BN - col0 / F8_BN) * ld_sb;
+            a_off = min(t.row0 + r_in + 8, M - 1) - ra;
+            const int brow = kOff || kVarK ? t.col0 : t.b0;
+            sb_p += static_cast<int64_t>(brow / F8_BN) * ld_sb;
+            if constexpr (EPI == EPI_SWIGLU) b_off = (t.b1 / F8_BN - t.b0 / F8_BN) * ld_sb;
+            if constexpr (kVarK) sa_p += static_cast<int64_t>(t.k0 / F8_BK) * ld_sa;
+            if constexpr (kOff || kVarK) sb_p += t.k0 / F8_BK;
         }
-        for (int kb = 0; kb < num_k; ++kb) {
+        for (int kb = 0; kb < nk; ++kb) {
             // s[2 h + i]: the scale of row r_in + 8 i in column half h (the two halves differ for SwiGLU only); loaded
             // before the wait so the loads are not behind the k-block's wgmmas
             float s[4];
@@ -684,19 +716,28 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
             }
         }
 
+        // an expert without rows (variable K): its dW is zero (STORE; acc is, and a NaN scale must not reach it) or unchanged
+        float tscale = scale;
+        if constexpr (kVarK) {
+            if (nk == 0) {
+                if constexpr (EPI == EPI_ACCUM) continue;
+                tscale = 0.f;
+            }
+        }
+
         // ---- epilogue from the accumulators: thread holds rows r_in (+8), column pairs c_in + 8 j ----
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const int lr = r_in + 8 * i;
-            if (row0 + lr >= M) continue;
-            const int64_t grow = row0 + lr;
+            if (lr >= t.rows) continue;
+            const int64_t grow = (kVarK ? t.crow0 : t.row0) + lr;
             if constexpr (EPI == EPI_SWIGLU) {
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    const int col = col0 + 8 * j + c_in;
+                    const int col = t.col0 + 8 * j + c_in;
                     if (col >= N) continue;
-                    const float g0 = acc[4 * j + 2 * i] * scale, g1 = acc[4 * j + 2 * i + 1] * scale;
-                    const float u0 = acc[4 * (j + 8) + 2 * i] * scale, u1 = acc[4 * (j + 8) + 2 * i + 1] * scale;
+                    const float g0 = acc[4 * j + 2 * i] * tscale, g1 = acc[4 * j + 2 * i + 1] * tscale;
+                    const float u0 = acc[4 * (j + 8) + 2 * i] * tscale, u1 = acc[4 * (j + 8) + 2 * i + 1] * tscale;
                     st_bf16x2(ep.c + grow * ep.ldc + col, silu_f(g0) * u0, silu_f(g1) * u1);
                     if (ep.out2 != nullptr) {
                         st_bf16x2(ep.out2 + grow * ep.ld_out2 + col, g0, g1);
@@ -706,9 +747,9 @@ gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant
             } else {
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
-                    const int col = col0 + 8 * j + c_in;
+                    const int col = t.col0 + 8 * j + c_in;
                     if (col >= N) continue;
-                    float v0 = acc[4 * j + 2 * i] * scale, v1 = acc[4 * j + 2 * i + 1] * scale;
+                    float v0 = acc[4 * j + 2 * i] * tscale, v1 = acc[4 * j + 2 * i + 1] * tscale;
                     __nv_bfloat16* dst = ep.c + grow * ep.ldc + col;
                     if constexpr (EPI == EPI_ACCUM) {
                         const float2 o = ld_bf16x2(dst);
@@ -1005,18 +1046,19 @@ DSB_EXPORT int dsb_gemm_ragged_wgrad_bf16(const void* a, const void* b, void* c,
                       : launch_kernel<true, true, EPI_STORE, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, ag, stream);
 }
 
-template <int AE5M2, int EPI, bool BLOCK>
+template <int AE5M2, int EPI, bool BLOCK, int MODE = MODE_PLAIN>
 static int launch_fp8(const CUtensorMap& ma, const CUtensorMap& mb, int M, int N, int K, int grid, const EpiParams& ep,
                       const float* sa_inv, const float* sb_inv, int ld_sa, int ld_sb, cudaStream_t stream)
 {
     static bool attr = false;
     if (!attr) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_fp8_kernel<AE5M2, EPI, BLOCK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             SMEM_TOTAL);
+        cudaError_t e = cudaFuncSetAttribute(gemm_fp8_kernel<AE5M2, EPI, BLOCK, MODE>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL);
         if (e != cudaSuccess) return static_cast<int>(e);
         attr = true;
     }
-    gemm_fp8_kernel<AE5M2, EPI, BLOCK><<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, sa_inv, sb_inv, ld_sa, ld_sb);
+    gemm_fp8_kernel<AE5M2, EPI, BLOCK, MODE>
+        <<<grid, kThreads, SMEM_TOTAL, stream>>>(ma, mb, M, N, K, ep, sa_inv, sb_inv, ld_sa, ld_sb);
     DSB_CHECK_LAUNCH();
     return 0;
 }
@@ -1107,6 +1149,116 @@ DSB_EXPORT int dsb_gemm_fp8_block(const void* a, const void* b, void* c, int M, 
 {
     return gemm_fp8_host<true>(a, b, c, M, N, K, lda, ldb, ldc, a_fmt, sa_inv, ld_sa, sb_inv, ld_sb, epi, aux, ld_aux, out2,
                                ld_out2, group_m, sms, stream);
+}
+
+// ---- ragged (dropless MoE training) FP8 forms ----------------------------------------------------------------------
+// The contract of the bf16 ragged forms (expert-sorted rows, int32 device offsets [E + 1], zero-padded segments, rows
+// outside [offsets[0], offsets[E]) neither read into a result nor written, malformed device offsets refused by the
+// kernel, which then writes nothing) with a 128-row segment granule: every offset is a multiple of 128, the FP8 k-block,
+// so no k-block, scale strip or scale block straddles two experts.  Scales are those of dsb_gemm_fp8 (block == 0: two
+// device scalars; a stacked weight is one tensor with one scale) or dsb_gemm_fp8_block (block == 1), indexed by the
+// tile's expert as the kernel's MODE comment says.
+
+// m-tiled ragged FP8 GEMM, c [rows, N] (ldc) from a [rows, K] (lda), for each expert e and its rows r:
+//   a e4m3 (forward):  b = the stacked weight viewed [E * Nb, K] (ldb), c[r] = epi(a[r] b_e^T) with b_e its rows
+//                      [e Nb, (e+1) Nb); epi STORE (Nb = N) or SWIGLU (Nb = 2N: gate rows, then up rows; out2 = gate|up
+//                      [rows, 2N], nullable)
+//   a e5m2 (dgrad):    b = the transposed cast of that view, [N, E * K] (ldb), c[r] = epi(a[r] b_e^T) with b_e its
+//                      columns [e K, (e+1) K); epi STORE or DSWIGLU (aux = saved gate|up [rows, 2N], out2 = dgate|dup
+//                      [rows, 2N], c its left half)
+// block == 1: sa_inv [ceil(K/128), rows] (ld_sa), sb_inv the block scales of b as dsb_fp8_cast_block writes them (ld_sb).
+// Host-checked (-2, nothing launched): 1 <= E <= 256, N >= 1, K >= 16, K % 16 == 0, N % 8 == 0 (SWIGLU: N % 64 == 0),
+// dgrad K % 128 == 0, blockwise forward STORE N % 128 == 0; lda, ldb multiples of 16 with lda >= K and ldb >= K
+// (dgrad: E * K); ldc, ld_aux, ld_out2 multiples of 8, ldc >= N; 16-byte aligned pointers; offsets, sa_inv and sb_inv
+// not null; the epilogue allowed for the A format; block: ld_sa >= rows and ld_sb >= the k-blocks of b.
+DSB_EXPORT int dsb_gemm_fp8_ragged(const void* a, const void* b, void* c, const int* offsets, int rows, int E, int N, int K,
+                                   int lda, int ldb, int ldc, int a_fmt, const float* sa_inv, int ld_sa,
+                                   const float* sb_inv, int ld_sb, int epi, const void* aux, int ld_aux, void* out2,
+                                   int ld_out2, int block, int sms, cudaStream_t stream)
+{
+    if (rows < 0 || E < 1 || E > kMaxGroups || N <= 0 || K <= 0 || K % 16 || N % 8) return -2;
+    if (lda % 16 || ldb % 16 || lda < K || ldc % 8 || ldc < N || ld_aux % 8 || ld_out2 % 8) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
+         reinterpret_cast<uintptr_t>(aux) | reinterpret_cast<uintptr_t>(out2)) & 15)
+        return -2;
+    if (!offsets || !sa_inv || !sb_inv || (a_fmt != dsb::kF8E4M3 && a_fmt != dsb::kF8E5M2)) return -2;
+    const bool dgrad = a_fmt == dsb::kF8E5M2;
+    if (dgrad ? (epi != EPI_STORE && epi != EPI_DSWIGLU) : (epi != EPI_STORE && epi != EPI_SWIGLU)) return -2;
+    if (epi == EPI_SWIGLU && N % 64) return -2;
+    if (epi == EPI_DSWIGLU && (!aux || !out2)) return -2;
+    const uint64_t e = static_cast<uint64_t>(E);
+    const uint64_t b_rows = dgrad ? N : e * (epi == EPI_SWIGLU ? 2 * N : N), b_cols = dgrad ? e * K : K;
+    if (dgrad && K % F8_BK) return -2;
+    if (static_cast<uint64_t>(ldb) < b_cols) return -2;
+    if (block && (ld_sa < rows || static_cast<uint64_t>(ld_sb) < (b_cols + F8_BK - 1) / F8_BK ||
+                  (!dgrad && epi == EPI_STORE && N % F8_BN)))
+        return -2;
+    if (rows == 0) return 0;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map_fp8(&ma, a, rows, K, lda, 64))) return rc;
+    if ((rc = make_map_fp8(&mb, b, b_rows, b_cols, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.aux = static_cast<const __nv_bfloat16*>(aux);
+    ep.out2 = static_cast<__nv_bfloat16*>(out2);
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ld_aux = ld_aux;
+    ep.ld_out2 = ld_out2;
+    ep.ldc = ldc;
+    ep.inter = N;
+    ep.offsets = offsets;
+    ep.E = E;
+    int grid = sms > 0 ? sms : sm_count();
+    const int tn = epi == EPI_SWIGLU ? F8_BN / 2 : F8_BN;
+    const int64_t max_tiles = (static_cast<int64_t>(rows + BM - 1) / BM + E) * ((N + tn - 1) / tn);
+    if (grid > max_tiles) grid = static_cast<int>(max_tiles);
+#define DSB_F8R(AF, EP, BL) \
+    launch_fp8<AF, EP, BL, MODE_RAGGED>(ma, mb, rows, N, K, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream)
+    if (block) {
+        if (dgrad) return epi == EPI_DSWIGLU ? DSB_F8R(1, EPI_DSWIGLU, true) : DSB_F8R(1, EPI_STORE, true);
+        return epi == EPI_SWIGLU ? DSB_F8R(0, EPI_SWIGLU, true) : DSB_F8R(0, EPI_STORE, true);
+    }
+    if (dgrad) return epi == EPI_DSWIGLU ? DSB_F8R(1, EPI_DSWIGLU, false) : DSB_F8R(1, EPI_STORE, false);
+    return epi == EPI_SWIGLU ? DSB_F8R(0, EPI_SWIGLU, false) : DSB_F8R(0, EPI_STORE, false);
+#undef DSB_F8R
+}
+
+// Variable-K FP8 weight gradient: c[e] (+)= a_e b_e^T for every expert, where a_e / b_e are the columns
+// [offsets[e], offsets[e+1]) of a [M, rows] (e5m2, lda) and b [N, rows] (e4m3, ldb) -- the transposed casts of the
+// gradient and of the input -- and c [E, M, N] is contiguous bf16.  One launch of E x ceil(M/128) x ceil(N/128) tiles;
+// a tile sums its expert's k-blocks only.  An expert without rows gets c[e] = 0, or keeps c[e] with `accumulate`.
+// block == 1: sa_inv [ceil(rows/128), M] (ld_sa; strips along the rows), sb_inv [ceil(N/128), ceil(rows/128)] (ld_sb).
+// Host-checked (-2): rows >= 1, M, N >= 1 with N % 8 == 0, lda and ldb multiples of 16 and >= rows,
+// 16-byte aligned pointers, offsets / sa_inv / sb_inv not null, 1 <= E <= 256; block: ld_sa >= M and
+// ld_sb >= ceil(rows/128).
+DSB_EXPORT int dsb_gemm_fp8_ragged_wgrad(const void* a, const void* b, void* c, const int* offsets, int rows, int E, int M,
+                                         int N, int lda, int ldb, const float* sa_inv, int ld_sa, const float* sb_inv,
+                                         int ld_sb, int accumulate, int block, int sms, cudaStream_t stream)
+{
+    if (rows < 1 || E < 1 || E > kMaxGroups || M <= 0 || N <= 0 || N % 8) return -2;
+    if (lda % 16 || ldb % 16 || lda < rows || ldb < rows) return -2;
+    if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) return -2;
+    if (!offsets || !sa_inv || !sb_inv) return -2;
+    if (block && (ld_sa < M || ld_sb < (rows + F8_BK - 1) / F8_BK)) return -2;
+    CUtensorMap ma, mb;
+    int rc;
+    if ((rc = make_map_fp8(&ma, a, M, rows, lda, 64))) return rc;
+    if ((rc = make_map_fp8(&mb, b, N, rows, ldb, 64))) return rc;
+    EpiParams ep;
+    memset(&ep, 0, sizeof(ep));
+    ep.c = static_cast<__nv_bfloat16*>(c);
+    ep.ldc = N;
+    ep.offsets = offsets;
+    ep.E = E;
+    int grid = sms > 0 ? sms : sm_count();
+    const int64_t tiles = static_cast<int64_t>(E) * ((M + BM - 1) / BM) * ((N + F8_BN - 1) / F8_BN);
+    if (grid > tiles) grid = static_cast<int>(tiles);
+#define DSB_F8K(EP, BL) \
+    launch_fp8<1, EP, BL, MODE_RAGGED_K>(ma, mb, M, N, rows, grid, ep, sa_inv, sb_inv, ld_sa, ld_sb, stream)
+    if (block) return accumulate ? DSB_F8K(EPI_ACCUM, true) : DSB_F8K(EPI_STORE, true);
+    return accumulate ? DSB_F8K(EPI_ACCUM, false) : DSB_F8K(EPI_STORE, false);
+#undef DSB_F8K
 }
 
 DSB_EXPORT int dsb_gemm_tile_m() { return BM; }

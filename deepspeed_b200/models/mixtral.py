@@ -24,6 +24,15 @@ class MixtralConfig(LlamaConfig):
     ep_size: int = 1
     capacity_factor: float = 1.25
     drop_tokens: bool = True
+    # FP8 products in the experts (gate|up with SwiGLU, down; forward, dgrad and wgrad) under ``fp8_recipe``, independent
+    # of ``fp8`` (which keeps meaning the attention projections).  Dropless routing on one expert-parallel rank only
+    fp8_experts: bool = False
+
+    def __post_init__(self):
+        super().__post_init__()
+        if self.fp8_experts and (self.drop_tokens or self.ep_size > 1):
+            raise ValueError("fp8_experts=True needs the dropless layout on one expert-parallel rank (drop_tokens=False, "
+                             f"ep_size=1); got drop_tokens={self.drop_tokens}, ep_size={self.ep_size}")
 
 
 MIXTRAL_PRESETS = {
@@ -50,7 +59,8 @@ class MixtralDecoderLayer(nn.Module):
         self.self_attn = LlamaAttention(cfg)
         self.post_attention_layernorm = RMSNorm(cfg.hidden_size, cfg.rms_norm_eps)
         assert cfg.num_local_experts % cfg.ep_size == 0
-        experts = GroupedSwiGLUExperts(cfg.num_local_experts // cfg.ep_size, cfg.hidden_size, cfg.intermediate_size)
+        experts = GroupedSwiGLUExperts(cfg.num_local_experts // cfg.ep_size, cfg.hidden_size, cfg.intermediate_size,
+                                       fp8_recipe=cfg.fp8_recipe if cfg.fp8_experts else None)
         self.block_sparse_moe = MoE(cfg.hidden_size, experts, num_experts=cfg.num_local_experts, ep_size=cfg.ep_size,
                                     k=cfg.num_experts_per_tok, capacity_factor=cfg.capacity_factor,
                                     eval_capacity_factor=cfg.capacity_factor, min_capacity=4,

@@ -269,12 +269,17 @@ class MOELayer(nn.Module):
                     raise TypeError(f"dropless routing (drop_tokens=False) with ep_size == 1 takes user expert modules "
                                     f"(wrapped in Experts) or GroupedSwiGLUExperts; {type(self.experts).__name__} is a "
                                     f"grouped container that does not take the (rows, offsets) layout")
-                # grouped experts: every expert's segment padded to a multiple of 64 rows (zero-filled by the scatter), the
-                # offsets built on the device and the buffer sized by its static bound T*k + E*63 -- no host
-                # synchronisation in forward or backward
-                seg = (g.counts + 63) // 64 * 64
+                # grouped experts: every expert's segment padded to a multiple of the experts' row granule (64 rows bf16,
+                # 128 FP8; zero-filled by the scatter), the offsets built on the device and the buffer sized by its
+                # static bound T*k + E*(granule - 1) -- no host synchronisation in forward or backward.  FP8 rounds that
+                # bound up to a multiple of 128: the transposed casts of the rows need R % 16
+                align = self.experts.row_align
+                seg = (g.counts + align - 1) // align * align
                 offsets = torch.cat([seg.new_zeros(1), torch.cumsum(seg, 0, dtype=torch.int32)])
-                rows, slots = moe_ops.scatter(flat, g.expert_ids, g.positions, offsets, k, 0, T * k + E * 63)
+                R = T * k + E * (align - 1)
+                if self.experts.fp8_recipe is not None:
+                    R = -(-R // 128) * 128
+                rows, slots = moe_ops.scatter(flat, g.expert_ids, g.positions, offsets, k, 0, R)
                 eo = self.experts((rows, offsets))
             y = moe_ops.gather(eo, g.weights.to(torch.float32), slots, T, k)
             return y.reshape(x.shape).to(x.dtype)

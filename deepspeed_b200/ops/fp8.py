@@ -206,3 +206,111 @@ def gemm_dswiglu(a8, b8, sa, sb, gu, native, block=False):
     d = _reference_matmul(block)(a8, b8, sa, sb)
     g, u = gu.float().chunk(2, dim=1)
     return torch.cat([d * u * dsilu32(g), d * silu32(g)], dim=1).to(torch.bfloat16)
+
+
+# ---- the ragged (dropless MoE) products --------------------------------------------------------------------------------
+# Rows are sorted by expert, expert e owning rows [offsets[e], offsets[e+1]) (multiples of 128).  The stacked weights are
+# cast as one 2-D matrix [E * Nb, K] (and its transpose [K, E * Nb]), so expert e's operand is a row slab of the cast or a
+# column slab of the transposed cast, and its block scales are the matching slab of the scale tensor.  The references
+# below loop over the experts with the offsets read on the host; rows outside the segments come out as zeros there.
+def _host_segments(offsets):
+    off = offsets.tolist()
+    if any(o % BLOCK for o in off) or any(b < a for a, b in zip(off, off[1:])):
+        raise ValueError(f"ragged FP8 segments must start at non-decreasing multiples of {BLOCK} rows, got {off}")
+    return off
+
+
+def _dequant(q, s, mode):
+    """fp32 values of the blockwise cast ``q [R, C]``: ``mode`` "strip" (``s [ceil(C/128), R]``) or "block"."""
+    R, C = q.shape
+    if mode == "strip":
+        return q.float() * s.t().repeat_interleave(BLOCK, dim=1)[:, :C]
+    return q.float() * s.repeat_interleave(BLOCK, dim=0)[:R].repeat_interleave(BLOCK, dim=1)[:, :C]
+
+
+def _expert_operands(a8, b8, sa, sb, e, E, lo, hi, block):
+    """Expert e's operands: its rows of ``a8`` and a row slab of the stacked weight's cast (forward, e4m3 ``a8``) or a
+    column slab of its transposed cast (dgrad, e5m2 ``a8``), with their scales.  Blockwise, the operands come back
+    dequantised (exact in fp32) with unit scales, so a slab need not start on a 128-row block."""
+    one = torch.ones(1, dtype=torch.float32, device=a8.device)
+    if a8.dtype == E5M2:  # dgrad: b8 [N, E K], expert e's columns
+        k = b8.shape[1] // E
+        sl = (slice(None), slice(e * k, (e + 1) * k))
+    else:  # forward: b8 [E Nb, K], expert e's rows
+        n = b8.shape[0] // E
+        sl = (slice(e * n, (e + 1) * n), slice(None))
+    if not block:
+        return a8[lo:hi], b8[sl], sa, sb
+    return _dequant(a8, sa, "strip")[lo:hi], _dequant(b8, sb, "block")[sl], one, one
+
+
+def ragged_gemm(a8, b8, offsets, sa, sb, E, native, block=False):
+    """bf16 ``[R, N]``: ``out[r] = epi_store(sa sb a8[r] b8_e^T)`` for the expert ``e`` of row ``r`` (forward with an e4m3
+    ``a8`` and ``b8 [E N, K]``; dgrad with an e5m2 ``a8`` and ``b8 [N, E K]``)."""
+    if native:
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        return K.fp8_ragged_matmul(a8, b8, offsets, sa, sb, E, block=block)
+    off = _host_segments(offsets)
+    n = b8.shape[0] if a8.dtype == E5M2 else b8.shape[0] // E
+    out = torch.zeros(a8.shape[0], n, dtype=torch.bfloat16, device=a8.device)
+    for e in range(E):
+        if off[e + 1] > off[e]:
+            out[off[e]:off[e + 1]] = gemm(*_expert_operands(a8, b8, sa, sb, e, E, off[e], off[e + 1], block), False)
+    return out
+
+
+def ragged_gemm_swiglu(a8, b8, offsets, sa, sb, E, native, save_gate_up=True, block=False):
+    """``(act [R, I], gate|up [R, 2I] or None)`` for the stacked ``[gate; up]`` weights ``b8 [E 2I, K]``.  ``act`` is zero
+    on the rows outside the segments (its cast reads every row); gate|up is unspecified there."""
+    R, I = a8.shape[0], b8.shape[0] // E // 2
+    act = torch.zeros(R, I, dtype=torch.bfloat16, device=a8.device)
+    gu = torch.empty(R, 2 * I, dtype=torch.bfloat16, device=a8.device) if save_gate_up else None
+    if native:
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        K.fp8_ragged_matmul(a8, b8, offsets, sa, sb, E, out=act, epi=K.EPI_SWIGLU, out2=gu, block=block)
+        return act, gu
+    off = _host_segments(offsets)
+    for e in range(E):
+        lo, hi = off[e], off[e + 1]
+        if hi > lo:
+            act[lo:hi], gue = gemm_swiglu(*_expert_operands(a8, b8, sa, sb, e, E, lo, hi, block), False, save_gate_up)
+            if save_gate_up:
+                gu[lo:hi] = gue
+    return act, gu
+
+
+def ragged_gemm_dswiglu(a8, b8, offsets, sa, sb, gu, E, native, block=False):
+    """dgate|dup ``[R, 2I]`` from the e5m2 ``a8 = dY`` and the transposed down weight ``b8 [I, E H]``; zero on the rows
+    outside the segments (its cast reads every row)."""
+    out2 = torch.zeros(gu.shape, dtype=torch.bfloat16, device=gu.device)
+    if native:
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        K.fp8_ragged_matmul(a8, b8, offsets, sa, sb, E, epi=K.EPI_DSWIGLU, aux=gu, out2=out2, block=block)
+        return out2
+    off = _host_segments(offsets)
+    for e in range(E):
+        lo, hi = off[e], off[e + 1]
+        if hi > lo:
+            out2[lo:hi] = gemm_dswiglu(*_expert_operands(a8, b8, sa, sb, e, E, lo, hi, block), gu[lo:hi], False)
+    return out2
+
+
+def ragged_wgrad(a8t, b8t, offsets, sa, sb, E, native, out=None, accumulate=False, block=False):
+    """``out [E, M, N]`` (bf16): ``out[e] (+)= sa sb a8t[:, rows of e] b8t[:, rows of e]^T`` for the transposed casts
+    ``a8t [M, R]`` (e5m2) and ``b8t [N, R]`` (e4m3); an expert without rows gets zeros or keeps ``out[e]``."""
+    if native:
+        from deepspeed_b200.ops.kernels import gemm_sm100 as K
+        return K.fp8_ragged_wgrad(a8t, b8t, offsets, sa, sb, E, out=out, accumulate=accumulate, block=block)
+    off = _host_segments(offsets)
+    if out is None:
+        out = torch.empty(E, a8t.shape[0], b8t.shape[0], dtype=torch.bfloat16, device=a8t.device)
+    for e in range(E):
+        lo, hi = off[e], off[e + 1]
+        if hi == lo:
+            if not accumulate:
+                out[e].zero_()
+            continue
+        sae = sa[lo // BLOCK:hi // BLOCK] if block else sa
+        sbe = sb[:, lo // BLOCK:hi // BLOCK] if block else sb
+        gemm(a8t[:, lo:hi], b8t[:, lo:hi], sae, sbe, False, out=out[e], accumulate=accumulate, block=block)
+    return out

@@ -255,6 +255,98 @@ def fp8_matmul_block(a, b, sa_inv, sb_inv, out=None, epi=EPI_STORE, aux=None, ou
     return out
 
 
+FP8_RAGGED_ALIGN = 128  # rows per FP8 ragged segment granule: the FP8 k-block, scale strip and scale block
+
+
+def _fp8_scales_ok(s, shape, block):
+    if s is None or s.dtype != torch.float32 or not s.is_cuda:
+        return False
+    if not block:
+        return s.numel() == 1
+    return tuple(s.shape) == shape and s.stride(1) == 1
+
+
+def fp8_ragged_matmul(a, b, offsets, sa_inv, sb_inv, E, out=None, epi=EPI_STORE, aux=None, out2=None, block=False, sms=0):
+    """m-tiled ragged FP8 GEMM over expert-sorted rows (``dsb_gemm_fp8_ragged``; offsets stay on the device, 128-row
+    segments).  The format of ``a [R, K]`` picks the form:
+
+    * ``float8_e4m3fn`` (forward): ``b`` is the stacked weight viewed ``[E * Nb, K]``; ``out[r] = a[r] @ b_e^T`` with
+      ``b_e = b[e Nb:(e+1) Nb]`` (``Nb = N``), or with ``epi=EPI_SWIGLU`` (``Nb = 2N``, gate rows then up rows)
+      ``out [R, N] = silu(gate) * up`` and ``out2`` (optional ``[R, 2N]``) the gate|up;
+    * ``float8_e5m2`` (dgrad): ``b [N, E * K]`` is the transposed cast of that view; ``out[r] = a[r] @ b_e^T`` with
+      ``b_e = b[:, e K:(e+1) K]``, or with ``epi=EPI_DSWIGLU`` ``aux`` the saved gate|up ``[R, 2N]``, ``out2`` the
+      ``[R, 2N]`` dgate|dup and ``out`` its left half.
+
+    Tensorwise (``block=False``): ``sa_inv`` / ``sb_inv`` one-element fp32 device tensors.  Blockwise: ``sa_inv
+    [ceil(K/128), R]`` (strips of ``a``) and ``sb_inv`` the block scales of ``b`` (``[rows of b / 128, ceil(cols of b /
+    128)]``).  Rows of ``out`` outside ``[offsets[0], offsets[E])`` are not written.  Shapes that do not fit together
+    raise :class:`NativeOpError` before anything is launched."""
+    fmt = {torch.float8_e4m3fn: N.F8E4M3, torch.float8_e5m2: N.F8E5M2}.get(a.dtype)
+    dgrad = fmt == N.F8E5M2
+    R, K = a.shape if a.dim() == 2 else (0, 0)
+    bad = fmt is None or a.dim() != 2 or b.dim() != 2 or b.dtype != torch.float8_e4m3fn or a.stride(1) != 1
+    bad = bad or b.stride(1) != 1 or not torch.is_tensor(offsets) or offsets.dtype != torch.int32
+    bad = bad or offsets.numel() != E + 1 or not offsets.is_cuda or not offsets.is_contiguous() or E < 1
+    Nn = 0
+    if not bad:
+        if dgrad:
+            Nn = b.shape[0]
+            bad = b.shape[1] != E * K or epi not in (EPI_STORE, EPI_DSWIGLU)
+        else:
+            Nb = b.shape[0] // E
+            Nn = Nb // 2 if epi == EPI_SWIGLU else Nb
+            bad = b.shape[0] != E * Nb or b.shape[1] != K or epi not in (EPI_STORE, EPI_SWIGLU)
+            bad = bad or (epi == EPI_SWIGLU and Nb != 2 * Nn)
+        kb = -(-K // 128)
+        bad = bad or not _fp8_scales_ok(sa_inv, (kb, R), block)
+        bad = bad or not _fp8_scales_ok(sb_inv, (-(-b.shape[0] // 128), -(-b.shape[1] // 128)), block)
+    for t, shape in ((out, (R, Nn)), (out2, (R, 2 * Nn)), (aux, (R, 2 * Nn))):
+        if t is not None:
+            bad = bad or tuple(t.shape) != shape or t.dtype != torch.bfloat16 or t.stride(1) != 1
+    if epi == EPI_DSWIGLU:
+        bad = bad or aux is None or out2 is None
+    if bad:
+        raise N.NativeOpError(f"gemm_fp8_ragged: a {tuple(a.shape)} {a.dtype}, b {tuple(b.shape)} {b.dtype}, offsets, "
+                              f"the scales and the outputs do not fit together (E={E}, epi={epi}, block={block})")
+    if out is None:
+        out = out2[:, :Nn] if epi == EPI_DSWIGLU else torch.empty(R, Nn, dtype=torch.bfloat16, device=a.device)
+    ld = lambda t: t.stride(0) if t is not None else 0
+    rc = N.cuda().dsb_gemm_fp8_ragged(N.ptr(a), N.ptr(b), N.ptr(out), N.ptr(offsets), R, E, Nn, K, a.stride(0),
+                                      b.stride(0), out.stride(0), fmt, N.ptr(sa_inv), ld(sa_inv) if block else 0,
+                                      N.ptr(sb_inv), ld(sb_inv) if block else 0, int(epi), N.ptr(aux), ld(aux),
+                                      N.ptr(out2), ld(out2), int(bool(block)), sms, N.stream())
+    N.check(rc, "gemm_fp8_ragged")
+    return out
+
+
+def fp8_ragged_wgrad(a, b, offsets, sa_inv, sb_inv, E, out=None, accumulate=False, block=False, sms=0):
+    """Variable-K FP8 weight gradient (``dsb_gemm_fp8_ragged_wgrad``): ``out[e] (+)= a[:, rows of e] @ b[:, rows of
+    e]^T`` for ``a [M, R]`` (``float8_e5m2``, the transposed gradient) and ``b [N, R]`` (``float8_e4m3fn``, the transposed
+    input), ``out [E, M, N]`` contiguous bf16, in one launch over 128-row segments.  An expert without rows gets zeros
+    (or keeps ``out[e]`` when accumulating).  Blockwise: ``sa_inv [ceil(R/128), M]`` (strips along the rows) and ``sb_inv
+    [ceil(N/128), ceil(R/128)]``; tensorwise: one-element tensors."""
+    M, R = a.shape if a.dim() == 2 else (0, 0)
+    Nn = b.shape[0] if b.dim() == 2 else 0
+    kb = -(-R // 128)
+    bad = (a.dim() != 2 or b.dim() != 2 or a.dtype != torch.float8_e5m2 or b.dtype != torch.float8_e4m3fn
+           or b.shape[1] != R or a.stride(1) != 1 or b.stride(1) != 1 or not torch.is_tensor(offsets)
+           or offsets.dtype != torch.int32 or offsets.numel() != E + 1 or not offsets.is_cuda
+           or not offsets.is_contiguous() or not _fp8_scales_ok(sa_inv, (kb, M), block)
+           or not _fp8_scales_ok(sb_inv, (-(-Nn // 128), kb), block))
+    if out is None and not bad:
+        assert not accumulate
+        out = torch.empty(E, M, Nn, dtype=torch.bfloat16, device=a.device)
+    if bad or not out.is_contiguous() or tuple(out.shape) != (E, M, Nn) or out.dtype != torch.bfloat16:
+        raise N.NativeOpError(f"gemm_fp8_ragged_wgrad: a {tuple(a.shape)} {a.dtype}, b {tuple(b.shape)} {b.dtype}, offsets, "
+                              f"the scales and out do not fit together (E={E}, block={block})")
+    ld = lambda t: t.stride(0) if block else 0
+    rc = N.cuda().dsb_gemm_fp8_ragged_wgrad(N.ptr(a), N.ptr(b), N.ptr(out), N.ptr(offsets), R, E, M, Nn, a.stride(0),
+                                            b.stride(0), N.ptr(sa_inv), ld(sa_inv), N.ptr(sb_inv), ld(sb_inv),
+                                            int(bool(accumulate)), int(bool(block)), sms, N.stream())
+    N.check(rc, "gemm_fp8_ragged_wgrad")
+    return out
+
+
 def supports_2cta(a, b, a_mn, b_mn, out=None) -> bool:
     ok = lambda t: (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 8 == 0
                     and t.data_ptr() % 16 == 0 and t.shape[1] % 8 == 0)

@@ -574,6 +574,118 @@ def ragged_swiglu_mlp(x, offsets, w13, w2, act="silu"):
     return ragged_swiglu_reference(x, offsets, w13, w2, act)
 
 
+def _fp8_cast4(native, block):
+    """``cast(x, fmt, row, col) -> (q, sq, qt, sqt)`` for either recipe: the modes of :func:`fp8.quantize_blockwise`; under
+    the tensorwise recipe a mode only asks for its copy, and both copies share the one scale."""
+    if block:
+        return _fp8_block_cast_fn(native)
+    q = _fp8_cast_fn(native)
+
+    def cast(x, fmt, row="strip", col=None):
+        a, at, s = q(x, fmt, rowwise=row is not None, colwise=col is not None)
+        return a, s, at, s
+
+    return cast
+
+
+class _FP8RaggedSwiGLUFn(torch.autograd.Function):
+    """:class:`_RaggedSwiGLUFn` with FP8 products (tensorwise, or ``block``: blockwise, operand by operand as in
+    :class:`_FP8BlockSwiGLUMLPFn`), on 128-row segments.  The stacked weights are cast as the 2-D matrices
+    ``w13 [E 2I, H]`` and ``w2 [E H, I]`` (one tensorwise scale per stacked weight); forward and dgrad take expert e's
+    row slab of the cast or column slab of its transposed cast, and the variable-K wgrad sums each expert's rows of the
+    transposed activation and gradient copies.  The forward saves only those transposed copies, their scales and the
+    bf16 gate|up; backward re-reads the weights for their transposed casts, finishes every weight read before either
+    gradient is marked ready, and stores or accumulates dW13 / dW2 straight into the stacked parameters' flat ZeRO
+    gradient views.  No host synchronisation on the kernels (``native``); otherwise the torch reference of the recipe.
+    ``act`` and dgate|dup are zero outside the segments: their casts read every row, and a stray value there would
+    enter every expert's tensorwise scale."""
+
+    @staticmethod
+    def forward(ctx, x, offsets, w13, w2, block, native):
+        from deepspeed_b200.ops import fp8
+        E, H, I = w2.shape
+        w13f, w2f = w13.reshape(E * 2 * I, H), w2.reshape(E * H, I)
+        cast = _fp8_cast4(native, block)
+        need_grad = any(ctx.needs_input_grad)
+        need_d13, need_d2 = ctx.needs_input_grad[2], ctx.needs_input_grad[3]
+        x8, sx, x8t, sxt = cast(x, fp8.E4M3, row="strip", col="block" if need_d13 else None)
+        w13_8, s13, _, _ = cast(w13f, fp8.E4M3, row="block")
+        act, gu = fp8.ragged_gemm_swiglu(x8, w13_8, offsets, sx, s13, E, native, save_gate_up=need_grad, block=block)
+        act8, sa, act8t, sat = cast(act, fp8.E4M3, row="strip", col="block" if need_d2 else None)
+        w2_8, s2, _, _ = cast(w2f, fp8.E4M3, row="block")
+        y = fp8.ragged_gemm(act8, w2_8, offsets, sa, s2, E, native, block=block)
+        ctx.w13, ctx.w2, ctx.block, ctx.native = w13, w2, block, native
+        if need_grad:
+            ctx.save_for_backward(offsets, x8t, sxt, gu, act8t, sat)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops import fp8
+        offsets, x8t, sxt, gu, act8t, sat = ctx.saved_tensors
+        w13, w2, block, native = ctx.w13, ctx.w2, ctx.block, ctx.native
+        E, H, I = w2.shape
+        w13f, w2f = w13.reshape(E * 2 * I, H), w2.reshape(E * H, I)
+        cast = _fp8_cast4(native, block)
+        need_dx, need_d13, need_d2 = ctx.needs_input_grad[0], ctx.needs_input_grad[2], ctx.needs_input_grad[3]
+        dy = dy.contiguous()
+        dy8, sdy, dy8t, sdyt = cast(dy, fp8.E5M2, row="strip", col="strip" if need_d2 else None)
+        _, _, w2_8t, s2t = cast(w2f, fp8.E4M3, row=None, col="block")
+        dgu = fp8.ragged_gemm_dswiglu(dy8, w2_8t, offsets, sdy, s2t, gu, E, native, block=block)
+        dx = dgu8t = sgt = None
+        if need_dx or need_d13:
+            dgu8, sg, dgu8t, sgt = cast(dgu, fp8.E5M2, row="strip" if need_dx else None, col="strip" if need_d13 else None)
+            if need_dx:
+                _, _, w13_8t, s13t = cast(w13f, fp8.E4M3, row=None, col="block")
+                dx = fp8.ragged_gemm(dgu8, w13_8t, offsets, sg, s13t, E, native, block=block)
+        # weights are not read past this point
+        grads = {}
+        for i, w, a8t, b8t, s_a, s_b in ((3, w2, dy8t, act8t, sdyt, sat), (2, w13, dgu8t, x8t, sgt, sxt)):
+            if not ctx.needs_input_grad[i]:
+                grads[i] = None
+                continue
+            zo = _zo_of(w)
+            if zo is not None and (not native or zo.grad_view_for(w).dtype == torch.bfloat16):
+                g, accumulate = zo.grad_view_for(w), not zo.grad_is_fresh(w)
+            else:
+                zo, g, accumulate = None, torch.empty_like(w), False
+            fp8.ragged_wgrad(a8t, b8t, offsets, s_a, s_b, E, native, out=g, accumulate=accumulate, block=block)
+            if zo is not None:
+                zo.mark_grad_ready(w)
+                g = None
+            grads[i] = g
+        return dx, None, grads[2], grads[3], None, None
+
+
+def fp8_ragged_swiglu_native(x, offsets, w13, w2) -> bool:
+    """Whether :func:`fp8_ragged_swiglu_mlp` runs the wgmma kernels: CUDA bf16 contiguous rows and stacked weights, int32
+    device offsets, at most 256 experts, ``R % 16 == 0`` (the transposed casts), ``H % 128 == 0`` (the down projection's
+    dgrad takes 128-column expert slabs of its transposed cast) and ``I % 64 == 0`` (the SwiGLU tile, and 128-column
+    slabs for the gate|up dgrad)."""
+    from deepspeed_b200.ops.kernels import gemm_sm100 as K
+    R, H = x.shape
+    I = w2.shape[2]
+    return (K.supports_ragged(x, w13, offsets) and x.is_contiguous() and w2.is_cuda and w2.dtype == torch.bfloat16
+            and w2.is_contiguous() and R > 0 and R % 16 == 0 and H % 128 == 0 and I % 64 == 0)
+
+
+def fp8_ragged_swiglu_mlp(x, offsets, w13, w2, recipe="tensorwise"):
+    """SwiGLU experts over expert-sorted rows ``x [R, H]`` with FP8 products (see :class:`_FP8RaggedSwiGLUFn`): ``w13
+    [E, 2I, H]``, ``w2 [E, H, I]``, ``offsets [E + 1]`` non-decreasing multiples of 128, segments zero-padded and the rows
+    outside them finite (the dropless MoE layer's are zero).  Operands the kernels cannot take (see
+    :func:`fp8_ragged_swiglu_native`) run the same recipe through the torch reference, never a bf16 product.  Rows of
+    the result outside ``[offsets[0], offsets[E])`` are unspecified on the wgmma path."""
+    _check_recipe(recipe)
+    E, I = w13.shape[0], w2.shape[-1]
+    H = x.shape[-1]
+    if (x.dim() != 2 or w13.dim() != 3 or tuple(w13.shape) != (E, 2 * I, H) or tuple(w2.shape) != (E, H, I)
+            or offsets.dim() != 1 or offsets.numel() != E + 1):
+        raise ValueError(f"fp8_ragged_swiglu_mlp: rows {tuple(x.shape)}, w13 {tuple(w13.shape)}, w2 {tuple(w2.shape)} "
+                         f"and offsets {tuple(offsets.shape)} are not [R, H], [E, 2I, H], [E, H, I] and [E + 1]")
+    native = fp8_ragged_swiglu_native(x, offsets, w13, w2)
+    return _FP8RaggedSwiGLUFn.apply(x, offsets, w13, w2, recipe == "blockwise", native)
+
+
 class _ChunkedLinearXent(torch.autograd.Function):
 
     @staticmethod

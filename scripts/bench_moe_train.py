@@ -1,4 +1,5 @@
-"""Dropless MoE training cost at one Mixtral-8x7B MoE layer (H 4096, I 14336, 8 experts, top-2, bf16) and 8192 tokens.
+"""Dropless MoE training cost at one Mixtral-8x7B MoE layer (H 4096, I 14336, 8 experts, top-2, bf16 weights) and 8192
+tokens.
 
 Routing is fixed per run from a seed, either uniform (two distinct experts per token) or skewed (expert 0 is one of each
 token's two choices with probability 0.8, so it takes ~40 % of the assignments).  Every path starts from the same expert
@@ -9,7 +10,9 @@ ids and combine weights and covers dispatch, experts and combine; forward and fo
     path before the ragged kernels existed: bincount, ``.tolist()``, a Python fill loop and ``torch.cat``);
   * capacity_1.25: the capacity-factor path (``[E, C, H]`` with C = 1.25 x the mean load).  It drops tokens under skew, so
     it computes a different result: a cost reference only;
-  * torch_grouped_mm: ``torch._grouped_mm`` on the ragged layout, where this torch build and its shape constraints allow.
+  * torch_grouped_mm: ``torch._grouped_mm`` on the ragged layout, where this torch build and its shape constraints allow;
+  * fp8_tensorwise / fp8_blockwise: the ragged path with FP8 products (``ops.linear.fp8_ragged_swiglu_mlp``) on 128-row
+    segments, the times including every cast the node makes.
 Useful TFLOP/s count the true token-expert assignments only (6 H I FLOPs each forward, 3x that forward + backward).  CUDA
 events after a warm-up.  The card name and power limit are recorded with the numbers."""
 import argparse
@@ -26,7 +29,7 @@ import torch.nn.functional as F
 
 from deepspeed_b200.ops import gemm
 from deepspeed_b200.ops.kernels import moe_ops
-from deepspeed_b200.ops.linear import _RaggedSwiGLUFn, grouped_swiglu_mlp
+from deepspeed_b200.ops.linear import _RaggedSwiGLUFn, fp8_ragged_swiglu_mlp, fp8_ragged_swiglu_native, grouped_swiglu_mlp
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--tokens", type=int, default=8192)
@@ -76,6 +79,19 @@ def ragged(x, ids, w):
     rows, slots = moe_ops.scatter(x, ids, pos, off, k, 0, T * k + E * 63)
     eo = _RaggedSwiGLUFn.apply(rows, off, w13, w2)
     return moe_ops.gather(eo, w, slots, T, k)
+
+
+def fp8_ragged(recipe):
+    def run(x, ids, w):
+        pos, counts, _ = moe_ops.route(ids, E, counts=_counts(ids))
+        seg = (counts + 127) // 128 * 128
+        off = torch.cat([seg.new_zeros(1), torch.cumsum(seg, 0, dtype=torch.int32)])
+        rows, slots = moe_ops.scatter(x, ids, pos, off, k, 0, -(-(T * k + E * 127) // 128) * 128)
+        assert fp8_ragged_swiglu_native(rows, off, w13, w2), "the FP8 arm must run the wgmma kernels"
+        eo = fp8_ragged_swiglu_mlp(rows, off, w13, w2, recipe=recipe)
+        return moe_ops.gather(eo, w, slots, T, k)
+
+    return run
 
 
 def padded_to_max(x, ids, w):
@@ -141,7 +157,8 @@ gemm.set_backend("own")  # the padded and capacity paths on the in-tree kernels,
 useful_fwd = 6.0 * H * I * T * k
 res = {"shape": dict(T=T, H=H, I=I, E=E, k=k, capacity=C, seed=a.seed), "gemm_backend": gemm.get_backend(),
        "useful_fwd_tflop": useful_fwd / 1e12, **gpu_info()}
-paths = {"ragged": ragged, "padded_to_max": padded_to_max, "capacity_1.25": capacity, "torch_grouped_mm": grouped_mm}
+paths = {"ragged": ragged, "padded_to_max": padded_to_max, "capacity_1.25": capacity, "torch_grouped_mm": grouped_mm,
+         "fp8_tensorwise": fp8_ragged("tensorwise"), "fp8_blockwise": fp8_ragged("blockwise")}
 for kind in ("uniform", "skewed"):
     ids, w = routing(kind)
     counts = torch.bincount(ids.reshape(-1).long(), minlength=E).tolist()
@@ -153,6 +170,8 @@ for kind in ("uniform", "skewed"):
             y = fn(x, ids, w)
             if name == "ragged":
                 ref = y.float()
+            elif name.startswith("fp8"):  # a different rounding of the same product: its size relative to the bf16 one
+                r.setdefault("rel_l2_diff_vs_ragged", {})[name] = ((y.float() - ref).norm() / ref.norm()).item()
             elif name != "capacity_1.25":
                 r.setdefault("max_abs_diff_vs_ragged", {})[name] = (y.float() - ref).abs().max().item()
             del y
@@ -175,6 +194,9 @@ for kind in ("uniform", "skewed"):
         torch.cuda.empty_cache()
     if "fwd_ms" in r.get("padded_to_max", {}) and "fwd_ms" in r["ragged"]:
         r["speedup_ragged_vs_padded"] = {p: r["padded_to_max"][p] / r["ragged"][p] for p in ("fwd_ms", "fwd_bwd_ms")}
+    for name in ("fp8_tensorwise", "fp8_blockwise"):
+        if "fwd_ms" in r.get(name, {}) and "fwd_ms" in r["ragged"]:
+            r[f"speedup_{name}_vs_ragged"] = {p: r["ragged"][p] / r[name][p] for p in ("fwd_ms", "fwd_bwd_ms")}
     res[kind] = r
 print(json.dumps(res, indent=1))
 os.makedirs(a.out, exist_ok=True)
