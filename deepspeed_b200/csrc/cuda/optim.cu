@@ -75,6 +75,24 @@ __device__ __forceinline__ void adam_math(float& p, float& m, float& v, float g,
     p = fmaf(-a.lr, upd, p);
 }
 
+// Grid-stride scalar form of adam_flat_kernel for pointers that are not 16-byte aligned.  Kept out of line:
+// inlined, it made ptxas spill 8 bytes in the fp32-master kernels' vector path.
+template <typename PT, typename GT, typename ST, typename OT, bool kHasOut>
+__device__ __noinline__ void adam_flat_scalar(PT* __restrict__ p, const GT* __restrict__ g, ST* __restrict__ m,
+                                              ST* __restrict__ v, OT* __restrict__ out, int64_t n, AdamArgs a,
+                                              float gs)
+{
+    const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        float pf = Elem<PT>::to_f(p[i]), mf = Elem<ST>::to_f(m[i]), vf = Elem<ST>::to_f(v[i]);
+        adam_math(pf, mf, vf, Elem<GT>::to_f(g[i]), a, gs);
+        p[i] = Elem<PT>::from_f(pf);
+        m[i] = Elem<ST>::from_f(mf);
+        v[i] = Elem<ST>::from_f(vf);
+        if (kHasOut) out[i] = Elem<OT>::from_f(pf);
+    }
+}
+
 // PT: master/param dtype, GT: grad dtype, ST: state dtype, OT: low-precision copy dtype.
 template <typename PT, typename GT, typename ST, typename OT, bool kHasOut>
 __global__ void __launch_bounds__(256) adam_flat_kernel(PT* __restrict__ p, const GT* __restrict__ g,
@@ -85,8 +103,17 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(PT* __restrict__ p, cons
 {
     if (d_skip != nullptr && *d_skip != 0) return;
     const float gs = a.grad_scale * (d_gscale ? *d_gscale : 1.f);
-    const int64_t n8 = n >> 3;
     const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+    // The 16-byte vector path needs every pointer 16-byte aligned (ZeRO arenas are; arbitrary views of
+    // them need not be).  The test is uniform across the grid, so a misaligned call runs the scalar loop.
+    const bool aligned = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) |
+                           reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(v) |
+                           reinterpret_cast<uintptr_t>(out)) & 15) == 0;
+    if (!aligned) {
+        adam_flat_scalar<PT, GT, ST, OT, kHasOut>(p, g, m, v, out, n, a, gs);
+        return;
+    }
+    const int64_t n8 = n >> 3;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8; i += stride) {
         const int64_t o = i << 3;
         float pf[8], gf[8], mf[8], vf[8];

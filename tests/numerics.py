@@ -596,3 +596,220 @@ def attention_data(family, T, hq, hkv, d, gen):
     else:
         raise ValueError(family)
     return tuple(x.bfloat16() for x in (q, k, v, do))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# optimizers and gradient utilities (csrc/cuda/optim.cu, csrc/cpu/cpu_optim.cpp)
+# ---------------------------------------------------------------------------------------------------------------------
+# The kernels are built without fast-math: IEEE division and square root, and fp32 subnormals are kept (no flush to
+# zero).  nvcc and g++ may contract ``a * b + c`` into one fma, and the host tier writes some of the kernels' explicit
+# fmas as a product and a sum; every bound below counts the product's rounding too, so it holds either way.  Each rounding errs by at most ``U`` times its result plus ``TINY`` (half the
+# smallest fp32 subnormal), which covers results in the subnormal range.
+TINY = 2.0**-150
+
+
+def f32(x):
+    """``x`` rounded to fp32 (the value a ``float`` kernel argument carries), as a Python float."""
+    return float(torch.tensor(float(x), dtype=torch.float32))
+
+
+def adam_hyper(lr, beta1, beta2, eps, weight_decay, step, bias_correction=True, grad_scale=1.0, d_gscale=None,
+               adamw=True):
+    """The Adam hyperparameters as ``adam_math`` sees them: every argument rounded to fp32, the bias corrections
+    ``1 - beta**step`` formed in float64 by the wrapper and rounded to fp32, ``1 - beta`` in fp32 (exact by Sterbenz for
+    ``beta`` in [0.5, 1]) and the gradient scale ``fp32(grad_scale) * d_gscale`` rounded once."""
+    b1, b2 = f32(beta1), f32(beta2)
+    gs = f32(grad_scale)
+    if d_gscale is not None:
+        gs = f32(gs * f32(d_gscale))
+    return dict(lr=f32(lr), b1=b1, b2=b2, b1m=f32(1.0 - b1), b2m=f32(1.0 - b2), eps=f32(eps), wd=f32(weight_decay),
+                bc1=f32(1.0 - beta1**step) if bias_correction else 1.0,
+                bc2=f32(1.0 - beta2**step) if bias_correction else 1.0, gs=gs, adamw=bool(adamw))
+
+
+def _sqrt_err(x, e):
+    """Bound on ``|sqrt(x') - sqrt(x)|`` for ``|x' - x| <= e``, ``x >= 0``."""
+    lo = (x - e).clamp_min(0.0)
+    return torch.minimum(e.sqrt(), e / (x.sqrt() + lo.sqrt()).clamp_min(1e-300))
+
+
+def adam_reference(p, g, m, v, h, dtypes=None, update=False):
+    """Float64 one Adam/AdamW step of ``adam_math`` from the state the kernel starts from (any dtypes), with the
+    hyperparameters ``h`` of :func:`adam_hyper`.  Returns ``(p, m, v)`` and their bounds ``(bp, bm, bv)`` for outputs
+    stored in ``dtypes = (param dtype, state dtype)`` (fp32 when None).
+
+    The operation sequence and the error each step adds before the final rounding (absolute, ``e_x`` for value ``x``):
+
+    1. ``g1 = g * gs``: one rounding.
+    2. L2 (``adamw`` off): ``g2 = fma(wd, p, g1)``: one rounding.
+    3. ``m' = fma(b1, m, fp32(b1m * g2))``: the product rounds, plus ``b1m e_g2``; the fma's rounding is the stored
+       value's.
+    4. ``v' = fma(b2, v, fp32(fp32(b2m * g2) * g2))``: two product roundings, plus ``b2m (2 |g2| e_g2 + e_g2^2)``.
+    5. ``mh = m' / bc1`` and ``vh = v' / bc2`` round once each (twice each on the host tier's SIMD paths, which
+       multiply by the rounded reciprocal; the bound counts two); ``sqrt`` once more, with the input error carried by
+       ``min(sqrt(e), e / (sqrt(x) + sqrt(x - e)))``; ``+ eps`` once.
+    6. ``u = mh / d``: ``(e_mh + |u| e_d) / (d - e_d)`` and one rounding.
+    7. AdamW: ``u2 = fma(wd, p, u)``: one rounding.
+    8. ``p' = fma(-lr, u2, p)``: ``lr e_u2``, then the stored rounding.
+
+    Each stored value gets one :func:`ulp` of its dtype at ``|ref| + err`` on top (the header's convention).
+    ``update=True`` also returns the update ``u2`` and its error (LAMB's trust ratio is formed from it)."""
+    pd, sd = dtypes if dtypes is not None else (torch.float32, torch.float32)
+    p, g, m, v = p.double(), g.double(), m.double(), v.double()
+    R = lambda x: U * x.abs() + TINY  # noqa: E731  one rounding of a result of magnitude |x|
+    g1 = g * h["gs"]
+    e = R(g1)
+    if not h["adamw"]:
+        g1 = g1 + h["wd"] * p
+        e = e + R(h["wd"] * p) + R(g1.abs() + e)
+    t1 = h["b1m"] * g1
+    m1 = h["b1"] * m + t1
+    em = h["b1m"] * e + R(t1.abs() + h["b1m"] * e) + R(h["b1"] * m)
+    t2 = h["b2m"] * g1 * g1
+    v1 = h["b2"] * v + t2
+    ev = h["b2m"] * (2 * g1.abs() * e + e * e) + 2.0001 * R(t2.abs() + h["b2m"] * (2 * g1.abs() * e + e * e)) \
+        + R(h["b2"] * v)
+    bm = ulp(m1.abs() + em, sd) + em
+    bv = ulp(v1.abs() + ev, sd) + ev
+    # the moments the update uses are the kernel's fp32 values before the state's rounding: only em, ev
+    mh = m1 / h["bc1"]
+    emh = em / h["bc1"] + 2.0001 * R(mh.abs() + em / h["bc1"])
+    vh = v1 / h["bc2"]
+    evh = ev / h["bc2"] + 2.0001 * R(vh + ev / h["bc2"])
+    s = vh.sqrt()
+    es = _sqrt_err(vh, evh) + R(s + _sqrt_err(vh, evh))
+    d = s + h["eps"]
+    ed = es + R(d + es)
+    u = mh / d
+    eu = (emh + u.abs() * ed) / (d - ed).clamp_min(1e-300)
+    eu = eu + R(u.abs() + eu)
+    if h["adamw"]:
+        u = u + h["wd"] * p
+        eu = eu + R(h["wd"] * p) + R(u.abs() + eu)
+    p1 = p - h["lr"] * u
+    ep = h["lr"] * eu + R(h["lr"] * u)
+    bp = ulp(p1.abs() + ep, pd) + ep
+    if update:
+        return p1, m1, v1, bp, bm, bv, u, eu
+    return p1, m1, v1, bp, bm, bv
+
+
+def lion_reference(p, g, m, lr, beta1, beta2, weight_decay, gs, dtypes=None, fused=True):
+    """Float64 Lion step of ``lion_flat_kernel`` / ``dsb_cpu_lion`` from the kernel's state, ``gs`` the fp32 gradient
+    scale the kernel uses.  Returns ``(p, m, sign, bp, bm)``.
+
+    The sign is exact: ``g1 = fp32(g * gs)`` and ``t = fp32(fp32(1 - b1) * g1)`` are fp32 products (emulated bit for bit
+    in fp32), ``b1 m`` is exact in float64 (24 x 24 bits) and the float64 sum ``b1 m + t`` has the sign of the exact sum.
+    The fma rounds that sum once to fp32, which keeps its sign unless it underflows to zero (magnitude at most
+    ``2**-150``).  ``p' = p (1 - lr wd) - lr sign``: ``1 - lr wd`` rounds up to twice (``U (lr wd + |decay|)``), the
+    product once; the subtraction's rounding is the stored one.  ``m' = fma(b2, m, fp32((1 - b2) g1))``: one product
+    rounding, then the stored rounding.
+
+    ``fused=False`` is the host tier, which may round ``b1 m`` and ``b2 m`` before the sum: there the sign is only known
+    where ``|c|`` exceeds that rounding, elsewhere the bound on p widens by ``2 lr``, and m's bound gets one more ``U``."""
+    pd, sd = dtypes if dtypes is not None else (torch.float32, torch.float32)
+    b1, b2, lr, wd = f32(beta1), f32(beta2), f32(lr), f32(weight_decay)
+    g1 = g.float() * torch.tensor(f32(gs), dtype=torch.float32, device=g.device)
+    t = g1 * torch.tensor(f32(1.0 - b1), dtype=torch.float32, device=g.device)
+    c = b1 * m.double() + t.double()
+    sign = torch.where(c.abs() > TINY, torch.sign(c), 0.0)
+    p64 = p.double()
+    decay = 1.0 - lr * wd
+    p1 = p64 * decay - lr * sign
+    e_dec = U * (lr * wd + abs(decay))
+    ep = p64.abs() * e_dec + U * (p64 * decay).abs() + 2 * TINY
+    t2 = f32(1.0 - b2) * g1.double()
+    m1 = b2 * m.double() + t2
+    em = U * t2.abs() + TINY
+    if not fused:
+        ep = ep + torch.where(c.abs() <= U * (b1 * m.double()).abs() + TINY, 2 * lr, 0.0)
+        em = em + U * (b2 * m.double()).abs() + TINY
+    return p1, m1, sign, ulp(p1.abs() + ep, pd) + ep, ulp(m1.abs() + em, sd) + em
+
+
+def adagrad_reference(p, g, hsum, lr, eps, weight_decay, gs, pd=torch.float32):
+    """Float64 Adagrad step with ``torch.optim.Adagrad``'s formula (``lr_decay = 0``, no initial accumulator):
+    ``g' = g gs + wd p``, ``h' = h + g'^2``, ``p' = p - lr g' / (sqrt(h') + eps)``.  Returns ``(p, h, bp, bh)``.
+
+    The kernel rounds ``g gs`` and the fma with ``wd p`` once each, ``h + g'^2`` up to twice (the stored rounding is the
+    second), ``lr g'``, the sqrt, ``+ eps`` and the division once each; the subtraction is the stored rounding."""
+    lr, eps, wd = f32(lr), f32(eps), f32(weight_decay)
+    p, g, hsum = p.double(), g.double(), hsum.double()
+    g1 = g * f32(gs)
+    e = U * g1.abs() + TINY
+    g1 = g1 + wd * p
+    e = e + U * (wd * p).abs() + U * (g1.abs() + e) + 2 * TINY
+    h1 = hsum + g1 * g1
+    eh = 2 * g1.abs() * e + e * e + U * g1 * g1 + TINY
+    s = h1.sqrt()
+    es = _sqrt_err(h1, eh + U * h1) + U * s + TINY
+    d = s + eps
+    ed = es + U * (d + es) + TINY
+    q = lr * g1 / d
+    eq = (lr * e + q.abs() * ed) / (d - ed).clamp_min(1e-300) + 2.0001 * U * q.abs() + 2 * TINY
+    p1 = p - q
+    return p1, h1, ulp(p1.abs() + eq, pd) + eq, ulp(h1 + eh, torch.float32) + eh
+
+
+def sgd_reference(p, g, buf, lr, momentum, dampening, weight_decay, nesterov, first, gs, pd=torch.float32):
+    """Float64 SGD step with ``torch.optim.SGD``'s semantics: ``d = g gs + wd p``; with momentum the buffer is ``d`` on
+    the first step and ``momentum buf + (1 - dampening) d`` after, and the direction is ``d + momentum buf`` (nesterov)
+    or ``buf``; ``p' = p - lr d``.  Returns ``(p, buf, bp, bbuf)``; every operation of the kernel rounds at most once
+    (``2U`` for ``(1 - dampening) d`` and the fma)."""
+    lr, mom, damp, wd = f32(lr), f32(momentum), f32(dampening), f32(weight_decay)
+    p, g, buf = p.double(), g.double(), buf.double()
+    d = g * f32(gs)
+    e = U * d.abs() + TINY
+    d = d + wd * p
+    e = e + U * (wd * p).abs() + U * (d.abs() + e) + 2 * TINY
+    b1, eb = buf, torch.zeros_like(buf)
+    if mom != 0.0:
+        if first:
+            b1, eb = d, e
+        else:
+            b1 = mom * buf + f32(1.0 - damp) * d
+            eb = f32(1.0 - damp) * e + U * f32(1.0 - damp) * (d.abs() + e) + U * (mom * buf).abs() + 2 * TINY
+        if nesterov:
+            d, e = d + mom * b1, e + mom * eb + U * (mom * b1).abs() + U * (d + mom * b1).abs() + 2 * TINY
+        else:
+            d, e = b1, eb
+    p1 = p - lr * d
+    ep = lr * e + U * lr * d.abs() + TINY
+    return p1, b1, ulp(p1.abs() + ep, pd) + ep, ulp(b1.abs() + eb, torch.float32) + eb
+
+
+def sumsq_depth(n, dtype, grid_cap=132 * 4, threads=512):
+    """Longest chain of fp32 additions behind ``dsb_sumsq``'s result for ``n`` elements: a thread's grid-stride fma chain
+    (vector path, then the scalar tail, or all scalar when misaligned), the block tree (5 warp levels twice), the
+    partials' per-thread sum and tree, and the accumulate."""
+    per = 4 if dtype == torch.float32 else 8
+    grid = max(1, min(-(-(n // 8 + 1) // threads), grid_cap))
+    chain = per * -(-(n // per) // (grid * threads)) + -(-n // (grid * threads))
+    return chain + 10 + -(-grid // 1024) + 10 + 1
+
+
+def sumsq_bound(total, n, dtype):
+    """Bound on ``|dsb_sumsq(x) - sum(x^2)|`` for a sum of squares ``total`` of ``n`` elements: every term and partial
+    sum is non-negative, so ``L`` roundings along the longest chain err by at most ``_rel(L)`` of the total."""
+    return _rel(sumsq_depth(n, dtype)) * total + 2 * TINY
+
+
+def clip_coeff_reference(sumsq, inv_loss_scale, max_norm):
+    """Float64 ``(gscale, norm)`` of ``clip_coeff_kernel`` for a finite fp32 ``sumsq``:
+    ``norm = sqrt(ss) inv_ls`` and ``gscale = inv_ls min(1, max_norm / (norm + 1e-6))`` (with the fp32 arguments), and
+    their relative bounds: sqrt and product round once each (2U), ``norm + 1e-6f``, the division and the last product
+    once each, plus ``1e-6f``'s distance from 1e-6."""
+    inv, mx = f32(inv_loss_scale), f32(max_norm)
+    norm = math.sqrt(sumsq) * inv
+    c = inv
+    if mx > 0:
+        c = inv * min(1.0, mx / (norm + 1e-6))
+    rel_norm = 2.0001 * U
+    eps_err = abs(f32(1e-6) - 1e-6) / (norm + 1e-6)
+    rel_c = (rel_norm + 3.0001 * U + eps_err) if mx > 0 else 0.0
+    return c, norm, rel_c, rel_norm
+
+
+def round_bf16_truncate(x):
+    """fp32 -> bf16 by dropping the low 16 bits (round toward zero): the wrong cast a bound check must reject."""
+    return (x.float().contiguous().view(torch.int32) & -65536).view(torch.float32).bfloat16()
