@@ -491,10 +491,13 @@ gated_act_fwd_kernel(const T* __restrict__ gate_up, T* __restrict__ out, int64_t
     }
 }
 
-template <typename T>
+// kAct: also write act_out = act(gate) * up, computed exactly as gated_act_fwd_kernel does, so a caller that did not
+// keep the forward's output gets it back bit for bit from the same read of gate_up.  A template flag rather than a null
+// check, so the plain backward compiles to the same code (and register count) as without the extra output.
+template <typename T, bool kAct>
 __global__ void __launch_bounds__(256)
 gated_act_bwd_kernel(const T* __restrict__ dout, const T* __restrict__ gate_up, T* __restrict__ dgate_up,
-                     int64_t tokens, int inter, int act)
+                     T* __restrict__ act_out, int64_t tokens, int inter, int act)
 {
     constexpr int kPer = Elem<T>::kPerVec;
     const int vpr = inter / kPer;
@@ -510,12 +513,15 @@ gated_act_bwd_kernel(const T* __restrict__ dout, const T* __restrict__ gate_up, 
         Elem<T>::unpack(ld_stream(dout + t * inter + v * kPer), d);
 #pragma unroll
         for (int e = 0; e < kPer; ++e) {
+            const float a = act_fwd(g[e], act);
             dg[e] = d[e] * u[e] * act_bwd(g[e], act);
-            du[e] = d[e] * act_fwd(g[e], act);
+            du[e] = d[e] * a;
+            if constexpr (kAct) g[e] = a * u[e];
         }
         T* orow = dgate_up + t * 2 * inter;
         st_plain(orow + v * kPer, Elem<T>::pack(dg));
         st_plain(orow + inter + v * kPer, Elem<T>::pack(du));
+        if constexpr (kAct) st_plain(act_out + t * inter + v * kPer, Elem<T>::pack(g));
     }
 }
 
@@ -890,16 +896,21 @@ DSB_EXPORT int dsb_gated_act_fwd(const void* gate_up, void* out, int64_t tokens,
     return 0;
 }
 
-DSB_EXPORT int dsb_gated_act_bwd(const void* dout, const void* gate_up, void* dgate_up, int64_t tokens, int inter,
-                                 int act, int dtype, cudaStream_t stream)
+DSB_EXPORT int dsb_gated_act_bwd(const void* dout, const void* gate_up, void* dgate_up, void* act_out, int64_t tokens,
+                                 int inter, int act, int dtype, cudaStream_t stream)
 {
     if (tokens <= 0) return 0;
     const int per = (dtype == kF32) ? 4 : 8;
     if (inter % per != 0) return -2;
     const int grid = flat_grid(tokens * (inter / per), 256, 16);
     DISPATCH_T(dtype, T, {
-        gated_act_bwd_kernel<T>
-            <<<grid, 256, 0, stream>>>((const T*)dout, (const T*)gate_up, (T*)dgate_up, tokens, inter, act);
+        if (act_out != nullptr) {
+            gated_act_bwd_kernel<T, true><<<grid, 256, 0, stream>>>((const T*)dout, (const T*)gate_up, (T*)dgate_up,
+                                                                    (T*)act_out, tokens, inter, act);
+        } else {
+            gated_act_bwd_kernel<T, false><<<grid, 256, 0, stream>>>((const T*)dout, (const T*)gate_up, (T*)dgate_up,
+                                                                     nullptr, tokens, inter, act);
+        }
     })
     DSB_CHECK_LAUNCH();
     return 0;

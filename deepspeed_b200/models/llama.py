@@ -15,6 +15,7 @@ H100 is PyTorch ops.  H100-first choices here:
   ``sequence/fpdt_layer.py:1137``);
 * attention core through ``ops.attention`` (cuDNN/flash SDPA library path or the native sm_90a kernel).
 """
+import functools
 import math
 from dataclasses import dataclass, field
 from typing import Optional
@@ -200,19 +201,28 @@ class LlamaMLP(nn.Module):
         self.act = cfg.hidden_act
         self.fp8, self.fp8_recipe = cfg.fp8, cfg.fp8_recipe
 
-    def forward(self, x):
-        if self.act == "silu" and self.gate_up_proj.bias is None and self.down_proj.bias is None:
-            if self.fp8:
-                from deepspeed_b200.ops.linear import fp8_swiglu_mlp
-                return fp8_swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight, recipe=self.fp8_recipe)
+    @property
+    def trimmed_recompute(self) -> bool:
+        """Whether this block runs the bf16 fused SwiGLU node, whose replay for activation checkpointing stops at gate|up
+        (``forward(x, recompute=True)``).  The FP8 node and the unfused form replay their whole forward."""
+        return self.act == "silu" and self.gate_up_proj.bias is None and self.down_proj.bias is None and not self.fp8
+
+    def forward(self, x, recompute=False):
+        if self.trimmed_recompute:
             from deepspeed_b200.ops.linear import swiglu_mlp
-            return swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight)
+            return swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight, recompute=recompute)
+        assert not recompute, "only the bf16 fused SwiGLU block has a trimmed recompute"
+        if self.act == "silu" and self.gate_up_proj.bias is None and self.down_proj.bias is None:
+            from deepspeed_b200.ops.linear import fp8_swiglu_mlp
+            return fp8_swiglu_mlp(x, self.gate_up_proj.weight, self.down_proj.weight, recipe=self.fp8_recipe)
         return self.down_proj(T.gated_act(self.gate_up_proj(x), self.act))
 
 
 class LlamaDecoderLayer(nn.Module):
     """Takes and returns ``(delta, residual)``: ``residual`` is the running stream *before* adding
-    ``delta`` (the previous branch output), so every add is fused into the following RMSNorm."""
+    ``delta`` (the previous branch output), so every add is fused into the following RMSNorm.  ``recompute=True`` is the
+    backward replay of an activation-checkpointed layer: the returned ``delta`` (the MLP output, which backward never
+    reads) holds no data, see :meth:`LlamaMLP.forward`."""
 
     def __init__(self, cfg: LlamaConfig, layer_idx: int):
         super().__init__()
@@ -222,7 +232,7 @@ class LlamaDecoderLayer(nn.Module):
         self.post_attention_layernorm = RMSNorm(cfg.hidden_size, cfg.rms_norm_eps)
         self.mlp = LlamaMLP(cfg)
 
-    def forward(self, delta, residual, rope, positions=None, cu_seqlens=None, max_seqlen=None):
+    def forward(self, delta, residual, rope, positions=None, cu_seqlens=None, max_seqlen=None, recompute=False):
         if residual is None:
             residual = delta
             h = self.input_layernorm(delta)
@@ -230,7 +240,7 @@ class LlamaDecoderLayer(nn.Module):
             h, residual = self.input_layernorm(delta, residual)
         attn = self.self_attn(h, rope, positions, cu_seqlens, max_seqlen)
         h, residual = self.post_attention_layernorm(attn, residual)
-        return self.mlp(h), residual
+        return self.mlp(h, recompute), residual
 
 
 class LlamaModel(nn.Module):
@@ -263,7 +273,10 @@ class LlamaModel(nn.Module):
         for i, layer in enumerate(self.layers):
             if self.training and i < cfg.checkpoint_layers and torch.is_grad_enabled():
                 from deepspeed_b200.runtime.activation_checkpointing import checkpointing as ckpt
-                delta, residual = ckpt.checkpoint(layer, delta, residual, rope, positions, cu_seqlens, max_seqlen)
+                # the replay in backward stops where that backward stops reading: no down GEMM (see LlamaMLP.forward)
+                replay = functools.partial(layer, recompute=True) if layer.mlp.trimmed_recompute else None
+                delta, residual = ckpt.checkpoint(layer, delta, residual, rope, positions, cu_seqlens, max_seqlen,
+                                                  replay=replay)
             else:
                 delta, residual = layer(delta, residual, rope, positions, cu_seqlens, max_seqlen)
         h, _ = self.norm(delta, residual)

@@ -231,14 +231,29 @@ def matmul_tn(a, b, out=None, accumulate=False):
     return torch.mm(a.t(), b, out=out)
 
 
+def _swiglu_key(x, w_gu):
+    """Table key of the fused gate|up + SwiGLU problem, or None when the own kernel cannot take these operands."""
+    T, H = x.shape
+    I = w_gu.shape[0] // 2
+    return f"nt_swiglu:{T}x{I}x{H}" if _eligible(T, I, H, x, w_gu) and I % 128 == 0 else None
+
+
+def gate_up_swiglu_in_tree(x, w_gu) -> bool:
+    """Whether :func:`gate_up_swiglu` of these operands ran the own fused kernel (valid after that call).  Its ``act`` then
+    comes from the fp32 accumulators and differs from ``silu(gate) * up`` recomputed from the bf16 ``gate_up``; on the
+    library path the two are bit-identical (:func:`down_dx_dswiglu` ``act_out``)."""
+    key = _swiglu_key(x, w_gu)
+    return key is not None and _used.get(key) == "own"
+
+
 def gate_up_swiglu(x, w_gu, save_gate_up=True):
     """``x [T, H]``, ``w_gu [2I, H]`` (gate rows then up rows) -> ``(act [T, I], gate_up [T, 2I] | None)`` where
     ``act = silu(x Wg^T) * (x Wu^T)``.  Own path: ONE kernel (activation in the GEMM epilogue, gate|up saved for backward
-    from the same accumulators); library path: cuBLAS GEMM + the element-wise gated-activation kernel."""
+    from the same accumulators); library path: :func:`matmul_nt` + the element-wise gated-activation kernel."""
     T, H = x.shape
     I = w_gu.shape[0] // 2
-    if _eligible(T, I, H, x, w_gu) and I % 128 == 0:
-        key = f"nt_swiglu:{T}x{I}x{H}"
+    key = _swiglu_key(x, w_gu)
+    if key is not None:
 
         def own(scratch=True):
             act = _scratch(T, I, x, 1) if scratch else torch.empty(T, I, dtype=x.dtype, device=x.device)
@@ -261,9 +276,12 @@ def gate_up_swiglu(x, w_gu, save_gate_up=True):
     return T_.gated_act_fwd_raw(gu), (gu if save_gate_up else None)
 
 
-def down_dx_dswiglu(dy, w_down, gate_up):
+def down_dx_dswiglu(dy, w_down, gate_up, act_out=None):
     """``dy [T, H]``, ``w_down [H, I]``, saved ``gate_up [T, 2I]`` -> ``dgate_up [T, 2I]``: the down-projection's input
-    gradient ``dy @ w_down`` never reaches memory -- the SwiGLU backward is applied to the accumulators in the epilogue."""
+    gradient ``dy @ w_down`` never reaches memory -- the SwiGLU backward is applied to the accumulators in the epilogue.
+    ``act_out [T, I]`` (optional) receives ``silu(gate) * up`` of ``gate_up``, bit-identical to the library path of
+    :func:`gate_up_swiglu`: written by the library path's dSwiGLU pass, or on the own path by a gated-activation pass
+    after the fused kernel."""
     T, H = dy.shape
     I = w_down.shape[1]
     if _eligible(T, I, H, dy, w_down, gate_up):
@@ -281,9 +299,13 @@ def down_dx_dswiglu(dy, w_down, gate_up):
 
         if _choose(key, own, lib) == "own":
             _report(T * I * H)
-            return own(scratch=False)
+            dgu = own(scratch=False)
+            if act_out is not None:
+                from deepspeed_b200.ops.kernels import transformer_ops as T_
+                T_.gated_act_fwd_raw(gate_up, "silu", out=act_out)
+            return dgu
     from deepspeed_b200.ops.kernels import transformer_ops as T_
-    return T_.gated_act_bwd(matmul_nn(dy, w_down), gate_up, "silu")
+    return T_.gated_act_bwd(matmul_nn(dy, w_down), gate_up, "silu", act_out=act_out)
 
 
 _scratch_bufs = {}

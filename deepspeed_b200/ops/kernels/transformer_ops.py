@@ -229,22 +229,27 @@ def rope_qk_inplace(qkv, n_q, n_kv, head_dim, table, positions=None, seq_len=Non
 # ---------------------------------------------------------------------------------------------------
 # gated activation (SwiGLU & friends)
 # ---------------------------------------------------------------------------------------------------
-def gated_act_fwd_raw(gu, act=ACT_SILU):
-    """``act(gate) * up`` of a contiguous packed ``[T, 2I]`` tensor, no autograd."""
+def gated_act_fwd_raw(gu, act=ACT_SILU, out=None):
+    """``act(gate) * up`` of a contiguous packed ``[T, 2I]`` tensor (into the contiguous ``out [T, I]`` when given), no
+    autograd."""
     if isinstance(act, str):
         act = act_code(act)
     inter = gu.shape[-1] // 2
     if gu.is_cuda:
-        out = torch.empty(gu.shape[0], inter, dtype=gu.dtype, device=gu.device)
+        if out is None:
+            out = torch.empty(gu.shape[0], inter, dtype=gu.dtype, device=gu.device)
         rc = N.cuda().dsb_gated_act_fwd(_p(gu), _p(out), N.c_i64(gu.shape[0]), inter, act, N.dt(gu), N.stream())
         N.check(rc, "gated_act_fwd")
         return out
     g, u = gu[:, :inter].float(), gu[:, inter:].float()
-    return (_act_torch(g, act) * u).to(gu.dtype)
+    y = (_act_torch(g, act) * u).to(gu.dtype)
+    return y if out is None else out.copy_(y)
 
 
-def gated_act_bwd(dout, gu, act=ACT_SILU):
-    """Gradient of :func:`gated_act` w.r.t. the packed ``[T, 2I]`` input: ``[d * up * act'(gate) | d * act(gate)]``."""
+def gated_act_bwd(dout, gu, act=ACT_SILU, act_out=None):
+    """Gradient of :func:`gated_act` w.r.t. the packed ``[T, 2I]`` input: ``[d * up * act'(gate) | d * act(gate)]``.
+    ``act_out`` (contiguous ``[T, I]``, optional) also receives the forward output ``act(gate) * up`` from the same pass,
+    bit-identical to :func:`gated_act_fwd_raw` of ``gu``: a caller need not keep the forward's output for backward."""
     if isinstance(act, str):
         act = act_code(act)
     inter = gu.shape[-1] // 2
@@ -253,7 +258,10 @@ def gated_act_bwd(dout, gu, act=ACT_SILU):
         d2 = d2.contiguous()
     if gu.is_cuda:
         dgu = torch.empty_like(gu)
-        rc = N.cuda().dsb_gated_act_bwd(_p(d2), _p(gu), _p(dgu), N.c_i64(gu.shape[0]), inter, act, N.dt(gu), N.stream())
+        if act_out is not None:
+            assert act_out.is_contiguous() and act_out.shape == (gu.shape[0], inter) and act_out.dtype == gu.dtype
+        rc = N.cuda().dsb_gated_act_bwd(_p(d2), _p(gu), _p(dgu), _p(act_out), N.c_i64(gu.shape[0]), inter, act, N.dt(gu),
+                                        N.stream())
         N.check(rc, "gated_act_bwd")
         return dgu
     g = gu[:, :inter].float().requires_grad_(True)
@@ -261,7 +269,10 @@ def gated_act_bwd(dout, gu, act=ACT_SILU):
     with torch.enable_grad():
         a = _act_torch(g, act)
         (da, ) = torch.autograd.grad(a, g, torch.ones_like(a))
-    return torch.cat([d2.float() * u * da, d2.float() * a.detach()], dim=-1).to(gu.dtype)
+    a = a.detach()
+    if act_out is not None:
+        act_out.copy_((a * u).to(gu.dtype))
+    return torch.cat([d2.float() * u * da, d2.float() * a], dim=-1).to(gu.dtype)
 
 
 class _GatedActFn(torch.autograd.Function):

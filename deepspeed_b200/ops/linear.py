@@ -106,20 +106,37 @@ class _SwiGLUMLPFn(torch.autograd.Function):
     backward  ``dY W_down`` GEMM with the SwiGLU *backward* applied in its epilogue (the ``[tokens, I]`` intermediate
               gradient never reaches memory) -> dW_down, dX and dW_gate_up GEMMs, weight gradients written (or
               accumulated, GAS > 1) directly into the ZeRO flat gradient views.
+    Only ``x`` and gate|up are saved: the library path's dSwiGLU pass writes ``act`` for dW_down again from the same bf16
+    gate|up, bit for bit.  When the gate|up GEMM ran the own fused kernel, whose ``act`` comes from the fp32 accumulators,
+    ``act`` is saved too.
+
+    ``recompute``: the forward is a replay for backward (activation checkpointing) that stops at what backward reads --
+    gate|up, and ``act`` where it is saved -- and returns a placeholder of the output's shape with no data: backward never
+    reads the output, so the down GEMM (and, on the library path, the SwiGLU pass) is not run.
     Reference role: the three ``nn.Linear`` + ``ACT2FN`` of an HF MLP block / ``csrc/transformer/gelu_kernels.cu``
     (``fused_bias_gelu``) -- there the activation is a separate pass over the intermediate tensor."""
 
     @staticmethod
-    def forward(ctx, x, w_gu, w_down):
+    def forward(ctx, x, w_gu, w_down, recompute):
         from deepspeed_b200.ops import gemm
         x2 = x.reshape(-1, x.shape[-1])
-        need_grad = any(ctx.needs_input_grad)  # (grad mode is off inside Function.forward)
-        act, gu = gemm.gate_up_swiglu(x2, w_gu, save_gate_up=need_grad)
-        y = gemm.matmul_nt(act, w_down)
+        out_shape = (*x.shape[:-1], w_down.shape[0])
+        if recompute:
+            if gemm.gate_up_swiglu_in_tree(x2, w_gu):
+                act, gu = gemm.gate_up_swiglu(x2, w_gu)
+            else:
+                act, gu = None, gemm.matmul_nt(x2, w_gu)
+            y = x2.new_empty(1).expand(out_shape)
+        else:
+            need_grad = any(ctx.needs_input_grad)  # (grad mode is off inside Function.forward)
+            act, gu = gemm.gate_up_swiglu(x2, w_gu, save_gate_up=need_grad)
+            y = gemm.matmul_nt(act, w_down).view(out_shape)
+            if not gemm.gate_up_swiglu_in_tree(x2, w_gu):
+                act = None
         ctx.w_gu, ctx.w_down = w_gu, w_down
         ctx.save_for_backward(x2, gu, act)
         ctx.x_shape = x.shape
-        return y.view(*x.shape[:-1], w_down.shape[0])
+        return y
 
     @staticmethod
     def backward(ctx, dy):
@@ -129,16 +146,20 @@ class _SwiGLUMLPFn(torch.autograd.Function):
         dy2 = dy.reshape(-1, dy.shape[-1])
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
-        dgu = gemm.down_dx_dswiglu(dy2, w_down, gu)
+        act_out = None
+        if act is None and ctx.needs_input_grad[2]:
+            act = act_out = torch.empty(gu.shape[0], gu.shape[1] // 2, dtype=gu.dtype, device=gu.device)
+        dgu = gemm.down_dx_dswiglu(dy2, w_down, gu, act_out=act_out)
         dw_down = _write_weight_grad(w_down, dy2, act) if ctx.needs_input_grad[2] else None
         dx = gemm.matmul_nn(dgu, w_gu).view(ctx.x_shape) if ctx.needs_input_grad[0] else None
         dw_gu = _write_weight_grad(w_gu, dgu, x2) if ctx.needs_input_grad[1] else None
-        return dx, dw_gu, dw_down
+        return dx, dw_gu, dw_down, None
 
 
-def swiglu_mlp(x, w_gate_up, w_down):
-    """Fused SwiGLU MLP block (no biases): see :class:`_SwiGLUMLPFn`."""
-    return _SwiGLUMLPFn.apply(x, w_gate_up, w_down)
+def swiglu_mlp(x, w_gate_up, w_down, recompute=False):
+    """Fused SwiGLU MLP block (no biases): see :class:`_SwiGLUMLPFn`.  ``recompute=True`` is the trimmed replay of an
+    activation-checkpointed block: its output holds no data, only its gradient is used."""
+    return _SwiGLUMLPFn.apply(x, w_gate_up, w_down, recompute)
 
 
 def _fp8_native(x2, *ws, inter=None) -> bool:

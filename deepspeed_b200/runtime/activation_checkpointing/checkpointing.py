@@ -305,6 +305,21 @@ class CheckpointFunction(torch.autograd.Function):
         return tuple(ret)
 
 
+class ReplayCheckpointFunction(CheckpointFunction):
+    """:class:`CheckpointFunction` whose backward re-runs ``replay_function`` instead of ``run_function``: a replay that
+    returns outputs of the same shapes whose backward is the same, but computes only what that backward reads."""
+
+    @staticmethod
+    def forward(ctx, run_function, replay_function, all_outputs, *args):
+        outputs = CheckpointFunction.forward(ctx, run_function, all_outputs, *args)
+        ctx.run_function = replay_function  # what backward re-runs
+        return outputs
+
+    @staticmethod
+    def backward(ctx, *grads):
+        return (None, ) + CheckpointFunction.backward(ctx, *grads)
+
+
 def _timers():
     global timers
     if timers is None:
@@ -312,10 +327,14 @@ def _timers():
     return timers
 
 
-def checkpoint(function, *args):
-    """Checkpoint a model or part of the model (reference :980).  Returns what ``function`` returns."""
+def checkpoint(function, *args, replay=None):
+    """Checkpoint a model or part of the model (reference :980).  Returns what ``function`` returns.  ``replay``
+    (optional) is what backward re-runs instead of ``function``: see :class:`ReplayCheckpointFunction`."""
     all_outputs = []
-    out = CheckpointFunction.apply(function, all_outputs, *args)
+    if replay is None:
+        out = CheckpointFunction.apply(function, all_outputs, *args)
+    else:
+        out = ReplayCheckpointFunction.apply(function, replay, all_outputs, *args)
     if len(all_outputs) == 1:
         return out if torch.is_tensor(out) else out[0]
     # re-attach non-tensor outputs in their original positions
