@@ -432,6 +432,175 @@ rope_kernel(T* __restrict__ x, const float* __restrict__ cos_t, const float* __r
 }
 
 // ------------------------------------------------------------------------------------------------
+// QK-norm + rotary embedding (Qwen3 attention), in place on the Q|K heads of a packed
+// [tokens, (hq + 2 hkv) * head_dim] buffer with an arbitrary token stride:
+//   q_h <- rope(w_q * q_h * rsqrt(mean(q_h^2) + eps)) for every query head, the same with w_k for every key head.
+// One 16-byte vector per lane: a head spans L = head_dim / kPer lanes (8, 16 or 32), a warp holds 32 / L heads, and both
+// the sum of squares and the rotate-half partner (element i <-> i + head_dim / 2, lane ^ L/2) move through shuffles.
+// All arithmetic is fp32 and each output is rounded once.  rot_dim == head_dim.
+// ------------------------------------------------------------------------------------------------
+template <int L>
+__device__ __forceinline__ float head_sum(float v)
+{
+#pragma unroll
+    for (int o = L / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+template <int kPer>
+__device__ __forceinline__ void ld_table(const float* p, float (&f)[kPer])
+{
+#pragma unroll
+    for (int e = 0; e < kPer; e += 4) {
+        const float4 q = *reinterpret_cast<const float4*>(p + e);
+        f[e] = q.x; f[e + 1] = q.y; f[e + 2] = q.z; f[e + 3] = q.w;
+    }
+}
+
+// Forward.  Also copies the pre-norm Q|K into `raw` [tokens, (hq + hkv) * head_dim] (contiguous) unless it is null: the
+// backward reads it and derives rstd from it again.
+template <typename T, int L>
+__global__ void __launch_bounds__(256)
+qk_norm_rope_kernel(T* __restrict__ qkv, T* __restrict__ raw, const float* __restrict__ cos_t,
+                    const float* __restrict__ sin_t, const int* __restrict__ positions, const T* __restrict__ w_q,
+                    const T* __restrict__ w_k, int64_t tokens, int hq, int hkv, int64_t token_stride, int seq_len,
+                    float eps)
+{
+    constexpr int kPer = Elem<T>::kPerVec;
+    constexpr int kDim = L * kPer, kHeadsPerWarp = 32 / L;
+    const int lane = threadIdx.x & 31, v = lane % L;
+    const bool upper = v >= L / 2;
+    const int hv = (upper ? v - L / 2 : v) * kPer;  // offset into a [rot_dim / 2] table row
+    const float rsign = upper ? 1.f : -1.f;
+    const int heads = hq + hkv;
+    const int64_t items = tokens * heads;
+    const int64_t groups = ceil_div(items, kHeadsPerWarp);
+    const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x / 32);
+    for (int64_t g = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32; g < groups; g += nwarps) {
+        const int64_t item = g * kHeadsPerWarp + lane / L;
+        const bool ok = item < items;  // a whole head group is in or out: the shuffles below stay within it
+        const int64_t t = ok ? item / heads : 0;
+        const int h = ok ? static_cast<int>(item - t * heads) : 0;
+        T* px = qkv + t * token_stride + static_cast<int64_t>(h) * kDim + v * kPer;
+        Vec16 xv{};
+        float x[kPer], w[kPer] = {}, c[kPer] = {}, s[kPer] = {};
+        if (ok) {
+            xv = ld_plain(px);
+            Elem<T>::unpack(ld_plain((h < hq ? w_q : w_k) + v * kPer), w);
+            const int pos = positions ? positions[t] : static_cast<int>(t % seq_len);
+            ld_table<kPer>(cos_t + static_cast<int64_t>(pos) * (kDim / 2) + hv, c);
+            ld_table<kPer>(sin_t + static_cast<int64_t>(pos) * (kDim / 2) + hv, s);
+        }
+        Elem<T>::unpack(xv, x);
+        float ss = 0.f;
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) ss = fmaf(x[e], x[e], ss);
+        const float rstd = rsqrtf(head_sum<L>(ss) / kDim + eps);
+        float n[kPer], o[kPer];
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) n[e] = x[e] * rstd * w[e];
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) {
+            const float p = __shfl_xor_sync(0xffffffffu, n[e], L / 2);
+            o[e] = fmaf(n[e], c[e], rsign * p * s[e]);
+        }
+        if (ok) {
+            if (raw) st_plain(raw + item * kDim + v * kPer, xv);
+            st_plain(px, Elem<T>::pack(o));
+        }
+    }
+}
+
+// Backward, in place on the dQ|dK heads of the packed gradient: r = rope^-1(dy), g = w * r,
+// dx = rstd * (g - xhat * mean(g * xhat)).  dw_q / dw_k partial sums of r * xhat over the CTA's heads of each kind land in
+// dw_part [gridDim.x, 2 * head_dim] (q | k) in a fixed order; colsum_kernel finishes them, so dw is bit-reproducible.
+template <typename T, int L>
+__global__ void __launch_bounds__(256)
+qk_norm_rope_bwd_kernel(T* __restrict__ dqkv, const T* __restrict__ raw, const float* __restrict__ cos_t,
+                        const float* __restrict__ sin_t, const int* __restrict__ positions, const T* __restrict__ w_q,
+                        const T* __restrict__ w_k, float* __restrict__ dw_part, int64_t tokens, int hq, int hkv,
+                        int64_t token_stride, int seq_len, float eps)
+{
+    constexpr int kPer = Elem<T>::kPerVec;
+    constexpr int kDim = L * kPer, kHeadsPerWarp = 32 / L, kWarps = 8;
+    __shared__ float red[kWarps][2 * kDim];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, v = lane % L;
+    const bool upper = v >= L / 2;
+    const int hv = (upper ? v - L / 2 : v) * kPer;
+    const float rsign = upper ? -1.f : 1.f;  // the transpose rotation
+    const int heads = hq + hkv;
+    const int64_t items = tokens * heads;
+    const int64_t groups = ceil_div(items, kHeadsPerWarp);
+    const int64_t nwarps = static_cast<int64_t>(gridDim.x) * kWarps;
+    float acc_q[kPer], acc_k[kPer];
+#pragma unroll
+    for (int e = 0; e < kPer; ++e) acc_q[e] = acc_k[e] = 0.f;
+    for (int64_t g = static_cast<int64_t>(blockIdx.x) * kWarps + warp; g < groups; g += nwarps) {
+        const int64_t item = g * kHeadsPerWarp + lane / L;
+        const bool ok = item < items;
+        const int64_t t = ok ? item / heads : 0;
+        const int h = ok ? static_cast<int>(item - t * heads) : 0;
+        T* pd = dqkv + t * token_stride + static_cast<int64_t>(h) * kDim + v * kPer;
+        Vec16 dv{}, xv{};
+        float dy[kPer], x[kPer], w[kPer] = {}, c[kPer] = {}, s[kPer] = {};
+        if (ok) {
+            dv = ld_plain(pd);
+            xv = ld_stream(raw + item * kDim + v * kPer);
+            Elem<T>::unpack(ld_plain((h < hq ? w_q : w_k) + v * kPer), w);
+            const int pos = positions ? positions[t] : static_cast<int>(t % seq_len);
+            ld_table<kPer>(cos_t + static_cast<int64_t>(pos) * (kDim / 2) + hv, c);
+            ld_table<kPer>(sin_t + static_cast<int64_t>(pos) * (kDim / 2) + hv, s);
+        }
+        Elem<T>::unpack(dv, dy);
+        Elem<T>::unpack(xv, x);
+        float r[kPer], ss = 0.f;
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) {
+            const float p = __shfl_xor_sync(0xffffffffu, dy[e], L / 2);
+            r[e] = fmaf(dy[e], c[e], rsign * p * s[e]);
+            ss = fmaf(x[e], x[e], ss);
+        }
+        const float rstd = rsqrtf(head_sum<L>(ss) / kDim + eps);
+        float s2 = 0.f;
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) s2 = fmaf(w[e] * r[e], x[e] * rstd, s2);
+        const float m2 = head_sum<L>(s2) / kDim;
+        float o[kPer];
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) {
+            const float xhat = x[e] * rstd;
+            o[e] = rstd * (w[e] * r[e] - xhat * m2);
+            if (ok && h < hq) acc_q[e] = fmaf(r[e], xhat, acc_q[e]);
+            if (ok && h >= hq) acc_k[e] = fmaf(r[e], xhat, acc_k[e]);
+        }
+        if (ok) st_plain(pd, Elem<T>::pack(o));
+    }
+    // the warp's head groups, then the CTA's warps, each in a fixed order
+#pragma unroll
+    for (int e = 0; e < kPer; ++e) {
+#pragma unroll
+        for (int o = L; o < 32; o <<= 1) {
+            acc_q[e] += __shfl_xor_sync(0xffffffffu, acc_q[e], o);
+            acc_k[e] += __shfl_xor_sync(0xffffffffu, acc_k[e], o);
+        }
+    }
+    if (lane < L) {
+#pragma unroll
+        for (int e = 0; e < kPer; ++e) {
+            red[warp][v * kPer + e] = acc_q[e];
+            red[warp][kDim + v * kPer + e] = acc_k[e];
+        }
+    }
+    __syncthreads();
+    for (int col = threadIdx.x; col < 2 * kDim; col += blockDim.x) {
+        float sum = 0.f;
+#pragma unroll
+        for (int k = 0; k < kWarps; ++k) sum += red[k][col];
+        dw_part[static_cast<int64_t>(blockIdx.x) * 2 * kDim + col] = sum;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Gated activation: out[t, i] = act(gate[t, i]) * up[t, i], gate_up = [T, 2I] (gate | up).
 // act: 0 SiLU (SwiGLU), 1 GELU-tanh (GEGLU), 2 ReLU (ReGLU), 3 GELU-erf.
 // ------------------------------------------------------------------------------------------------
@@ -881,6 +1050,72 @@ DSB_EXPORT int dsb_rope(void* x, const float* cos_t, const float* sin_t, const i
     DSB_CHECK_LAUNCH();
     return 0;
 }
+
+// The QK-norm kernels take head dim 64 or 128; L = head_dim / (elements per 16-byte vector) lanes per head.
+#define DSB_DISPATCH_QK_HEAD_DIM(head_dim, T, L, ...) \
+    if ((head_dim) == 64) {                           \
+        constexpr int L = 64 / Elem<T>::kPerVec;      \
+        __VA_ARGS__                                   \
+    } else {                                          \
+        constexpr int L = 128 / Elem<T>::kPerVec;     \
+        __VA_ARGS__                                   \
+    }
+
+// In place on the Q|K heads of `qkv` [tokens, (hq + 2 hkv) * head_dim] (row stride token_stride elements, 16-byte aligned),
+// cos/sin [max_pos, head_dim / 2] fp32, positions int32 [tokens] or null (pos = token % seq_len), w_q / w_k [head_dim] in
+// the buffer's dtype.  raw: [tokens, (hq + hkv) * head_dim] contiguous, receives the pre-norm Q|K; null when no backward
+// follows.
+DSB_EXPORT int dsb_qk_norm_rope(void* qkv, void* raw, const float* cos_t, const float* sin_t, const int* positions,
+                                const void* w_q, const void* w_k, int64_t tokens, int hq, int hkv, int head_dim,
+                                int64_t token_stride, int seq_len, float eps, int dtype, cudaStream_t stream)
+{
+    const int per = (dtype == kF32) ? 4 : 8;
+    if ((head_dim != 64 && head_dim != 128) || token_stride % per != 0) return -2;
+    if (tokens <= 0 || hq + hkv <= 0) return 0;
+    const int64_t warps = ceil_div(tokens * (hq + hkv), 32 / (head_dim / per));
+    const int grid = flat_grid(warps * 32, 256, 8);
+    DISPATCH_T(dtype, T, {
+        DSB_DISPATCH_QK_HEAD_DIM(head_dim, T, L, {
+            qk_norm_rope_kernel<T, L><<<grid, 256, 0, stream>>>((T*)qkv, (T*)raw, cos_t, sin_t, positions, (const T*)w_q,
+                                                                (const T*)w_k, tokens, hq, hkv, token_stride, seq_len, eps);
+        })
+    })
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+// Rows of the dw_part scratch dsb_qk_norm_rope_bwd needs ([rows, 2 * head_dim] fp32): its grid.
+DSB_EXPORT int dsb_qk_norm_rope_bwd_grid(int64_t tokens, int heads, int head_dim, int dtype)
+{
+    const int per = (dtype == kF32) ? 4 : 8;
+    return flat_grid(ceil_div(tokens * heads, 32 / (head_dim / per)) * 32, 256, 4);
+}
+
+// Backward of dsb_qk_norm_rope, in place on the dQ|dK heads of `dqkv` (same layout as qkv; dV untouched), from the `raw`
+// the forward wrote.  dw: [2 * head_dim] in `wdtype` (dw_q | dw_k), overwritten.
+DSB_EXPORT int dsb_qk_norm_rope_bwd(void* dqkv, const void* raw, const float* cos_t, const float* sin_t,
+                                    const int* positions, const void* w_q, const void* w_k, float* dw_part, void* dw,
+                                    int64_t tokens, int hq, int hkv, int head_dim, int64_t token_stride, int seq_len,
+                                    float eps, int dtype, int wdtype, cudaStream_t stream)
+{
+    const int per = (dtype == kF32) ? 4 : 8;
+    if ((head_dim != 64 && head_dim != 128) || token_stride % per != 0) return -2;
+    // no tokens: the kernel writes zero partials, so dw is zero
+    const int grid = dsb_qk_norm_rope_bwd_grid(tokens, hq + hkv, head_dim, dtype);
+    DISPATCH_T(dtype, T, {
+        DSB_DISPATCH_QK_HEAD_DIM(head_dim, T, L, {
+            qk_norm_rope_bwd_kernel<T, L><<<grid, 256, 0, stream>>>((T*)dqkv, (const T*)raw, cos_t, sin_t, positions,
+                                                                    (const T*)w_q, (const T*)w_k, dw_part, tokens, hq,
+                                                                    hkv, token_stride, seq_len, eps);
+        })
+    })
+    DISPATCH_T(wdtype, TO, {
+        colsum_kernel<TO><<<(2 * head_dim + 31) / 32, 256, 0, stream>>>(dw_part, (TO*)dw, grid, 2 * head_dim, 0);
+    })
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+#undef DSB_DISPATCH_QK_HEAD_DIM
 
 DSB_EXPORT int dsb_gated_act_fwd(const void* gate_up, void* out, int64_t tokens, int inter, int act, int dtype,
                                  cudaStream_t stream)

@@ -1,4 +1,4 @@
-"""Llama-family decoder (Llama-2/3, Mistral, Phi-3, Qwen2) built on the deepspeed_b200 kernels.
+"""Llama-family decoder (Llama-2/3, Mistral, Phi-3, Qwen2, Qwen3) built on the deepspeed_b200 kernels.
 
 This is the flagship training model of the framework (``BASELINE.json``: Llama-3-8B ZeRO-3 bf16).
 The reference ships no training model; its users bring HF ``LlamaForCausalLM`` whose hot path on
@@ -6,7 +6,8 @@ H100 is PyTorch ops.  H100-first choices here:
 
 * packed ``qkv`` and ``gate_up`` projections -> 4 large GEMMs per layer instead of 7;
 * residual-add fused into RMSNorm (one pass over the residual stream per norm);
-* RoPE applied in place on the packed QKV buffer with precomputed fp32 tables (one launch for Q+K);
+* RoPE applied in place on the packed QKV buffer with precomputed fp32 tables (one launch for Q+K), fused with Qwen3's
+  per-head QK-norm when ``qk_norm`` is on;
 * SwiGLU as one kernel on the packed gate_up output;
 * weight gradients are written **directly into the ZeRO flat gradient buffer** by the linear's
   backward (``out=`` GEMM), bypassing AccumulateGrad and the copy into the reduce bucket;
@@ -56,6 +57,10 @@ class LlamaConfig:
     # scaling granularity when ``fp8`` is on: "tensorwise" (one scale per tensor) or "blockwise" (1 x 128 strips of
     # activations and gradients, 128 x 128 blocks of weights: an outlier costs precision in its own block only)
     fp8_recipe: str = "tensorwise"
+    # QK-norm (Qwen3): an RMSNorm with its own learned [head_dim] weight on every query head (``self_attn.q_norm``) and
+    # every key head (``self_attn.k_norm``), after the projection and before RoPE, in fp32 (see
+    # ``transformer_ops.qk_norm_rope_inplace``)
+    qk_norm: bool = False
     # training knobs
     checkpoint_layers: int = 0  # number of decoder layers (from the front) run with activation recompute
     loss_chunk_tokens: int = 2048
@@ -78,6 +83,8 @@ class LlamaConfig:
     def num_parameters(self, include_embeddings=True):
         h, i, L = self.hidden_size, self.intermediate_size, self.num_hidden_layers
         per = h * (self.q_size + 2 * self.kv_size) + self.q_size * h + 3 * h * i + 2 * h
+        if self.qk_norm:
+            per += 2 * self.head_dim
         n = L * per + h
         if include_embeddings:
             n += self.vocab_size * h * (1 if self.tie_word_embeddings else 2)
@@ -120,6 +127,13 @@ PRESETS = {
     "mistral-7b": dict(vocab_size=32000, hidden_size=4096, intermediate_size=14336, num_hidden_layers=32,
                        num_attention_heads=32, num_key_value_heads=8, rope_theta=10000.0, max_position_embeddings=32768,
                        sliding_window=4096),
+    # Qwen3 dense (QK-norm, head dim 128 with hidden / heads != 128 for the 1.7B); the 1.7B ties its LM head
+    "qwen3-8b": dict(vocab_size=151936, hidden_size=4096, intermediate_size=12288, num_hidden_layers=36,
+                     num_attention_heads=32, num_key_value_heads=8, head_dim=128, rope_theta=1e6, rms_norm_eps=1e-6,
+                     max_position_embeddings=40960, qk_norm=True),
+    "qwen3-1.7b": dict(vocab_size=151936, hidden_size=2048, intermediate_size=6144, num_hidden_layers=28,
+                       num_attention_heads=16, num_key_value_heads=8, head_dim=128, tie_word_embeddings=True,
+                       rope_theta=1e6, rms_norm_eps=1e-6, max_position_embeddings=40960, qk_norm=True),
     "tiny": dict(vocab_size=512, hidden_size=128, intermediate_size=256, num_hidden_layers=2, num_attention_heads=4,
                  num_key_value_heads=2, max_position_embeddings=256, rope_theta=10000.0),
 }
@@ -181,14 +195,19 @@ class LlamaAttention(nn.Module):
         self.qkv_proj = FlatLinear(cfg.hidden_size, cfg.q_size + 2 * cfg.kv_size, bias=cfg.attention_bias, fp8=cfg.fp8,
                                    fp8_recipe=cfg.fp8_recipe)
         self.o_proj = FlatLinear(cfg.q_size, cfg.hidden_size, bias=False, fp8=cfg.fp8, fp8_recipe=cfg.fp8_recipe)
+        if cfg.qk_norm:
+            # weights only: the attention node applies them, fused with RoPE; the module names match HF's keys
+            self.q_norm = RMSNorm(cfg.head_dim, cfg.rms_norm_eps)
+            self.k_norm = RMSNorm(cfg.head_dim, cfg.rms_norm_eps)
 
     def forward(self, x, rope, positions=None, cu_seqlens=None, max_seqlen=None):
         cfg = self.cfg
         B, S, _ = x.shape
         qkv = self.qkv_proj(x)  # [B, S, (hq + 2 hkv) d]
+        qk_norm = (self.q_norm.weight, self.k_norm.weight, cfg.rms_norm_eps) if cfg.qk_norm else None
         out = causal_attention(qkv.view(B * S, -1), B, S, cfg.num_attention_heads, cfg.num_key_value_heads,
                                cfg.head_dim, rope, positions, backend=cfg.attention_backend, cu_seqlens=cu_seqlens,
-                               max_seqlen=max_seqlen, sliding_window=cfg.sliding_window)
+                               max_seqlen=max_seqlen, sliding_window=cfg.sliding_window, qk_norm=qk_norm)
         return self.o_proj(out.view(B, S, cfg.q_size))
 
 

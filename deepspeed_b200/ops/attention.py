@@ -18,6 +18,10 @@ counting its own position (HF's ``sliding_window``, flash-attn's ``window_size=(
 with ``cu_seqlens``.  ``auto`` / ``native`` run the in-tree windowed kernel (head dim 64 or 128), which skips the tiles
 outside the band; every other case runs SDPA with an explicit boolean band mask per sequence or document.  A window that covers the whole sequence
 (or the longest document) is dropped, so such a call is exactly the unwindowed one.
+QK-norm (``qk_norm=(w_q, w_k, eps)``, Qwen3): every query head is RMS-normalised with its own ``[d]`` weight ``w_q`` and
+every key head with ``w_k`` before RoPE, in the same in-place pass (``transformer.cu:qk_norm_rope_kernel``, see
+``transformer_ops.qk_norm_rope_inplace``); the autograd nodes take the two weights as inputs and return their gradients.
+``qk_norm=None`` runs exactly the calls it ran without the argument.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
 """
@@ -27,7 +31,7 @@ import os
 import torch
 import torch.nn.functional as F
 
-from deepspeed_b200.ops.kernels.transformer_ops import rope_qk_inplace
+from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_bwd_inplace, qk_norm_rope_inplace, rope_qk_inplace
 
 _ENV = os.environ.get("DSB200_ATTN", "").lower()
 
@@ -91,9 +95,12 @@ def _sdpa(q, k, v, backend, causal=True, scale=None, window=None):
 class _PackedCausalAttention(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, backend, window):
+    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, backend, window, w_q, w_k, qk_eps):
         T = B * S
-        if rope is not None:
+        raw = None
+        if w_q is not None:
+            raw = qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
+        elif rope is not None:
             rope_qk_inplace(qkv, hq, hkv, d, rope, positions, S, backward=False)
         x = qkv.view(B, S, hq + 2 * hkv, d)
         q = x[:, :, :hq].transpose(1, 2)
@@ -103,13 +110,15 @@ class _PackedCausalAttention(torch.autograd.Function):
             qd, kd, vd = (t.detach().requires_grad_(True) for t in (q, k, v))
             out = _sdpa(qd, kd, vd, backend, window=window)
         ctx.graph = (qd, kd, vd, out)
-        ctx.meta = (B, S, hq, hkv, d, rope, positions)
+        ctx.meta = (B, S, hq, hkv, d, rope, positions, qk_eps)
         ctx.qkv_shape = qkv.shape
+        if w_q is not None:
+            ctx.save_for_backward(raw, w_q, w_k)
         return out.detach().transpose(1, 2).reshape(T, hq * d)
 
     @staticmethod
     def backward(ctx, dout):
-        B, S, hq, hkv, d, rope, positions = ctx.meta
+        B, S, hq, hkv, d, rope, positions, qk_eps = ctx.meta
         qd, kd, vd, out = ctx.graph
         ctx.graph = None
         do = dout.view(B, S, hq, d).transpose(1, 2)
@@ -119,9 +128,27 @@ class _PackedCausalAttention(torch.autograd.Function):
         y[:, :, :hq].copy_(dq.transpose(1, 2))
         y[:, :, hq:hq + hkv].copy_(dk.transpose(1, 2))
         y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
-        if rope is not None:
+        dw_q = dw_k = None
+        if qk_eps is not None:
+            raw, w_q, w_k = ctx.saved_tensors
+            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
+        elif rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, S, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None, None, None, dw_q, dw_k, None
+
+
+def _qk_norm_grad(qk_norm):
+    """Whether a QK-norm weight needs a gradient (then the autograd node runs even for a ``qkv`` that needs none)."""
+    return qk_norm is not None and (qk_norm[0].requires_grad or qk_norm[1].requires_grad)
+
+
+def _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, seq_len, qk_norm):
+    """The no-grad branches' in-place QK-norm + RoPE (or RoPE alone): nothing is kept for a backward."""
+    if qk_norm is not None:
+        w_q, w_k, eps = qk_norm
+        qk_norm_rope_inplace(qkv2d, hq, hkv, d, rope, w_q, w_k, eps, positions, seq_len, need_raw=False)
+    elif rope is not None:
+        rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, seq_len, backward=False)
 
 
 _TABLE = None
@@ -196,9 +223,11 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
     in-place RoPE with per-token positions, packed ``dqkv`` in the backward, un-rotated in place."""
 
     @staticmethod
-    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal, window):
+    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal, window, w_q, w_k, qk_eps):
         T = qkv.shape[0]
-        if rope is not None:
+        if w_q is not None:
+            ctx.save_for_backward(qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T), w_q, w_k)
+        elif rope is not None:
             rope_qk_inplace(qkv, hq, hkv, d, rope, positions, T, backward=False)
         out = qkv.new_empty(T, hq * d)
         graphs = []
@@ -210,13 +239,13 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
             out[s:e] = o.detach().transpose(1, 2).reshape(e - s, hq * d)
             graphs.append((s, e, qd, kd, vd, o))
         ctx.graphs = graphs
-        ctx.meta = (hq, hkv, d, rope, positions)
+        ctx.meta = (hq, hkv, d, rope, positions, qk_eps)
         ctx.qkv_shape = qkv.shape
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        hq, hkv, d, rope, positions = ctx.meta
+        hq, hkv, d, rope, positions, qk_eps = ctx.meta
         graphs, ctx.graphs = ctx.graphs, None
         T = ctx.qkv_shape[0]
         dqkv = torch.zeros(ctx.qkv_shape, dtype=dout.dtype, device=dout.device)
@@ -227,16 +256,20 @@ class _PackedVarlenCausalAttention(torch.autograd.Function):
             y[:, :, :hq].copy_(dq.transpose(1, 2))
             y[:, :, hq:hq + hkv].copy_(dk.transpose(1, 2))
             y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
-        if rope is not None:
+        dw_q = dw_k = None
+        if qk_eps is not None:
+            raw, w_q, w_k = ctx.saved_tensors
+            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T)
+        elif rope is not None:
             rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, T, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, None
+        return dqkv, None, None, None, None, None, None, None, None, None, dw_q, dw_k, None
 
 
 def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=None, backend="auto", causal=True,
-                          sliding_window=None):
-    """Per-document SDPA over packed documents (any device / dtype / head dim); ``positions`` as in
-    :func:`causal_attention` (defaults to :func:`document_positions`).  ``sliding_window`` needs ``causal``; a document
-    longer than the window runs with a boolean band mask."""
+                          sliding_window=None, qk_norm=None):
+    """Per-document SDPA over packed documents (any device / dtype / head dim); ``positions`` and ``qk_norm`` as in
+    :func:`causal_attention` (``positions`` defaults to :func:`document_positions`).  ``sliding_window`` needs ``causal``;
+    a document longer than the window runs with a boolean band mask."""
     window = check_sliding_window(sliding_window)
     if window is not None and not causal:
         raise ValueError("a sliding window is defined only for causal attention")
@@ -246,10 +279,11 @@ def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=No
     if positions is not None:
         positions = positions.reshape(-1).to(device=qkv2d.device, dtype=torch.int32)
     spans = _doc_spans(cu_seqlens, T)
-    if torch.is_grad_enabled() and qkv2d.requires_grad:
-        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal, window)
-    if rope is not None:
-        rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
+    w_q, w_k, qk_eps = qk_norm or (None, None, None)
+    if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
+        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal, window, w_q,
+                                                  w_k, qk_eps)
+    _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, T, qk_norm)
     out = qkv2d.new_empty(T, hq * d)
     for s, e in spans:
         o = _sdpa(*_split_doc(qkv2d, s, e, hq, hkv, d), backend, causal=causal, window=window)
@@ -257,7 +291,7 @@ def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=No
     return out
 
 
-def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window):
+def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window, qk_norm):
     max_seqlen = check_cu_seqlens(cu_seqlens, T, max_seqlen)
     if window is not None and window >= max_seqlen:
         window = None  # no document is longer than the window: exactly the unwindowed call
@@ -268,29 +302,32 @@ def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_
             if rope is not None:
                 positions = (document_positions(cu, T) if positions is None else positions.reshape(-1).to(
                     device=qkv2d.device, dtype=torch.int32))
-            if torch.is_grad_enabled() and qkv2d.requires_grad:
-                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions, window)
-            if rope is not None:
-                rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, T, backward=False)
+            if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
+                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions, window,
+                                                               qk_norm)
+            _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, T, qk_norm)
             q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
             return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False,
                                               window=window, head_dim=d)[0]
     if backend == "native":
         raise RuntimeError("native varlen attention kernel requested but unsupported for this input (needs a CUDA bf16 "
                            "tensor, head dim 64 or 128, 16-byte aligned rows)")
-    return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend, sliding_window=window)
+    return varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope, positions, backend, sliding_window=window,
+                                 qk_norm=qk_norm)
 
 
 def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend="auto", cu_seqlens=None, max_seqlen=None,
-                     sliding_window=None):
+                     sliding_window=None, qk_norm=None):
     """``qkv2d [B*S, (hq + 2 hkv) * d]`` -> ``[B*S, hq*d]``.  With ``cu_seqlens`` (int32 ``[n_docs + 1]`` offsets into the
     ``B*S`` rows, see :func:`check_cu_seqlens`) attention is masked to each document and ``positions`` defaults to
     :func:`document_positions`; a device ``cu_seqlens`` needs ``max_seqlen``.  ``sliding_window``: see the module
-    docstring; a value that is not an int >= 1 raises ``ValueError``."""
+    docstring; a value that is not an int >= 1 raises ``ValueError``.  ``qk_norm``: ``None`` or ``(w_q, w_k, eps)``, the
+    per-head RMSNorm of Q and K before RoPE (module docstring)."""
     backend = _ENV or backend or "auto"
     window = check_sliding_window(sliding_window)
     if cu_seqlens is not None:
-        return _varlen_causal_attention(qkv2d, B * S, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window)
+        return _varlen_causal_attention(qkv2d, B * S, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window,
+                                        qk_norm)
     if window is not None and window >= S:
         window = None  # every row sees its whole causal prefix: exactly the unwindowed call
     # `auto` takes the in-tree kernel for a window whenever it can: it skips the tiles outside the band, the fallback masks
@@ -298,21 +335,20 @@ def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend
                                (window is not None or _native_wins(B, S, hq, hkv, d))):
         from deepspeed_b200.ops.kernels import attention_sm100
         if attention_sm100.supports(qkv2d, hq, hkv, d, S):
-            if torch.is_grad_enabled() and qkv2d.requires_grad:
-                return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions, window)
-            if rope is not None:
-                rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)
+            if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
+                return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions, window, qk_norm)
+            _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, S, qk_norm)
             q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
             return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False, window=window,
                                        head_dim=d)[0]
         if backend == "native":
             raise RuntimeError("native attention kernel requested but unsupported for this shape (needs bf16, head dim 64 "
                                "or 128, sequence length a multiple of 128)")
-    if not (torch.is_grad_enabled() and qkv2d.requires_grad):
-        if rope is not None:
-            rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, S, backward=False)
+    if not (torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm))):
+        _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, S, qk_norm)
         x = qkv2d.view(B, S, hq + 2 * hkv, d)
         out = _sdpa(x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2),
                     x[:, :, hq + hkv:].transpose(1, 2), backend, window=window)
         return out.transpose(1, 2).reshape(B * S, hq * d)
-    return _PackedCausalAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, backend, window)
+    w_q, w_k, qk_eps = qk_norm or (None, None, None)
+    return _PackedCausalAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, backend, window, w_q, w_k, qk_eps)

@@ -227,6 +227,115 @@ def rope_qk_inplace(qkv, n_q, n_kv, head_dim, table, positions=None, seq_len=Non
 
 
 # ---------------------------------------------------------------------------------------------------
+# QK-norm + rotary embedding (Qwen3 attention)
+# ---------------------------------------------------------------------------------------------------
+def _qk_norm_native(qkv, head_dim, table):
+    """Whether ``transformer.cu``'s fused QK-norm kernels take this buffer: CUDA bf16 / fp16 / fp32, head dim 64 or 128,
+    a full rotary table, unit column stride and 16-byte aligned rows."""
+    per = 4 if qkv.dtype == torch.float32 else 8
+    return (qkv.is_cuda and qkv.dtype in (torch.bfloat16, torch.float16, torch.float32) and head_dim in (64, 128)
+            and table is not None and table.rot_dim == head_dim and qkv.stride(-1) == 1 and qkv.stride(0) % per == 0
+            and qkv.data_ptr() % 16 == 0)
+
+
+def _qk_heads(qkv, n_q, n_kv, head_dim):
+    return qkv.as_strided((qkv.shape[0], n_q + n_kv, head_dim), (qkv.stride(0), head_dim, 1))
+
+
+def _qk_weights(w_q, w_k, n_q, n_kv):
+    """fp32 ``[n_q + n_kv, head_dim]``: ``w_q`` for every query head, then ``w_k`` for every key head."""
+    return torch.cat([w_q.float().expand(n_q, -1), w_k.float().expand(n_kv, -1)])
+
+
+def _rotate_f32(x, table, positions, seq_len, sign):
+    """Rotate-half RoPE (``sign`` -1: the transpose) of fp32 ``x [tokens, heads, head_dim]``, out of place; the dims past
+    ``table.rot_dim`` pass through."""
+    if table is None:
+        return x
+    half = table.rot_dim // 2
+    pos = positions.long() if positions is not None else torch.arange(x.shape[0], device=x.device) % seq_len
+    c = table.cos.to(x.device)[pos][:, None, :]
+    s = table.sin.to(x.device)[pos][:, None, :] * sign
+    a, b = x[..., :half], x[..., half:2 * half]
+    return torch.cat([a * c - b * s, b * c + a * s, x[..., 2 * half:]], dim=-1)
+
+
+def qk_norm_rope_inplace(qkv, n_q, n_kv, head_dim, table, w_q, w_k, eps, positions=None, seq_len=None, need_raw=True):
+    """Qwen3's QK-norm followed by RoPE, **in place** on the Q and K heads of a packed
+    ``[tokens, (n_q + 2 n_kv) * head_dim]`` buffer (any row stride): every query head becomes
+    ``rope(w_q * q * rsqrt(mean(q^2) + eps))`` and every key head the same with ``w_k``; V is untouched.  ``positions`` /
+    ``seq_len`` as in :func:`rope_qk_inplace`; ``table=None`` normalises without rotating.
+
+    All arithmetic is fp32 and each result is rounded to the buffer's dtype once.  (HF's ``Qwen3RMSNorm`` rounds the
+    normalised value to the input dtype before the weight multiply and RoPE rounds again, so a bf16 HF model differs
+    from this in the last bits; in fp32 the two agree.)
+
+    Returns the pre-norm Q|K heads ``[tokens, (n_q + n_kv) * head_dim]`` (contiguous, the buffer's dtype), which
+    :func:`qk_norm_rope_bwd_inplace` takes, or ``None`` with ``need_raw=False`` (no backward follows).  Not
+    autograd-tracked.  CUDA bf16 / fp16 / fp32 buffers with head dim 64 or
+    128 and a full rotary table run one fused kernel; every other case (another head dim, a partial rotary table, a CPU
+    tensor) an fp32 torch composition with the same semantics."""
+    tokens = qkv.shape[0]
+    seq_len = seq_len or tokens
+    heads = _qk_heads(qkv, n_q, n_kv, head_dim)
+    if _qk_norm_native(qkv, head_dim, table):
+        raw = torch.empty(tokens, (n_q + n_kv) * head_dim, dtype=qkv.dtype, device=qkv.device) if need_raw else None
+        w_q, w_k = w_q.to(qkv.dtype).contiguous(), w_k.to(qkv.dtype).contiguous()
+        rc = N.cuda().dsb_qk_norm_rope(_p(qkv), _p(raw), _p(table.cos), _p(table.sin), _p(positions), _p(w_q), _p(w_k),
+                                       N.c_i64(tokens), n_q, n_kv, head_dim, N.c_i64(qkv.stride(0)), seq_len,
+                                       N.c_f(eps), N.dt(qkv), N.stream())
+        N.check(rc, "qk_norm_rope")
+        return raw
+    return _qk_norm_rope_torch(heads, n_q, table, w_q, w_k, eps, positions, seq_len, need_raw)
+
+
+def _qk_norm_rope_torch(heads, n_q, table, w_q, w_k, eps, positions, seq_len, need_raw=True):
+    """The fp32 torch composition of :func:`qk_norm_rope_inplace`, on its ``[tokens, n_q + n_kv, head_dim]`` view."""
+    tokens, n, head_dim = heads.shape
+    raw = heads.reshape(tokens, n * head_dim).clone() if need_raw else None
+    x = heads.float()
+    y = x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps) * _qk_weights(w_q, w_k, n_q, n - n_q)
+    heads.copy_(_rotate_f32(y, table, positions, seq_len, 1.0).to(heads.dtype))
+    return raw
+
+
+def qk_norm_rope_bwd_inplace(dqkv, raw, n_q, n_kv, head_dim, table, w_q, w_k, eps, positions=None, seq_len=None):
+    """Backward of :func:`qk_norm_rope_inplace`, **in place** on the dQ and dK heads of the packed gradient ``dqkv`` (same
+    layout as the forward's buffer; dV untouched), given the ``raw`` pre-norm heads the forward returned.  Returns
+    ``(dw_q, dw_k)`` in the weights' dtypes: fp32 sums over tokens and over the heads of each kind, in a fixed order (the
+    CUDA kernel reduces per-CTA partials with the column-sum kernel), so they are bit-reproducible from run to run."""
+    tokens = dqkv.shape[0]
+    seq_len = seq_len or tokens
+    heads = _qk_heads(dqkv, n_q, n_kv, head_dim)
+    if _qk_norm_native(dqkv, head_dim, table):
+        assert raw.is_contiguous() and raw.dtype == dqkv.dtype and raw.shape == (tokens, (n_q + n_kv) * head_dim)
+        lib = N.cuda()
+        grid = lib.dsb_qk_norm_rope_bwd_grid(N.c_i64(tokens), n_q + n_kv, head_dim, N.dt(dqkv))
+        dw_part = torch.empty(grid, 2 * head_dim, dtype=torch.float32, device=dqkv.device)
+        dw = torch.empty(2 * head_dim, dtype=w_q.dtype, device=dqkv.device)
+        wq, wk = w_q.to(dqkv.dtype).contiguous(), w_k.to(dqkv.dtype).contiguous()
+        rc = lib.dsb_qk_norm_rope_bwd(_p(dqkv), _p(raw), _p(table.cos), _p(table.sin), _p(positions), _p(wq), _p(wk),
+                                      _p(dw_part), _p(dw), N.c_i64(tokens), n_q, n_kv, head_dim,
+                                      N.c_i64(dqkv.stride(0)), seq_len, N.c_f(eps), N.dt(dqkv), N.dt(w_q), N.stream())
+        N.check(rc, "qk_norm_rope_bwd")
+        return dw[:head_dim].to(w_q.dtype), dw[head_dim:].to(w_k.dtype)
+    return _qk_norm_rope_bwd_torch(heads, raw, n_q, table, w_q, w_k, eps, positions, seq_len)
+
+
+def _qk_norm_rope_bwd_torch(heads, raw, n_q, table, w_q, w_k, eps, positions, seq_len):
+    """The fp32 torch composition of :func:`qk_norm_rope_bwd_inplace`, on its ``[tokens, n_q + n_kv, head_dim]`` view."""
+    tokens, n, head_dim = heads.shape
+    r = _rotate_f32(heads.float(), table, positions, seq_len, -1.0)
+    x = raw.view(tokens, n, head_dim).float()
+    rstd = torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps)
+    xhat = x * rstd
+    g = r * _qk_weights(w_q, w_k, n_q, n - n_q)
+    dw = r * xhat  # before the store below: without a table r is a view of the fp32 buffer
+    heads.copy_((rstd * (g - xhat * (g * xhat).mean(-1, keepdim=True))).to(heads.dtype))
+    return dw[:, :n_q].sum((0, 1)).to(w_q.dtype), dw[:, n_q:].sum((0, 1)).to(w_k.dtype)
+
+
+# ---------------------------------------------------------------------------------------------------
 # gated activation (SwiGLU & friends)
 # ---------------------------------------------------------------------------------------------------
 def gated_act_fwd_raw(gu, act=ACT_SILU, out=None):
