@@ -9,6 +9,8 @@
   produced in place by the fused kernel, ``dh`` and ``dW`` are accumulated per chunk, so the
   ``[tokens, vocab]`` logits tensor is never materialised (role: reference ``FPDT_LogitsLoss``).
 """
+import functools
+
 import torch
 import torch.nn.functional as F
 
@@ -29,6 +31,28 @@ def _gemm(a, b_t):
     return gemm.matmul_nt(a, b_t)
 
 
+def _weight_grad_sink(w, dtype, into, product, unowned=None):
+    """Where the gradient of the 2-D weight ``w`` goes.  With a ZeRO owner it lands in the flat gradient view
+    ``grad_view_for(w)``, stored on the micro step's first contribution and accumulated on later ones, and ``w`` is
+    marked ready (returns None): ``into(out=view, accumulate=...)`` writes it there when the view has the product's
+    ``dtype``; a view of another dtype (fp32 accumulation) takes ``product()`` by copy or add.  Without an owner
+    ``unowned()`` (default ``product()``) is returned to autograd.
+
+    Marking a unit's last gradient reduces it, which under ZeRO-3 releases the gathered weights and with the step fused
+    into backward rewrites them: a node reads no weight after it has marked all of them."""
+    zo = _zo_of(w)
+    if zo is None:
+        return (unowned or product)()
+    gv = zo.grad_view_for(w)
+    if gv.dtype == dtype:
+        into(out=gv, accumulate=not zo.grad_is_fresh(w))
+    else:
+        g = product()
+        gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
+    zo.mark_grad_ready(w)
+    return None
+
+
 class _FlatLinearFn(torch.autograd.Function):
 
     @staticmethod
@@ -44,29 +68,17 @@ class _FlatLinearFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy):
+        from deepspeed_b200.ops import gemm
         (x, ) = ctx.saved_tensors
         w = ctx.weight_ref
         dy2 = dy.reshape(-1, dy.shape[-1])
         x2 = x.reshape(-1, x.shape[-1])
-        dx = None
-        if ctx.needs_input_grad[0]:
-            from deepspeed_b200.ops import gemm
-            dx = gemm.matmul_nn(dy2, w).view(x.shape)
+        dx = gemm.matmul_nn(dy2, w).view(x.shape) if ctx.needs_input_grad[0] else None
         dw = None
         if ctx.needs_input_grad[1]:
-            zo = _zo_of(w)
-            if zo is not None:
-                gv = zo.grad_view_for(w)
-                if gv.dtype == dy2.dtype:
-                    from deepspeed_b200.ops import gemm
-                    # first micro step: overwrite; later ones: accumulate in the GEMM epilogue (no addmm, no memset)
-                    gemm.matmul_tn(dy2, x2, out=gv, accumulate=not zo.grad_is_fresh(w))
-                else:
-                    g = torch.mm(dy2.t(), x2)
-                    gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
-                zo.mark_grad_ready(w)
-            else:
-                dw = torch.mm(dy2.t(), x2)
+            # into the view: stored on the first micro step, accumulated in the GEMM epilogue later (no addmm, no memset)
+            dw = _weight_grad_sink(w, dy2.dtype, functools.partial(gemm.matmul_tn, dy2, x2),
+                                   lambda: torch.mm(dy2.t(), x2))
         db = dy2.sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
         return dx, dw, db
 
@@ -79,23 +91,6 @@ def flat_linear(x, weight, bias=None):
             y = y + bias
         return y.view(*x.shape[:-1], weight.shape[0])
     return _FlatLinearFn.apply(x, weight, bias)
-
-
-def _write_weight_grad(w, dy2, x2):
-    """dW = dy2^T x2 for parameter ``w``: straight into the ZeRO flat gradient view when there is one (returns None),
-    else returned for autograd."""
-    from deepspeed_b200.ops import gemm
-    zo = _zo_of(w)
-    if zo is None:
-        return gemm.matmul_tn(dy2, x2)
-    gv = zo.grad_view_for(w)
-    if gv.dtype == dy2.dtype:
-        gemm.matmul_tn(dy2, x2, out=gv, accumulate=not zo.grad_is_fresh(w))
-    else:
-        g = torch.mm(dy2.t(), x2)
-        gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
-    zo.mark_grad_ready(w)
-    return None
 
 
 class _SwiGLUMLPFn(torch.autograd.Function):
@@ -150,9 +145,14 @@ class _SwiGLUMLPFn(torch.autograd.Function):
         if act is None and ctx.needs_input_grad[2]:
             act = act_out = torch.empty(gu.shape[0], gu.shape[1] // 2, dtype=gu.dtype, device=gu.device)
         dgu = gemm.down_dx_dswiglu(dy2, w_down, gu, act_out=act_out)
-        dw_down = _write_weight_grad(w_down, dy2, act) if ctx.needs_input_grad[2] else None
+
+        def weight_grad(w, a, b):  # dW = a^T b
+            mm = functools.partial(gemm.matmul_tn, a, b)
+            return _weight_grad_sink(w, a.dtype, mm, lambda: torch.mm(a.t(), b), unowned=mm)
+
+        dw_down = weight_grad(w_down, dy2, act) if ctx.needs_input_grad[2] else None
         dx = gemm.matmul_nn(dgu, w_gu).view(ctx.x_shape) if ctx.needs_input_grad[0] else None
-        dw_gu = _write_weight_grad(w_gu, dgu, x2) if ctx.needs_input_grad[1] else None
+        dw_gu = weight_grad(w_gu, dgu, x2) if ctx.needs_input_grad[1] else None
         return dx, dw_gu, dw_down, None
 
 
@@ -174,75 +174,6 @@ def _fp8_native(x2, *ws, inter=None) -> bool:
     return inter is None or inter % 64 == 0
 
 
-def _fp8_cast_fn(native):
-    from deepspeed_b200.ops import fp8
-    return fp8.quantize_tensorwise if native else fp8.quantize_reference
-
-
-def _fp8_weight_grad(w, a8t, b8t, sa, sb, native, block=False):
-    """dW = sa sb a8t b8t^T (``a8t`` the e5m2 gradient transposed, ``b8t`` the e4m3 input transposed; ``block``: scaled
-    blockwise): stored, or accumulated on later micro steps, straight into the ZeRO flat gradient view when there is one
-    (returns None), else returned for autograd."""
-    from deepspeed_b200.ops import fp8
-    zo = _zo_of(w)
-    if zo is None:
-        return fp8.gemm(a8t, b8t, sa, sb, native, block=block).to(w.dtype)
-    gv = zo.grad_view_for(w)
-    if gv.dtype == torch.bfloat16:
-        fp8.gemm(a8t, b8t, sa, sb, native, out=gv, accumulate=not zo.grad_is_fresh(w), block=block)
-    else:
-        g = fp8.gemm(a8t, b8t, sa, sb, native, block=block)
-        gv.copy_(g) if zo.grad_is_fresh(w) else gv.add_(g)
-    zo.mark_grad_ready(w)
-    return None
-
-
-class _FP8LinearFn(torch.autograd.Function):
-    """``y = x W^T (+ b)`` in FP8 (the recipe of :mod:`deepspeed_b200.ops.fp8`): forward casts ``x`` to e4m3 (and its
-    transpose, for dW) and ``W`` to e4m3 and saves only the transposed ``x`` and its scale; backward casts ``dY`` (and its
-    transpose) to e5m2 and re-reads the weight (as :class:`_FlatLinearFn`, so ZeRO-3 may release it after forward) to
-    cast ``W^T``.  dW lands in the ZeRO flat gradient view."""
-
-    @staticmethod
-    def forward(ctx, x, weight, bias):
-        from deepspeed_b200.ops import fp8
-        x2 = x.reshape(-1, x.shape[-1])
-        native = _fp8_native(x2, weight)
-        cast = _fp8_cast_fn(native)
-        x8, x8t, sx = cast(x2, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[1])
-        w8, _, sw = cast(weight, fp8.E4M3)
-        y = fp8.gemm(x8, w8, sx, sw, native).to(x.dtype)
-        if bias is not None:
-            y = y + bias
-        ctx.weight_ref = weight
-        ctx.has_bias = bias is not None
-        ctx.native = native
-        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
-        ctx.save_for_backward(x8t, sx)
-        return y.view(*x.shape[:-1], weight.shape[0])
-
-    @staticmethod
-    def backward(ctx, dy):
-        from deepspeed_b200.ops import fp8
-        x8t, sx = ctx.saved_tensors
-        w, native = ctx.weight_ref, ctx.native
-        cast = _fp8_cast_fn(native)
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        dx = dw = None
-        if need_dx or need_dw:
-            dy8, dy8t, sdy = cast(dy2, fp8.E5M2, rowwise=need_dx, colwise=need_dw)
-            if need_dx:
-                _, w8t, sw = cast(w, fp8.E4M3, rowwise=False, colwise=True)
-                dx = fp8.gemm(dy8, w8t, sdy, sw, native).to(ctx.x_dtype).view(ctx.x_shape)
-            if need_dw:
-                dw = _fp8_weight_grad(w, dy8t, x8t, sdy, sx, native)
-        db = dy2.sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
-        return dx, dw, db
-
-
 FP8_RECIPES = ("tensorwise", "blockwise")
 
 
@@ -251,33 +182,47 @@ def _check_recipe(recipe):
         raise ValueError(f"fp8 recipe must be one of {FP8_RECIPES}, got {recipe!r}")
 
 
-def _fp8_block_cast_fn(native):
+def _fp8_cast4(native, block):
+    """``cast(x, fmt, row, col) -> (q, sq, qt, sqt)`` for either recipe (``block``: blockwise), on the cast kernels
+    (``native``) or the torch reference: the modes of :func:`fp8.quantize_blockwise`; under the tensorwise recipe a mode
+    only asks for its copy, and both copies share the one scale."""
     from deepspeed_b200.ops import fp8
-    return fp8.quantize_blockwise if native else fp8.quantize_blockwise_reference
+    if block:
+        return fp8.quantize_blockwise if native else fp8.quantize_blockwise_reference
+    q = fp8.quantize_tensorwise if native else fp8.quantize_reference
+
+    def cast(x, fmt, row="strip", col=None):
+        a, at, s = q(x, fmt, rowwise=row is not None, colwise=col is not None)
+        return a, s, at, s
+
+    return cast
 
 
-class _FP8BlockLinearFn(torch.autograd.Function):
-    """:class:`_FP8LinearFn` under the blockwise recipe of :mod:`deepspeed_b200.ops.fp8`.  The ``A`` of each product is
-    scaled in 1 x 128 strips along its contraction, the ``B`` in 128 x 128 blocks:
+class _FP8LinearFn(torch.autograd.Function):
+    """``y = x W^T (+ b)`` in FP8 under either recipe of :mod:`deepspeed_b200.ops.fp8` (``block``: blockwise).  Forward
+    saves only the transposed cast of ``x`` and its scales; backward re-reads the weight (as :class:`_FlatLinearFn`, so
+    ZeRO-3 may release it after forward) to cast ``W^T``, and dW lands in the ZeRO flat gradient view.  Under the
+    blockwise recipe the ``A`` of each product is scaled in 1 x 128 strips along its contraction, the ``B`` in 128 x 128
+    blocks (tensorwise: one scale per cast):
 
     forward  ``x`` -> e4m3 strips (and, in the same pass, ``x^T`` in blocks for dW, the only copy saved); ``W`` in blocks;
     dgrad    ``dY`` -> e5m2 strips along the output features; ``W^T`` in blocks, cast from the re-read weight;
     wgrad    ``dY^T`` -> e5m2 strips along the tokens (same pass as dgrad's copy, different scales); saved ``x^T``."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias):
+    def forward(ctx, x, weight, bias, block):
         from deepspeed_b200.ops import fp8
         x2 = x.reshape(-1, x.shape[-1])
         native = _fp8_native(x2, weight)
-        cast = _fp8_block_cast_fn(native)
+        cast = _fp8_cast4(native, block)
         x8, sx, x8t, sxt = cast(x2, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[1] else None)
         w8, sw, _, _ = cast(weight, fp8.E4M3, row="block")
-        y = fp8.gemm(x8, w8, sx, sw, native, block=True).to(x.dtype)
+        y = fp8.gemm(x8, w8, sx, sw, native, block=block).to(x.dtype)
         if bias is not None:
             y = y + bias
         ctx.weight_ref = weight
         ctx.has_bias = bias is not None
-        ctx.native = native
+        ctx.native, ctx.block = native, block
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.save_for_backward(x8t, sxt)
         return y.view(*x.shape[:-1], weight.shape[0])
@@ -286,8 +231,8 @@ class _FP8BlockLinearFn(torch.autograd.Function):
     def backward(ctx, dy):
         from deepspeed_b200.ops import fp8
         x8t, sxt = ctx.saved_tensors
-        w, native = ctx.weight_ref, ctx.native
-        cast = _fp8_block_cast_fn(native)
+        w, native, block = ctx.weight_ref, ctx.native, ctx.block
+        cast = _fp8_cast4(native, block)
         dy2 = dy.reshape(-1, dy.shape[-1])
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
@@ -297,100 +242,48 @@ class _FP8BlockLinearFn(torch.autograd.Function):
             dy8, sdy, dy8t, sdyt = cast(dy2, fp8.E5M2, row="strip" if need_dx else None, col="strip" if need_dw else None)
             if need_dx:
                 _, _, w8t, swt = cast(w, fp8.E4M3, row=None, col="block")
-                dx = fp8.gemm(dy8, w8t, sdy, swt, native, block=True).to(ctx.x_dtype).view(ctx.x_shape)
+                dx = fp8.gemm(dy8, w8t, sdy, swt, native, block=block).to(ctx.x_dtype).view(ctx.x_shape)
             if need_dw:
-                dw = _fp8_weight_grad(w, dy8t, x8t, sdyt, sxt, native, block=True)
+                mm = functools.partial(fp8.gemm, dy8t, x8t, sdyt, sxt, native, block=block)
+                dw = _weight_grad_sink(w, torch.bfloat16, mm, mm, lambda: mm().to(w.dtype))
         db = dy2.sum(0) if ctx.has_bias and ctx.needs_input_grad[2] else None
-        return dx, dw, db
+        return dx, dw, db, None
 
 
 def fp8_linear(x, weight, bias=None, recipe="tensorwise"):
-    """``x W^T (+ b)`` with FP8 products (see :class:`_FP8LinearFn`; ``recipe="blockwise"``:
-    :class:`_FP8BlockLinearFn`).  CUDA bf16 operands whose dimensions are multiples of 16 run the wgmma kernels; anything
-    else runs the torch reference of the same recipe (never a bf16 product)."""
+    """``x W^T (+ b)`` with FP8 products (see :class:`_FP8LinearFn`).  CUDA bf16 operands whose dimensions are multiples
+    of 16 run the wgmma kernels; anything else runs the torch reference of the same recipe (never a bf16 product)."""
     _check_recipe(recipe)
-    if recipe == "blockwise":
-        return _FP8BlockLinearFn.apply(x, weight, bias)
-    return _FP8LinearFn.apply(x, weight, bias)
+    return _FP8LinearFn.apply(x, weight, bias, recipe == "blockwise")
 
 
 class _FP8SwiGLUMLPFn(torch.autograd.Function):
-    """``down(silu(gate(x)) * up(x))`` in FP8, one node like :class:`_SwiGLUMLPFn`:
+    """``down(silu(gate(x)) * up(x))`` in FP8, one node like :class:`_SwiGLUMLPFn` (``block``: the blockwise recipe):
 
     forward   x -> e4m3 (+ transposed); gate|up FP8 GEMM with the SwiGLU epilogue (gate|up saved in bf16);
               act -> e4m3 (+ transposed); FP8 down GEMM;
     backward  dY -> e5m2 (+ transposed); FP8 ``dY W_down`` GEMM with the dSwiGLU epilogue; dgate|dup -> e5m2 (+ transposed);
               FP8 dX, dW_down and dW_gate_up, the weight gradients into the ZeRO flat gradient views.
-    Every read of a weight comes before either weight's gradient is marked ready (marking a unit's last gradient reduces
-    it, which under ZeRO-3 releases the gathered weights and with the step fused into backward rewrites them)."""
+    Operand by operand as in :class:`_FP8LinearFn`: the row-major casts (``x``, ``act``, ``dY``, ``dgate|dup``) are scaled
+    in 1 x 128 strips, the weights and the saved ``x^T`` and ``act^T`` in 128 x 128 blocks, ``dY^T`` and ``dgate|dup^T``
+    in strips along the tokens.  Every read of a weight comes before either weight's gradient is marked ready (marking a
+    unit's last gradient reduces it, which under ZeRO-3 releases the gathered weights and with the step fused into
+    backward rewrites them)."""
 
     @staticmethod
-    def forward(ctx, x, w_gu, w_down):
+    def forward(ctx, x, w_gu, w_down, block):
         from deepspeed_b200.ops import fp8
         x2 = x.reshape(-1, x.shape[-1])
         native = _fp8_native(x2, w_gu, w_down, inter=w_down.shape[1])
-        cast = _fp8_cast_fn(native)
-        need_grad = any(ctx.needs_input_grad)
-        x8, x8t, sx = cast(x2, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[1])
-        wgu8, _, sgu = cast(w_gu, fp8.E4M3)
-        act, gu = fp8.gemm_swiglu(x8, wgu8, sx, sgu, native, save_gate_up=need_grad)
-        act8, act8t, sa = cast(act, fp8.E4M3, rowwise=True, colwise=ctx.needs_input_grad[2])
-        wd8, _, sd = cast(w_down, fp8.E4M3)
-        y = fp8.gemm(act8, wd8, sa, sd, native).to(x.dtype)
-        ctx.w_gu, ctx.w_down, ctx.native = w_gu, w_down, native
-        ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
-        ctx.save_for_backward(x8t, sx, gu, act8t, sa)
-        return y.view(*x.shape[:-1], w_down.shape[0])
-
-    @staticmethod
-    def backward(ctx, dy):
-        from deepspeed_b200.ops import fp8
-        x8t, sx, gu, act8t, sa = ctx.saved_tensors
-        w_gu, w_down, native = ctx.w_gu, ctx.w_down, ctx.native
-        cast = _fp8_cast_fn(native)
-        need_dx, need_dgu, need_dd = ctx.needs_input_grad
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
-        dy8, dy8t, sdy = cast(dy2, fp8.E5M2, rowwise=True, colwise=need_dd)
-        _, wd8t, sd = cast(w_down, fp8.E4M3, rowwise=False, colwise=True)
-        dgu = fp8.gemm_dswiglu(dy8, wd8t, sdy, sd, gu, native)
-        wgu8t = sgu = None
-        if need_dx:
-            _, wgu8t, sgu = cast(w_gu, fp8.E4M3, rowwise=False, colwise=True)
-        dx = dw_gu = dw_down = None
-        if need_dx or need_dgu:
-            dgu8, dgu8t, sg = cast(dgu, fp8.E5M2, rowwise=need_dx, colwise=need_dgu)
-            if need_dx:
-                dx = fp8.gemm(dgu8, wgu8t, sg, sgu, native).to(ctx.x_dtype).view(ctx.x_shape)
-        # weights are not read past this point
-        if need_dd:
-            dw_down = _fp8_weight_grad(w_down, dy8t, act8t, sdy, sa, native)
-        if need_dgu:
-            dw_gu = _fp8_weight_grad(w_gu, dgu8t, x8t, sg, sx, native)
-        return dx, dw_gu, dw_down
-
-
-class _FP8BlockSwiGLUMLPFn(torch.autograd.Function):
-    """:class:`_FP8SwiGLUMLPFn` under the blockwise recipe, operand by operand as in :class:`_FP8BlockLinearFn`: the row-major
-    casts (``x``, ``act``, ``dY``, ``dgate|dup``) are scaled in 1 x 128 strips, the weights and the saved ``x^T`` and
-    ``act^T`` in 128 x 128 blocks, ``dY^T`` and ``dgate|dup^T`` in strips along the tokens.  The same order of weight
-    reads and gradient marks."""
-
-    @staticmethod
-    def forward(ctx, x, w_gu, w_down):
-        from deepspeed_b200.ops import fp8
-        x2 = x.reshape(-1, x.shape[-1])
-        native = _fp8_native(x2, w_gu, w_down, inter=w_down.shape[1])
-        cast = _fp8_block_cast_fn(native)
+        cast = _fp8_cast4(native, block)
         need_grad = any(ctx.needs_input_grad)
         x8, sx, x8t, sxt = cast(x2, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[1] else None)
         wgu8, sgu, _, _ = cast(w_gu, fp8.E4M3, row="block")
-        act, gu = fp8.gemm_swiglu(x8, wgu8, sx, sgu, native, save_gate_up=need_grad, block=True)
+        act, gu = fp8.gemm_swiglu(x8, wgu8, sx, sgu, native, save_gate_up=need_grad, block=block)
         act8, sa, act8t, sat = cast(act, fp8.E4M3, row="strip", col="block" if ctx.needs_input_grad[2] else None)
         wd8, sd, _, _ = cast(w_down, fp8.E4M3, row="block")
-        y = fp8.gemm(act8, wd8, sa, sd, native, block=True).to(x.dtype)
-        ctx.w_gu, ctx.w_down, ctx.native = w_gu, w_down, native
+        y = fp8.gemm(act8, wd8, sa, sd, native, block=block).to(x.dtype)
+        ctx.w_gu, ctx.w_down, ctx.native, ctx.block = w_gu, w_down, native, block
         ctx.x_shape, ctx.x_dtype = x.shape, x.dtype
         ctx.save_for_backward(x8t, sxt, gu, act8t, sat)
         return y.view(*x.shape[:-1], w_down.shape[0])
@@ -399,15 +292,15 @@ class _FP8BlockSwiGLUMLPFn(torch.autograd.Function):
     def backward(ctx, dy):
         from deepspeed_b200.ops import fp8
         x8t, sxt, gu, act8t, sat = ctx.saved_tensors
-        w_gu, w_down, native = ctx.w_gu, ctx.w_down, ctx.native
-        cast = _fp8_block_cast_fn(native)
-        need_dx, need_dgu, need_dd = ctx.needs_input_grad
+        w_gu, w_down, native, block = ctx.w_gu, ctx.w_down, ctx.native, ctx.block
+        cast = _fp8_cast4(native, block)
+        need_dx, need_dgu, need_dd = ctx.needs_input_grad[:3]
         dy2 = dy.reshape(-1, dy.shape[-1])
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
         dy8, sdy, dy8t, sdyt = cast(dy2, fp8.E5M2, row="strip", col="strip" if need_dd else None)
         _, _, wd8t, sdt = cast(w_down, fp8.E4M3, row=None, col="block")
-        dgu = fp8.gemm_dswiglu(dy8, wd8t, sdy, sdt, gu, native, block=True)
+        dgu = fp8.gemm_dswiglu(dy8, wd8t, sdy, sdt, gu, native, block=block)
         wgu8t = sgut = None
         if need_dx:
             _, _, wgu8t, sgut = cast(w_gu, fp8.E4M3, row=None, col="block")
@@ -415,23 +308,42 @@ class _FP8BlockSwiGLUMLPFn(torch.autograd.Function):
         if need_dx or need_dgu:
             dgu8, sg, dgu8t, sgt = cast(dgu, fp8.E5M2, row="strip" if need_dx else None, col="strip" if need_dgu else None)
             if need_dx:
-                dx = fp8.gemm(dgu8, wgu8t, sg, sgut, native, block=True).to(ctx.x_dtype).view(ctx.x_shape)
+                dx = fp8.gemm(dgu8, wgu8t, sg, sgut, native, block=block).to(ctx.x_dtype).view(ctx.x_shape)
         # weights are not read past this point
         if need_dd:
-            dw_down = _fp8_weight_grad(w_down, dy8t, act8t, sdyt, sat, native, block=True)
+            mm = functools.partial(fp8.gemm, dy8t, act8t, sdyt, sat, native, block=block)
+            dw_down = _weight_grad_sink(w_down, torch.bfloat16, mm, mm, lambda: mm().to(w_down.dtype))
         if need_dgu:
-            dw_gu = _fp8_weight_grad(w_gu, dgu8t, x8t, sgt, sxt, native, block=True)
-        return dx, dw_gu, dw_down
+            mm = functools.partial(fp8.gemm, dgu8t, x8t, sgt, sxt, native, block=block)
+            dw_gu = _weight_grad_sink(w_gu, torch.bfloat16, mm, mm, lambda: mm().to(w_gu.dtype))
+        return dx, dw_gu, dw_down, None
 
 
 def fp8_swiglu_mlp(x, w_gate_up, w_down, recipe="tensorwise"):
-    """SwiGLU MLP block (no biases) with FP8 products: see :class:`_FP8SwiGLUMLPFn` (``recipe="blockwise"``:
-    :class:`_FP8BlockSwiGLUMLPFn`).  CUDA bf16 operands with ``T, H, 2I`` multiples of 16 and ``I % 64 == 0`` run the
-    wgmma kernels; anything else runs the torch reference of the same recipe (never a bf16 product)."""
+    """SwiGLU MLP block (no biases) with FP8 products: see :class:`_FP8SwiGLUMLPFn`.  CUDA bf16 operands with ``T, H, 2I``
+    multiples of 16 and ``I % 64 == 0`` run the wgmma kernels; anything else runs the torch reference of the same recipe
+    (never a bf16 product)."""
     _check_recipe(recipe)
-    if recipe == "blockwise":
-        return _FP8BlockSwiGLUMLPFn.apply(x, w_gate_up, w_down)
-    return _FP8SwiGLUMLPFn.apply(x, w_gate_up, w_down)
+    return _FP8SwiGLUMLPFn.apply(x, w_gate_up, w_down, recipe == "blockwise")
+
+
+def _stacked_grad_target(w, dtype):
+    """-> (zo, gradient tensor, accumulate) for a stacked expert weight: its flat ZeRO gradient view when it has one of
+    ``dtype`` (None: of any dtype) -- the GEMM epilogue stores or accumulates there -- else a fresh tensor returned to
+    autograd.  :func:`_mark_or_return` finishes it."""
+    zo = _zo_of(w)
+    if zo is not None and (dtype is None or zo.grad_view_for(w).dtype == dtype):
+        return zo, zo.grad_view_for(w), not zo.grad_is_fresh(w)
+    return None, torch.empty_like(w), False
+
+
+def _mark_or_return(zo, w, g):
+    """The gradient ``g`` of ``w`` from :func:`_stacked_grad_target`, once written: ``w`` marked ready when ``g`` is its
+    owner's view (returns None), else ``g`` for autograd."""
+    if zo is None:
+        return g
+    zo.mark_grad_ready(w)
+    return None
 
 
 class _GroupedSwiGLUFn(torch.autograd.Function):
@@ -465,49 +377,23 @@ class _GroupedSwiGLUFn(torch.autograd.Function):
         E = x.shape[0]
         dy = dy.contiguous()
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
-        views = {}
-        for w, need in ((w13, ctx.needs_input_grad[1]), (w2, ctx.needs_input_grad[2])):
-            if not need:
-                views[id(w)] = (None, None, False)
-                continue
-            zo = _zo_of(w)
-            if zo is not None and zo.grad_view_for(w).dtype == dy.dtype:
-                views[id(w)] = (zo, zo.grad_view_for(w), not zo.grad_is_fresh(w))
-            else:
-                views[id(w)] = (None, torch.empty_like(w), False)
+        no_grad = (None, None, False)
+        zo13, g13, acc13 = _stacked_grad_target(w13, dy.dtype) if ctx.needs_input_grad[1] else no_grad
+        zo2, g2, acc2 = _stacked_grad_target(w2, dy.dtype) if ctx.needs_input_grad[2] else no_grad
         for e in range(E):
             dgu = gemm.down_dx_dswiglu(dy[e], w2[e], gus[e])
-            _, g2, acc2 = views[id(w2)]
             if g2 is not None:
                 gemm.matmul_tn(dy[e], acts[e], out=g2[e], accumulate=acc2)
             if dx is not None:
                 gemm.matmul_nn(dgu, w13[e], out=dx[e])
-            _, g13, acc13 = views[id(w13)]
             if g13 is not None:
                 gemm.matmul_tn(dgu, x[e], out=g13[e], accumulate=acc13)
             gus[e] = acts[e] = None
-        outs = []
-        for w in (w13, w2):
-            zo, g, _ = views[id(w)]
-            if zo is not None:
-                zo.mark_grad_ready(w)
-                outs.append(None)
-            else:
-                outs.append(g)
-        return dx, outs[0], outs[1]
+        return dx, _mark_or_return(zo13, w13, g13), _mark_or_return(zo2, w2, g2)
 
 
 def grouped_swiglu_mlp(x, w13, w2):
     return _GroupedSwiGLUFn.apply(x, w13, w2)
-
-
-def _stacked_grad_target(w, dtype):
-    """-> (zo, gradient tensor, accumulate) for a stacked expert weight: its flat ZeRO gradient view when it has one of
-    ``dtype`` (the GEMM epilogue stores or accumulates there), else a fresh tensor returned to autograd."""
-    zo = _zo_of(w)
-    if zo is not None and zo.grad_view_for(w).dtype == dtype:
-        return zo, zo.grad_view_for(w), not zo.grad_is_fresh(w)
-    return None, torch.empty_like(w), False
 
 
 class _RaggedSwiGLUFn(torch.autograd.Function):
@@ -551,10 +437,7 @@ class _RaggedSwiGLUFn(torch.autograd.Function):
                 continue
             zo, g, accumulate = _stacked_grad_target(w, dy.dtype)
             K.ragged_wgrad(a, b, offsets, E, out=g, accumulate=accumulate)
-            if zo is not None:
-                zo.mark_grad_ready(w)
-                g = None
-            outs[i] = g
+            outs[i] = _mark_or_return(zo, w, g)
         return dx, None, outs[2], outs[3]
 
 
@@ -595,23 +478,9 @@ def ragged_swiglu_mlp(x, offsets, w13, w2, act="silu"):
     return ragged_swiglu_reference(x, offsets, w13, w2, act)
 
 
-def _fp8_cast4(native, block):
-    """``cast(x, fmt, row, col) -> (q, sq, qt, sqt)`` for either recipe: the modes of :func:`fp8.quantize_blockwise`; under
-    the tensorwise recipe a mode only asks for its copy, and both copies share the one scale."""
-    if block:
-        return _fp8_block_cast_fn(native)
-    q = _fp8_cast_fn(native)
-
-    def cast(x, fmt, row="strip", col=None):
-        a, at, s = q(x, fmt, rowwise=row is not None, colwise=col is not None)
-        return a, s, at, s
-
-    return cast
-
-
 class _FP8RaggedSwiGLUFn(torch.autograd.Function):
     """:class:`_RaggedSwiGLUFn` with FP8 products (tensorwise, or ``block``: blockwise, operand by operand as in
-    :class:`_FP8BlockSwiGLUMLPFn`), on 128-row segments.  The stacked weights are cast as the 2-D matrices
+    :class:`_FP8SwiGLUMLPFn`), on 128-row segments.  The stacked weights are cast as the 2-D matrices
     ``w13 [E 2I, H]`` and ``w2 [E H, I]`` (one tensorwise scale per stacked weight); forward and dgrad take expert e's
     row slab of the cast or column slab of its transposed cast, and the variable-K wgrad sums each expert's rows of the
     transposed activation and gradient copies.  The forward saves only those transposed copies, their scales and the
@@ -665,16 +534,10 @@ class _FP8RaggedSwiGLUFn(torch.autograd.Function):
             if not ctx.needs_input_grad[i]:
                 grads[i] = None
                 continue
-            zo = _zo_of(w)
-            if zo is not None and (not native or zo.grad_view_for(w).dtype == torch.bfloat16):
-                g, accumulate = zo.grad_view_for(w), not zo.grad_is_fresh(w)
-            else:
-                zo, g, accumulate = None, torch.empty_like(w), False
+            # the kernels write a bf16 view; the torch reference one of any dtype
+            zo, g, accumulate = _stacked_grad_target(w, torch.bfloat16 if native else None)
             fp8.ragged_wgrad(a8t, b8t, offsets, s_a, s_b, E, native, out=g, accumulate=accumulate, block=block)
-            if zo is not None:
-                zo.mark_grad_ready(w)
-                g = None
-            grads[i] = g
+            grads[i] = _mark_or_return(zo, w, g)
         return dx, None, grads[2], grads[3], None, None
 
 

@@ -542,15 +542,16 @@ def _blockwise_llama_zero3():
     accumulated by the GEMM epilogue on the second; the gradients match the bf16 model's on the same weights."""
     from deepspeed_b200.ops import linear, native
     ran = {"accum": 0, "store": 0}
-    real = linear._fp8_weight_grad
+    real = linear._weight_grad_sink
 
-    def weight_grad(w, *a, **k):
+    def weight_grad(w, dtype, into, *a, **k):
+        # every projection of this model is an FP8 node, whose sink writes with a partial of the FP8 GEMM
         zo = linear._zo_of(w)
-        assert zo is not None and k.get("block") is True, "dW goes into the flat view, blockwise"
+        assert zo is not None and into.keywords.get("block") is True, "dW goes into the flat view, blockwise"
         ran["store" if zo.grad_is_fresh(w) else "accum"] += 1
-        return real(w, *a, **k)
+        return real(w, dtype, into, *a, **k)
 
-    linear._fp8_weight_grad = weight_grad
+    linear._weight_grad_sink = weight_grad
     engine = _engine(_llama("blockwise", checkpoint_layers=1), 3, gas=2)
     ids = torch.randint(0, 1024, (2, 256), generator=torch.Generator().manual_seed(1)).cuda()
     before = native.launch_count
@@ -567,7 +568,7 @@ def _blockwise_llama_zero3():
     assert ran["store"] > 0 and ran["accum"] > 0, ran
 
 
-def test_fp8_blockwise_llama_trains_zero3():
+def test_fp8_blockwise_llama_zero3_stores_then_accumulates_dw():
     run_distributed(_blockwise_llama_zero3, 1, ())
 
 

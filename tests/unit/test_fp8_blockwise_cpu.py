@@ -233,21 +233,19 @@ def _train_blockwise_llama(stage):
     import deepspeed_b200 as ds
     from deepspeed_b200.ops import linear
     calls = {"lin": 0, "mlp": 0}
-    real_lin, real_mlp = linear._FP8BlockLinearFn.apply, linear._FP8BlockSwiGLUMLPFn.apply
+    real_lin, real_mlp = linear._FP8LinearFn.apply, linear._FP8SwiGLUMLPFn.apply
 
     def lin(*a):
         calls["lin"] += 1
+        assert a[-1] is True, "a tensorwise node ran under fp8_recipe='blockwise'"
         return real_lin(*a)
 
     def mlp(*a):
         calls["mlp"] += 1
+        assert a[-1] is True, "a tensorwise node ran under fp8_recipe='blockwise'"
         return real_mlp(*a)
 
-    def tensorwise(*a):
-        raise AssertionError("a tensorwise node ran under fp8_recipe='blockwise'")
-
-    linear._FP8BlockLinearFn.apply, linear._FP8BlockSwiGLUMLPFn.apply = lin, mlp
-    linear._FP8LinearFn.apply = linear._FP8SwiGLUMLPFn.apply = tensorwise
+    linear._FP8LinearFn.apply, linear._FP8SwiGLUMLPFn.apply = lin, mlp
     model = _tiny(checkpoint_layers=1)
     cfg = {"train_micro_batch_size_per_gpu": 2, "gradient_accumulation_steps": 2, "bf16": {"enabled": True},
            "optimizer": {"type": "AdamW", "params": {"lr": 3e-3}}, "zero_optimization": {"stage": stage}}
@@ -268,7 +266,7 @@ def _train_blockwise_llama(stage):
 
 
 @pytest.mark.parametrize("stage", [1, 3])
-def test_fp8_blockwise_llama_trains_under_engine(stage):
+def test_fp8_blockwise_llama_trains_block_scaled_under_engine(stage):
     run_distributed(_train_blockwise_llama, 1, (stage, ))
 
 

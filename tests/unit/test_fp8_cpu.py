@@ -160,10 +160,12 @@ def _train_fp8_llama(stage):
 
     def lin(*a):
         calls["lin"] += 1
+        assert a[-1] is False, "a blockwise node ran under the default fp8_recipe='tensorwise'"
         return real_lin(*a)
 
     def mlp(*a):
         calls["mlp"] += 1
+        assert a[-1] is False, "a blockwise node ran under the default fp8_recipe='tensorwise'"
         return real_mlp(*a)
 
     linear._FP8LinearFn.apply, linear._FP8SwiGLUMLPFn.apply = lin, mlp
