@@ -2,7 +2,9 @@
 
 ``causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions)``: rotates Q and K **in place** inside the
 packed projection output (one launch, ``transformer.cu:rope_kernel``), runs the attention core and
-returns ``[B*S, hq*d]``.  The backward produces one packed ``dqkv`` buffer and un-rotates it in place.
+returns ``[B*S, hq*d]``.  The backward produces one packed ``dqkv`` buffer and un-rotates it in place.  One autograd
+node (``_PackedQKVAttention``) owns the rotation for each of the four cores: the in-tree kernel, dense or varlen, and
+SDPA, dense or one call per document.
 
 Attention-core backends (``backend=`` or ``DSB200_ATTN``):
   * ``cudnn`` / ``flash`` / ``efficient`` / ``math`` -- ``torch.nn.functional.scaled_dot_product_attention``
@@ -20,7 +22,7 @@ outside the band; every other case runs SDPA with an explicit boolean band mask 
 (or the longest document) is dropped, so such a call is exactly the unwindowed one.
 QK-norm (``qk_norm=(w_q, w_k, eps)``, Qwen3): every query head is RMS-normalised with its own ``[d]`` weight ``w_q`` and
 every key head with ``w_k`` before RoPE, in the same in-place pass (``transformer.cu:qk_norm_rope_kernel``, see
-``transformer_ops.qk_norm_rope_inplace``); the autograd nodes take the two weights as inputs and return their gradients.
+``transformer_ops.qk_norm_rope_inplace``); the autograd node takes the two weights as inputs and returns their gradients.
 ``qk_norm=None`` runs exactly the calls it ran without the argument.
 Role parity: the reference has no training attention kernel of its own for HF models (it relies on
 PyTorch / flash-attn, ``sequence/fpdt_layer.py:235``); the BERT-era fused layer is ``ops/transformer``.
@@ -31,6 +33,7 @@ import os
 import torch
 import torch.nn.functional as F
 
+from deepspeed_b200.ops.kernels import attention_sm100
 from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_bwd_inplace, qk_norm_rope_inplace, rope_qk_inplace
 
 _ENV = os.environ.get("DSB200_ATTN", "").lower()
@@ -92,63 +95,181 @@ def _sdpa(q, k, v, backend, causal=True, scale=None, window=None):
             return F.scaled_dot_product_attention(q, k, v, **kw)
 
 
-class _PackedCausalAttention(torch.autograd.Function):
+def _heads(x, hq, hkv):
+    """``q, k, v [B, heads, S, d]`` views of ``x [B, S, hq + 2 hkv, d]``."""
+    return x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2), x[:, :, hq + hkv:].transpose(1, 2)
+
+
+def _sdpa_graph(qkv, need_grad, *args, **kw):
+    """:func:`_sdpa` on the views ``qkv = (q, k, v)`` -> ``(out, graph)``.  With ``need_grad`` the call runs on detached
+    leaves under grad mode and ``graph`` keeps the leaves and the output, so :func:`_sdpa_grad` can differentiate this call
+    alone; without it ``graph`` is ``None``.  ``out`` is detached either way."""
+    if not need_grad:
+        return _sdpa(*qkv, *args, **kw), None
+    with torch.enable_grad():
+        leaves = tuple(t.detach().requires_grad_(True) for t in qkv)
+        out = _sdpa(*leaves, *args, **kw)
+    return out.detach(), (leaves, out)
+
+
+def _sdpa_grad(graph, do, y, hq, hkv):
+    """Backward of one :func:`_sdpa_graph` call for the output gradient ``do``, written into ``y``, a
+    ``[B, S, hq + 2 hkv, d]`` view of the packed ``dqkv``."""
+    leaves, out = graph
+    for dst, g in zip(_heads(y, hq, hkv), torch.autograd.grad(out, leaves, do)):
+        dst.copy_(g)
+
+
+# The four attention cores.  Each is built per call and carries ``hq, hkv, d`` and ``seq_len`` (the rotation's position
+# modulus when ``positions`` is None).  ``forward(qkv, need_grad) -> (out [T, hq*d], tensors to save)`` reads the rotated
+# packed buffer; ``backward(dout, saved) -> dqkv`` returns the packed gradient before the un-rotation.
+
+
+class _NativeDense:
+    """The in-tree kernel on ``B`` sequences of ``S`` tokens."""
+
+    def __init__(self, B, S, hq, hkv, d, window):
+        self.B, self.seq_len, self.hq, self.hkv, self.d, self.window = B, S, hq, hkv, d, window
+
+    def forward(self, qkv, need_grad):
+        q, k, v = attention_sm100.split_packed(qkv, self.hq, self.hkv, self.d)
+        o, lse = attention_sm100.fwd(q, k, v, self.B, self.seq_len, self.hq, self.hkv, causal=True, need_lse=need_grad,
+                                     window=self.window, head_dim=self.d)
+        return o, (qkv, o, lse)
+
+    def backward(self, dout, saved):
+        qkv, o, lse = saved
+        B, S, hq, hkv, d = self.B, self.seq_len, self.hq, self.hkv, self.d
+        dqkv = torch.empty_like(qkv)
+        dq, dk, dv = attention_sm100.split_packed(dqkv, hq, hkv, d)
+        attention_sm100.bwd(dout.reshape(B * S, hq * d), *attention_sm100.split_packed(qkv, hq, hkv, d), o, lse, B, S, hq,
+                            hkv, causal=True, dq=dq, dk=dk, dv=dv, window=self.window, head_dim=d)
+        return dqkv
+
+
+class _NativeVarlen:
+    """The in-tree varlen kernel on ``T`` packed rows: documents at the device offsets ``cu_seqlens``, none longer than
+    ``max_seqlen``."""
+
+    def __init__(self, cu_seqlens, max_seqlen, T, hq, hkv, d, window):
+        self.cu_seqlens, self.max_seqlen, self.seq_len = cu_seqlens, max_seqlen, T
+        self.hq, self.hkv, self.d, self.window = hq, hkv, d, window
+
+    def forward(self, qkv, need_grad):
+        q, k, v = attention_sm100.split_packed(qkv, self.hq, self.hkv, self.d)
+        o, lse = attention_sm100.fwd_varlen(q, k, v, self.cu_seqlens, self.max_seqlen, self.hq, self.hkv, causal=True,
+                                            need_lse=need_grad, window=self.window, head_dim=self.d)
+        return o, (qkv, o, lse, self.cu_seqlens)
+
+    def backward(self, dout, saved):
+        qkv, o, lse, cu_seqlens = saved
+        hq, hkv, d = self.hq, self.hkv, self.d
+        dqkv = torch.empty_like(qkv)
+        dq, dk, dv = attention_sm100.split_packed(dqkv, hq, hkv, d)
+        attention_sm100.bwd_varlen(dout.reshape(qkv.shape[0], hq * d), *attention_sm100.split_packed(qkv, hq, hkv, d), o,
+                                   lse, cu_seqlens, self.max_seqlen, hq, hkv, causal=True, dq=dq, dk=dk, dv=dv,
+                                   window=self.window, head_dim=d)
+        return dqkv
+
+
+class _SdpaDense:
+    """SDPA with ``backend`` on ``B`` sequences of ``S`` tokens."""
+
+    def __init__(self, B, S, hq, hkv, d, backend, window):
+        self.B, self.seq_len, self.hq, self.hkv, self.d, self.backend, self.window = B, S, hq, hkv, d, backend, window
+
+    def forward(self, qkv, need_grad):
+        B, S, hq, hkv, d = self.B, self.seq_len, self.hq, self.hkv, self.d
+        self.shape = qkv.shape
+        out, self.graph = _sdpa_graph(_heads(qkv.view(B, S, hq + 2 * hkv, d), hq, hkv), need_grad, self.backend,
+                                      window=self.window)
+        return out.transpose(1, 2).reshape(B * S, hq * d), ()
+
+    def backward(self, dout, saved):
+        B, S, hq, hkv, d = self.B, self.seq_len, self.hq, self.hkv, self.d
+        graph, self.graph = self.graph, None
+        dqkv = torch.empty(self.shape, dtype=dout.dtype, device=dout.device)
+        _sdpa_grad(graph, dout.view(B, S, hq, d).transpose(1, 2), dqkv.view(B, S, hq + 2 * hkv, d), hq, hkv)
+        return dqkv
+
+
+class _SdpaDocs:
+    """One SDPA call with ``backend`` per document of ``T`` packed rows (the portable path and the reference for the
+    varlen kernel); ``spans`` are the host ``(start, end)`` rows of the non-empty documents."""
+
+    def __init__(self, spans, T, hq, hkv, d, backend, causal, window):
+        self.spans, self.seq_len, self.hq, self.hkv, self.d = spans, T, hq, hkv, d
+        self.backend, self.causal, self.window = backend, causal, window
+
+    def forward(self, qkv, need_grad):
+        hq, hkv, d = self.hq, self.hkv, self.d
+        self.shape = qkv.shape
+        out = qkv.new_empty(self.seq_len, hq * d)
+        self.graphs = []
+        for s, e in self.spans:
+            o, graph = _sdpa_graph(_heads(qkv[s:e].view(1, e - s, hq + 2 * hkv, d), hq, hkv), need_grad, self.backend,
+                                   causal=self.causal, window=self.window)
+            out[s:e] = o.transpose(1, 2).reshape(e - s, hq * d)
+            self.graphs.append(graph)
+        return out, ()
+
+    def backward(self, dout, saved):
+        hq, hkv, d = self.hq, self.hkv, self.d
+        graphs, self.graphs = self.graphs, None
+        dqkv = torch.zeros(self.shape, dtype=dout.dtype, device=dout.device)
+        for (s, e), graph in zip(self.spans, graphs):
+            _sdpa_grad(graph, dout[s:e].view(1, e - s, hq, d).transpose(1, 2), dqkv[s:e].view(1, e - s, hq + 2 * hkv, d),
+                       hq, hkv)
+        return dqkv
+
+
+def _rotate(qkv, core, rope, positions, w_q, w_k, eps, need_raw):
+    """QK-norm + RoPE (or RoPE alone, or nothing) in place on the Q and K heads of ``qkv``; returns the pre-norm heads
+    for the backward when ``need_raw`` and QK-norm is on, else ``None``."""
+    if w_q is not None:
+        return qk_norm_rope_inplace(qkv, core.hq, core.hkv, core.d, rope, w_q, w_k, eps, positions, core.seq_len,
+                                    need_raw=need_raw)
+    if rope is not None:
+        rope_qk_inplace(qkv, core.hq, core.hkv, core.d, rope, positions, core.seq_len, backward=False)
+    return None
+
+
+class _PackedQKVAttention(torch.autograd.Function):
+    """Attention on the packed QKV projection output through ``core``: Q and K rotated in place, then the core.  The
+    backward takes the packed ``dqkv`` from the core -- the layout the QKV projection's backward GEMMs consume -- and
+    un-rotates it in place; with QK-norm it also returns the gradients of ``w_q`` and ``w_k``."""
 
     @staticmethod
-    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, backend, window, w_q, w_k, qk_eps):
-        T = B * S
-        raw = None
-        if w_q is not None:
-            raw = qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
-        elif rope is not None:
-            rope_qk_inplace(qkv, hq, hkv, d, rope, positions, S, backward=False)
-        x = qkv.view(B, S, hq + 2 * hkv, d)
-        q = x[:, :, :hq].transpose(1, 2)
-        k = x[:, :, hq:hq + hkv].transpose(1, 2)
-        v = x[:, :, hq + hkv:].transpose(1, 2)
-        with torch.enable_grad():
-            qd, kd, vd = (t.detach().requires_grad_(True) for t in (q, k, v))
-            out = _sdpa(qd, kd, vd, backend, window=window)
-        ctx.graph = (qd, kd, vd, out)
-        ctx.meta = (B, S, hq, hkv, d, rope, positions, qk_eps)
-        ctx.qkv_shape = qkv.shape
-        if w_q is not None:
-            ctx.save_for_backward(raw, w_q, w_k)
-        return out.detach().transpose(1, 2).reshape(T, hq * d)
+    def forward(ctx, qkv, core, rope, positions, w_q, w_k, eps):
+        raw = _rotate(qkv, core, rope, positions, w_q, w_k, eps, need_raw=True)
+        out, saved = core.forward(qkv, need_grad=True)
+        ctx.save_for_backward(*saved, *(() if w_q is None else (raw, w_q, w_k)))
+        ctx.core, ctx.n_core, ctx.rope, ctx.positions, ctx.eps = core, len(saved), rope, positions, eps
+        return out
 
     @staticmethod
     def backward(ctx, dout):
-        B, S, hq, hkv, d, rope, positions, qk_eps = ctx.meta
-        qd, kd, vd, out = ctx.graph
-        ctx.graph = None
-        do = dout.view(B, S, hq, d).transpose(1, 2)
-        dq, dk, dv = torch.autograd.grad(out, (qd, kd, vd), do)
-        dqkv = torch.empty(ctx.qkv_shape, dtype=dout.dtype, device=dout.device)
-        y = dqkv.view(B, S, hq + 2 * hkv, d)
-        y[:, :, :hq].copy_(dq.transpose(1, 2))
-        y[:, :, hq:hq + hkv].copy_(dk.transpose(1, 2))
-        y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
+        core, rope, positions, eps = ctx.core, ctx.rope, ctx.positions, ctx.eps
+        saved = ctx.saved_tensors
+        dqkv = core.backward(dout, saved[:ctx.n_core])
         dw_q = dw_k = None
-        if qk_eps is not None:
-            raw, w_q, w_k = ctx.saved_tensors
-            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
+        if eps is not None:
+            raw, w_q, w_k = saved[ctx.n_core:]
+            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, core.hq, core.hkv, core.d, rope, w_q, w_k, eps, positions,
+                                                  core.seq_len)
         elif rope is not None:
-            rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, S, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, None, dw_q, dw_k, None
+            rope_qk_inplace(dqkv, core.hq, core.hkv, core.d, rope, positions, core.seq_len, backward=True)
+        return dqkv, None, None, None, dw_q, dw_k, None
 
 
-def _qk_norm_grad(qk_norm):
-    """Whether a QK-norm weight needs a gradient (then the autograd node runs even for a ``qkv`` that needs none)."""
-    return qk_norm is not None and (qk_norm[0].requires_grad or qk_norm[1].requires_grad)
-
-
-def _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, seq_len, qk_norm):
-    """The no-grad branches' in-place QK-norm + RoPE (or RoPE alone): nothing is kept for a backward."""
-    if qk_norm is not None:
-        w_q, w_k, eps = qk_norm
-        qk_norm_rope_inplace(qkv2d, hq, hkv, d, rope, w_q, w_k, eps, positions, seq_len, need_raw=False)
-    elif rope is not None:
-        rope_qk_inplace(qkv2d, hq, hkv, d, rope, positions, seq_len, backward=False)
+def _attend(core, qkv2d, rope, positions, qk_norm):
+    """Rotate and attend through ``core``: with the autograd node when grad mode is on and ``qkv2d`` or a QK-norm weight
+    needs a gradient, else keeping nothing for a backward."""
+    w_q, w_k, eps = qk_norm or (None, None, None)
+    if torch.is_grad_enabled() and (qkv2d.requires_grad or (w_q is not None and (w_q.requires_grad or w_k.requires_grad))):
+        return _PackedQKVAttention.apply(qkv2d, core, rope, positions, w_q, w_k, eps)
+    _rotate(qkv2d, core, rope, positions, w_q, w_k, eps, need_raw=False)
+    return core.forward(qkv2d, need_grad=False)[0]
 
 
 _TABLE = None
@@ -213,58 +334,6 @@ def _doc_spans(cu_seqlens, T):
     return [(a, b) for a, b in zip(cu[:-1], cu[1:]) if b > a]
 
 
-def _split_doc(qkv, s, e, hq, hkv, d):
-    x = qkv[s:e].view(1, e - s, hq + 2 * hkv, d)
-    return x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2), x[:, :, hq + hkv:].transpose(1, 2)
-
-
-class _PackedVarlenCausalAttention(torch.autograd.Function):
-    """Packed documents through one SDPA call per document (the portable path and the reference for the varlen kernel):
-    in-place RoPE with per-token positions, packed ``dqkv`` in the backward, un-rotated in place."""
-
-    @staticmethod
-    def forward(ctx, qkv, spans, hq, hkv, d, rope, positions, backend, causal, window, w_q, w_k, qk_eps):
-        T = qkv.shape[0]
-        if w_q is not None:
-            ctx.save_for_backward(qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T), w_q, w_k)
-        elif rope is not None:
-            rope_qk_inplace(qkv, hq, hkv, d, rope, positions, T, backward=False)
-        out = qkv.new_empty(T, hq * d)
-        graphs = []
-        for s, e in spans:
-            parts = _split_doc(qkv, s, e, hq, hkv, d)  # views taken outside grad mode, like _PackedCausalAttention
-            with torch.enable_grad():
-                qd, kd, vd = (t.detach().requires_grad_(True) for t in parts)
-                o = _sdpa(qd, kd, vd, backend, causal=causal, window=window)
-            out[s:e] = o.detach().transpose(1, 2).reshape(e - s, hq * d)
-            graphs.append((s, e, qd, kd, vd, o))
-        ctx.graphs = graphs
-        ctx.meta = (hq, hkv, d, rope, positions, qk_eps)
-        ctx.qkv_shape = qkv.shape
-        return out
-
-    @staticmethod
-    def backward(ctx, dout):
-        hq, hkv, d, rope, positions, qk_eps = ctx.meta
-        graphs, ctx.graphs = ctx.graphs, None
-        T = ctx.qkv_shape[0]
-        dqkv = torch.zeros(ctx.qkv_shape, dtype=dout.dtype, device=dout.device)
-        for s, e, qd, kd, vd, o in graphs:
-            do = dout[s:e].view(1, e - s, hq, d).transpose(1, 2)
-            dq, dk, dv = torch.autograd.grad(o, (qd, kd, vd), do)
-            y = dqkv[s:e].view(1, e - s, hq + 2 * hkv, d)
-            y[:, :, :hq].copy_(dq.transpose(1, 2))
-            y[:, :, hq:hq + hkv].copy_(dk.transpose(1, 2))
-            y[:, :, hq + hkv:].copy_(dv.transpose(1, 2))
-        dw_q = dw_k = None
-        if qk_eps is not None:
-            raw, w_q, w_k = ctx.saved_tensors
-            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T)
-        elif rope is not None:
-            rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, T, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, None, dw_q, dw_k, None
-
-
 def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=None, backend="auto", causal=True,
                           sliding_window=None, qk_norm=None):
     """Per-document SDPA over packed documents (any device / dtype / head dim); ``positions`` and ``qk_norm`` as in
@@ -278,37 +347,20 @@ def varlen_attention_sdpa(qkv2d, cu_seqlens, hq, hkv, d, rope=None, positions=No
         positions = document_positions(cu_seqlens, T)
     if positions is not None:
         positions = positions.reshape(-1).to(device=qkv2d.device, dtype=torch.int32)
-    spans = _doc_spans(cu_seqlens, T)
-    w_q, w_k, qk_eps = qk_norm or (None, None, None)
-    if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
-        return _PackedVarlenCausalAttention.apply(qkv2d, spans, hq, hkv, d, rope, positions, backend, causal, window, w_q,
-                                                  w_k, qk_eps)
-    _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, T, qk_norm)
-    out = qkv2d.new_empty(T, hq * d)
-    for s, e in spans:
-        o = _sdpa(*_split_doc(qkv2d, s, e, hq, hkv, d), backend, causal=causal, window=window)
-        out[s:e] = o.transpose(1, 2).reshape(e - s, hq * d)
-    return out
+    return _attend(_SdpaDocs(_doc_spans(cu_seqlens, T), T, hq, hkv, d, backend, causal, window), qkv2d, rope, positions,
+                   qk_norm)
 
 
 def _varlen_causal_attention(qkv2d, T, hq, hkv, d, rope, positions, backend, cu_seqlens, max_seqlen, window, qk_norm):
     max_seqlen = check_cu_seqlens(cu_seqlens, T, max_seqlen)
     if window is not None and window >= max_seqlen:
         window = None  # no document is longer than the window: exactly the unwindowed call
-    if backend in ("native", "auto") and qkv2d.is_cuda:
-        from deepspeed_b200.ops.kernels import attention_sm100
-        if attention_sm100.supports_varlen(qkv2d, hq, hkv, d):
-            cu = cu_seqlens.to(qkv2d.device, non_blocking=True)
-            if rope is not None:
-                positions = (document_positions(cu, T) if positions is None else positions.reshape(-1).to(
-                    device=qkv2d.device, dtype=torch.int32))
-            if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
-                return attention_sm100.packed_varlen_attention(qkv2d, cu, max_seqlen, hq, hkv, d, rope, positions, window,
-                                                               qk_norm)
-            _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, T, qk_norm)
-            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
-            return attention_sm100.fwd_varlen(q, k, v, cu, max_seqlen, hq, hkv, causal=True, need_lse=False,
-                                              window=window, head_dim=d)[0]
+    if backend in ("native", "auto") and qkv2d.is_cuda and attention_sm100.supports_varlen(qkv2d, hq, hkv, d):
+        cu = cu_seqlens.to(qkv2d.device, non_blocking=True)
+        if rope is not None:
+            positions = (document_positions(cu, T) if positions is None else positions.reshape(-1).to(
+                device=qkv2d.device, dtype=torch.int32))
+        return _attend(_NativeVarlen(cu, max_seqlen, T, hq, hkv, d, window), qkv2d, rope, positions, qk_norm)
     if backend == "native":
         raise RuntimeError("native varlen attention kernel requested but unsupported for this input (needs a CUDA bf16 "
                            "tensor, head dim 64 or 128, 16-byte aligned rows)")
@@ -331,24 +383,12 @@ def causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, backend
     if window is not None and window >= S:
         window = None  # every row sees its whole causal prefix: exactly the unwindowed call
     # `auto` takes the in-tree kernel for a window whenever it can: it skips the tiles outside the band, the fallback masks
-    if backend == "native" or (backend == "auto" and qkv2d.is_cuda and
-                               (window is not None or _native_wins(B, S, hq, hkv, d))):
-        from deepspeed_b200.ops.kernels import attention_sm100
-        if attention_sm100.supports(qkv2d, hq, hkv, d, S):
-            if torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm)):
-                return attention_sm100.packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope, positions, window, qk_norm)
-            _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, S, qk_norm)
-            q, k, v = attention_sm100.split_packed(qkv2d, hq, hkv, d)
-            return attention_sm100.fwd(q, k, v, B, S, hq, hkv, causal=True, need_lse=False, window=window,
-                                       head_dim=d)[0]
+    native = backend == "native" or (backend == "auto" and qkv2d.is_cuda and
+                                     (window is not None or _native_wins(B, S, hq, hkv, d)))
+    if native and not attention_sm100.supports(qkv2d, hq, hkv, d, S):
         if backend == "native":
             raise RuntimeError("native attention kernel requested but unsupported for this shape (needs bf16, head dim 64 "
                                "or 128, sequence length a multiple of 128)")
-    if not (torch.is_grad_enabled() and (qkv2d.requires_grad or _qk_norm_grad(qk_norm))):
-        _rotate_nograd(qkv2d, hq, hkv, d, rope, positions, S, qk_norm)
-        x = qkv2d.view(B, S, hq + 2 * hkv, d)
-        out = _sdpa(x[:, :, :hq].transpose(1, 2), x[:, :, hq:hq + hkv].transpose(1, 2),
-                    x[:, :, hq + hkv:].transpose(1, 2), backend, window=window)
-        return out.transpose(1, 2).reshape(B * S, hq * d)
-    w_q, w_k, qk_eps = qk_norm or (None, None, None)
-    return _PackedCausalAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, backend, window, w_q, w_k, qk_eps)
+        native = False
+    core = _NativeDense(B, S, hq, hkv, d, window) if native else _SdpaDense(B, S, hq, hkv, d, backend, window)
+    return _attend(core, qkv2d, rope, positions, qk_norm)

@@ -9,9 +9,6 @@ only when ``i - window < j <= i`` (``window`` keys counting its own; flash-attn'
 inside each document for the varlen forms.  The kernels skip the key / query blocks outside the band, so the cost is
 O(S * window) instead of O(S^2).
 
-``qk_norm`` (:func:`packed_causal_attention`, :func:`packed_varlen_attention`; default ``None``): ``(w_q, w_k, eps)``, the
-per-head RMSNorm of Q and K fused with RoPE (``ops.attention``); the nodes return the two weights' gradients.
-
 ``head_dim`` (every entry point, default 128): 64 or 128.  It sizes the outputs and sets the default softmax scale
 ``1 / sqrt(head_dim)``.
 """
@@ -154,96 +151,3 @@ def bwd_varlen(d_o, q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=Tru
     N.check(rc, "attn_varlen_bwd_bf16")
     return dq, dk, dv
 
-
-class _PackedAttention(torch.autograd.Function):
-    """Causal GQA attention on the packed QKV projection output (RoPE applied in place first): the backward leaves
-    dQ | dK | dV in ONE packed buffer -- exactly the layout the QKV projection's backward GEMMs consume."""
-
-    @staticmethod
-    def forward(ctx, qkv, B, S, hq, hkv, d, rope, positions, window, w_q, w_k, qk_eps):
-        from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_inplace, rope_qk_inplace
-        if w_q is not None:
-            raw = qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
-        elif rope is not None:
-            rope_qk_inplace(qkv, hq, hkv, d, rope, positions, S, backward=False)
-        q, k, v = split_packed(qkv, hq, hkv, d)
-        o, lse = fwd(q, k, v, B, S, hq, hkv, causal=True, window=window, head_dim=d)
-        if w_q is not None:
-            ctx.save_for_backward(qkv, o, lse, raw, w_q, w_k)
-        else:
-            ctx.save_for_backward(qkv, o, lse)
-        ctx.meta = (B, S, hq, hkv, d, rope, positions, window, qk_eps)
-        return o
-
-    @staticmethod
-    def backward(ctx, d_o):
-        from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_bwd_inplace, rope_qk_inplace
-        qkv, o, lse = ctx.saved_tensors[:3]
-        B, S, hq, hkv, d, rope, positions, window, qk_eps = ctx.meta
-        q, k, v = split_packed(qkv, hq, hkv, d)
-        dqkv = torch.empty_like(qkv)
-        dq, dk, dv = split_packed(dqkv, hq, hkv, d)
-        bwd(d_o.reshape(B * S, hq * d), q, k, v, o, lse, B, S, hq, hkv, causal=True, dq=dq, dk=dk, dv=dv, window=window,
-            head_dim=d)
-        dw_q = dw_k = None
-        if qk_eps is not None:
-            raw, w_q, w_k = ctx.saved_tensors[3:]
-            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, S)
-        elif rope is not None:
-            rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, S, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, dw_q, dw_k, None
-
-
-def packed_causal_attention(qkv2d, B, S, hq, hkv, d, rope=None, positions=None, window=None, qk_norm=None):
-    assert d in HEAD_DIMS
-    w_q, w_k, qk_eps = qk_norm or (None, None, None)
-    return _PackedAttention.apply(qkv2d, B, S, hq, hkv, d, rope, positions, window, w_q, w_k, qk_eps)
-
-
-class _PackedVarlenAttention(torch.autograd.Function):
-    """:class:`_PackedAttention` over packed documents: ``positions`` (int32 ``[T]``, restarting per document) drive the
-    in-place RoPE, ``cu_seqlens`` / ``max_seqlen`` the document masking."""
-
-    @staticmethod
-    def forward(ctx, qkv, cu_seqlens, max_seqlen, hq, hkv, d, rope, positions, window, w_q, w_k, qk_eps):
-        from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_inplace, rope_qk_inplace
-        T = qkv.shape[0]
-        if w_q is not None:
-            raw = qk_norm_rope_inplace(qkv, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T)
-        elif rope is not None:
-            rope_qk_inplace(qkv, hq, hkv, d, rope, positions, T, backward=False)
-        q, k, v = split_packed(qkv, hq, hkv, d)
-        o, lse = fwd_varlen(q, k, v, cu_seqlens, max_seqlen, hq, hkv, causal=True, window=window, head_dim=d)
-        if w_q is not None:
-            ctx.save_for_backward(qkv, o, lse, cu_seqlens, raw, w_q, w_k)
-        else:
-            ctx.save_for_backward(qkv, o, lse, cu_seqlens)
-        ctx.meta = (max_seqlen, hq, hkv, d, rope, positions, window, qk_eps)
-        return o
-
-    @staticmethod
-    def backward(ctx, d_o):
-        from deepspeed_b200.ops.kernels.transformer_ops import qk_norm_rope_bwd_inplace, rope_qk_inplace
-        qkv, o, lse, cu_seqlens = ctx.saved_tensors[:4]
-        max_seqlen, hq, hkv, d, rope, positions, window, qk_eps = ctx.meta
-        T = qkv.shape[0]
-        q, k, v = split_packed(qkv, hq, hkv, d)
-        dqkv = torch.empty_like(qkv)
-        dq, dk, dv = split_packed(dqkv, hq, hkv, d)
-        bwd_varlen(d_o.reshape(T, hq * d), q, k, v, o, lse, cu_seqlens, max_seqlen, hq, hkv, causal=True, dq=dq, dk=dk,
-                   dv=dv, window=window, head_dim=d)
-        dw_q = dw_k = None
-        if qk_eps is not None:
-            raw, w_q, w_k = ctx.saved_tensors[4:]
-            dw_q, dw_k = qk_norm_rope_bwd_inplace(dqkv, raw, hq, hkv, d, rope, w_q, w_k, qk_eps, positions, T)
-        elif rope is not None:
-            rope_qk_inplace(dqkv, hq, hkv, d, rope, positions, T, backward=True)
-        return dqkv, None, None, None, None, None, None, None, None, dw_q, dw_k, None
-
-
-def packed_varlen_attention(qkv2d, cu_seqlens, max_seqlen, hq, hkv, d, rope=None, positions=None, window=None,
-                            qk_norm=None):
-    assert d in HEAD_DIMS
-    w_q, w_k, qk_eps = qk_norm or (None, None, None)
-    return _PackedVarlenAttention.apply(qkv2d, cu_seqlens, max_seqlen, hq, hkv, d, rope, positions, window, w_q, w_k,
-                                        qk_eps)

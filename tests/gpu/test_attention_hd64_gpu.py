@@ -309,12 +309,12 @@ def test_public_op_native_matches_sdpa(kind):
 
 # ---- 6. routing ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("kind,native", [("dense", False), ("packed", True), ("window", True), ("packed_window", True)])
-def test_auto_routing_at_head_dim_64(monkeypatch, kind, native):
-    """``auto`` takes the native kernels for packed and windowed inputs; a dense unwindowed input stays on SDPA (no
-    measured table entry selects the native kernel for it)."""
+def test_auto_routing_at_head_dim_64_calls_kernel_entry_points(monkeypatch, kind, native):
+    """``auto`` takes the native kernels (``fwd`` / ``fwd_varlen``) for packed and windowed inputs; a dense unwindowed
+    input stays on SDPA (no measured table entry selects the native kernel for it)."""
     A = _A()
     calls = []
-    for name in ("packed_causal_attention", "packed_varlen_attention"):
+    for name in ("fwd", "fwd_varlen"):
         fn = getattr(A, name)
         monkeypatch.setattr(A, name, lambda *a, _fn=fn, _n=name, **k: (calls.append(_n), _fn(*a, **k))[1])
     hq, hkv, B, S = 4, 2, 2, 256
