@@ -879,6 +879,116 @@ fused_add_kernel(const T* __restrict__ a, const T* __restrict__ b, const T* __re
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Embedding backward into a gradient buffer: out[v, :] += sum of dy[t, :] over the tokens t with ids[t] == v, with no
+// atomics and bit-reproducible.  `sid` / `order` are the stable sort of the ids (values, permutation), so one id's
+// tokens form a run of sorted positions (a segment) in token order.  The positions are cut into blocks of kEmbChunk; a
+// chunk is the part of a segment inside one block, so position p starts a chunk iff it starts a segment or a block, which
+// sid[p - 1] and sid[p] decide.  One lane takes one chunk and 8 columns:
+//   pass 1: a chunk that is a whole segment sums its rows in fp32 in token order, reads the out row once, adds and rounds
+//           once.  A chunk whose segment continues past its block writes its fp32 sum to part[block]; the last chunk of
+//           such a segment is left to pass 2.
+//   pass 2: one lane per block whose first position continues a segment that ends in it: the segment's partials in block
+//           order, then its own rows, then the out row.
+// The grid is sized by the token count (no host sync on the number of ids); a hot id costs at most kEmbChunk rows per
+// lane.  Rows whose id does not occur are neither read nor written.
+// ------------------------------------------------------------------------------------------------
+constexpr int kEmbChunk = 64;
+
+template <typename T>
+__device__ __forceinline__ void ld8(const T* p, float* f)  // 8 elements, 16-byte aligned
+{
+    constexpr int kPer = Elem<T>::kPerVec;
+#pragma unroll
+    for (int k = 0; k < 8 / kPer; ++k) Elem<T>::unpack(ld_plain(p + k * kPer), f + k * kPer);
+}
+
+template <typename T>
+__device__ __forceinline__ void st8(T* p, const float* f)
+{
+    constexpr int kPer = Elem<T>::kPerVec;
+#pragma unroll
+    for (int k = 0; k < 8 / kPer; ++k) st_plain(p + k * kPer, Elem<T>::pack(f + k * kPer));
+}
+
+// acc += dy rows order[q], q in [a, e), in that order
+template <typename TI>
+__device__ __forceinline__ void emb_sum_rows(const TI* __restrict__ dy, const int64_t* __restrict__ order, int64_t a,
+                                             int64_t e, int H, int64_t col, float* acc)
+{
+#pragma unroll 4
+    for (int64_t q = a; q < e; ++q) {
+        float f[8];
+        Elem<TI>::unpack(ld_stream(dy + order[q] * H + col), f);
+        if constexpr (Elem<TI>::kPerVec == 4) Elem<TI>::unpack(ld_stream(dy + order[q] * H + col + 4), f + 4);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] += f[k];
+    }
+}
+
+template <typename TO>
+__device__ __forceinline__ void emb_add_row(TO* __restrict__ out, int64_t v, int H, int64_t col, const float* acc)
+{
+    float o[8];
+    ld8(out + v * H + col, o);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[k] += acc[k];
+    st8(out + v * H + col, o);
+}
+
+template <typename TI, typename TO>
+__global__ void __launch_bounds__(256)
+embedding_bwd_kernel(const TI* __restrict__ dy, const int64_t* __restrict__ sid, const int64_t* __restrict__ order,
+                     float* __restrict__ part, TO* __restrict__ out, int64_t T, int H)
+{
+    const int64_t p = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int64_t col = (static_cast<int64_t>(blockIdx.y) * 32 + (threadIdx.x & 31)) * 8;
+    if (p >= T || col >= H) return;
+    const int64_t v = sid[p];
+    const bool seg_start = p == 0 || sid[p - 1] != v;
+    if (!seg_start && p % kEmbChunk != 0) return;
+    const int64_t block_end = min(T, (p / kEmbChunk + 1) * kEmbChunk);
+    int64_t e = p + 1;
+    while (e < block_end && sid[e] == v) ++e;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (e == block_end && e < T && sid[e] == v) {  // the segment continues in the next block
+        emb_sum_rows(dy, order, p, e, H, col, acc);
+        st8(part + (p / kEmbChunk) * H + col, acc);
+        return;
+    }
+    if (!seg_start) return;  // the last chunk of a segment spanning blocks: pass 2
+    emb_sum_rows(dy, order, p, e, H, col, acc);
+    emb_add_row(out, v, H, col, acc);
+}
+
+template <typename TI, typename TO>
+__global__ void __launch_bounds__(256)
+embedding_bwd_tail_kernel(const TI* __restrict__ dy, const int64_t* __restrict__ sid, const int64_t* __restrict__ order,
+                          const float* __restrict__ part, TO* __restrict__ out, int64_t T, int H)
+{
+    const int64_t b = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    const int64_t col = (static_cast<int64_t>(blockIdx.y) * 32 + (threadIdx.x & 31)) * 8;
+    const int64_t p = b * kEmbChunk;
+    if (p == 0 || p >= T || col >= H) return;
+    const int64_t v = sid[p];
+    if (sid[p - 1] != v) return;  // p starts a segment: pass 1 took it
+    const int64_t block_end = min(T, p + kEmbChunk);
+    if (block_end < T && sid[block_end] == v) return;  // not the segment's last chunk
+    int64_t b0 = b - 1;  // the block the segment starts in
+    while (b0 > 0 && sid[b0 * kEmbChunk - 1] == v) --b0;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int64_t k = b0; k < b; ++k) {
+        float f[8];
+        ld8(part + k * H + col, f);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[j] += f[j];
+    }
+    int64_t e = p + 1;
+    while (e < block_end && sid[e] == v) ++e;
+    emb_sum_rows(dy, order, p, e, H, col, acc);
+    emb_add_row(out, v, H, col, acc);
+}
+
 }  // namespace dsb
 
 using namespace dsb;
@@ -1204,6 +1314,34 @@ DSB_EXPORT int dsb_fused_add(const void* a, const void* b, const void* c, const 
     DISPATCH_T(dtype, T, {
         fused_add_kernel<T>
             <<<grid, 256, 0, stream>>>((const T*)a, (const T*)b, (const T*)c, (const T*)d, (T*)y, n, scale);
+    })
+    DSB_CHECK_LAUNCH();
+    return 0;
+}
+
+// Rows of the fp32 scratch dsb_embedding_bwd needs ([rows, hidden]).
+DSB_EXPORT int dsb_embedding_bwd_part_rows(int64_t tokens) { return static_cast<int>(ceil_div(tokens, kEmbChunk)); }
+
+// out[v, :] += sum of dy[t, :] over the tokens with ids[t] == v (see embedding_bwd_kernel).  dy [tokens, hidden] in
+// `dtype`, sid / order int64 [tokens]: the stable sort of the ids (values, permutation), out [vocab, hidden] in
+// `out_dtype`, part fp32 [dsb_embedding_bwd_part_rows(tokens), hidden].  -2: hidden not a multiple of 8 or a buffer
+// not 16-byte aligned.
+DSB_EXPORT int dsb_embedding_bwd(const void* dy, const int64_t* sid, const int64_t* order, float* part, void* out,
+                                 int64_t tokens, int hidden, int dtype, int out_dtype, cudaStream_t stream)
+{
+    if (hidden % 8 != 0 || ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(out) |
+                             reinterpret_cast<uintptr_t>(part)) & 15) != 0)
+        return -2;
+    if (tokens <= 0 || hidden <= 0) return 0;
+    const dim3 grid1(static_cast<unsigned>(ceil_div(tokens, 8)), static_cast<unsigned>(ceil_div(hidden, 256)));
+    const dim3 grid2(static_cast<unsigned>(ceil_div(dsb_embedding_bwd_part_rows(tokens), 8)), grid1.y);
+    DISPATCH_T(dtype, TI, {
+        DISPATCH_T(out_dtype, TO, {
+            embedding_bwd_kernel<TI, TO>
+                <<<grid1, 256, 0, stream>>>((const TI*)dy, sid, order, part, (TO*)out, tokens, hidden);
+            embedding_bwd_tail_kernel<TI, TO>
+                <<<grid2, 256, 0, stream>>>((const TI*)dy, sid, order, part, (TO*)out, tokens, hidden);
+        })
     })
     DSB_CHECK_LAUNCH();
     return 0;

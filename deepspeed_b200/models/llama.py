@@ -179,12 +179,30 @@ class LMHead(FlatLinear):
     the ZeRO-3 fetch hooks in the loop; its backward needs no weights (dW/dh are produced in forward)."""
     ds_skip_backward_fetch = True
 
+    def __init__(self, in_features, out_features, defer_ready=False):
+        super().__init__(in_features, out_features)
+        # the weight is tied to the input embedding, whose backward comes later and marks it ready (see TiedEmbedding)
+        self.defer_ready = defer_ready
+
     def forward(self, h, labels=None, chunk=2048, assumed_scale=1.0):
         if labels is None:
             return flat_linear(h, self.weight, self.bias)
         from deepspeed_b200.ops.linear import chunked_linear_xent
+        if self.defer_ready:
+            return chunked_linear_xent(h.reshape(-1, h.shape[-1]), self.weight, labels.reshape(-1), chunk=chunk,
+                                       assumed_scale=assumed_scale, defer_ready=True)
         return chunked_linear_xent(h.reshape(-1, h.shape[-1]), self.weight, labels.reshape(-1), chunk=chunk,
                                    assumed_scale=assumed_scale)
+
+
+class TiedEmbedding(nn.Embedding):
+    """The input embedding of a model whose LM head shares its weight.  Under ZeRO the head's dW sits in the weight's
+    flat gradient view first; this module's backward adds the embedding gradient into the same view with the
+    deterministic native kernel and marks the weight ready, once per backward (:func:`ops.linear.embedding`)."""
+
+    def forward(self, input_ids):
+        from deepspeed_b200.ops.linear import embedding
+        return embedding(input_ids, self.weight)
 
 
 class LlamaAttention(nn.Module):
@@ -267,7 +285,7 @@ class LlamaModel(nn.Module):
     def __init__(self, cfg: LlamaConfig):
         super().__init__()
         self.cfg = cfg
-        self.embed_tokens = nn.Embedding(cfg.vocab_size, cfg.hidden_size)
+        self.embed_tokens = (TiedEmbedding if cfg.tie_word_embeddings else nn.Embedding)(cfg.vocab_size, cfg.hidden_size)
         self.embed_tokens.ds_skip_backward_fetch = True  # embedding backward is an index-add: no weights needed
         self.layers = nn.ModuleList([LlamaDecoderLayer(cfg, i) for i in range(cfg.num_hidden_layers)])
         self.norm = RMSNorm(cfg.hidden_size, cfg.rms_norm_eps)
@@ -333,7 +351,7 @@ class LlamaForCausalLM(nn.Module):
         super().__init__()
         self.cfg = cfg
         self.model = LlamaModel(cfg)
-        self.lm_head = LMHead(cfg.hidden_size, cfg.vocab_size)
+        self.lm_head = LMHead(cfg.hidden_size, cfg.vocab_size, defer_ready=cfg.tie_word_embeddings)
         if cfg.tie_word_embeddings:
             self.lm_head.weight = self.model.embed_tokens.weight
         self.ds_loss_multiplier = 1.0  # set by the engine: loss_scale / grad_accum_steps
@@ -366,7 +384,8 @@ class LlamaForCausalLM(nn.Module):
     # ---- HF checkpoint interop ---------------------------------------------------------------------
     @staticmethod
     def convert_hf_state_dict(sd, cfg: LlamaConfig):
-        """Pack HF ``q_proj/k_proj/v_proj`` and ``gate_proj/up_proj`` into this model's layout."""
+        """Pack HF ``q_proj/k_proj/v_proj`` and ``gate_proj/up_proj`` into this model's layout.  A tied model's
+        ``lm_head.weight``, which HF checkpoint files omit, is the embedding's."""
         out = {}
         for k, v in sd.items():
             if ".self_attn.q_proj." in k:
@@ -384,6 +403,8 @@ class LlamaForCausalLM(nn.Module):
                 continue
             else:
                 out[k] = v
+        if cfg.tie_word_embeddings and "lm_head.weight" not in out and "model.embed_tokens.weight" in out:
+            out["lm_head.weight"] = out["model.embed_tokens.weight"]
         return out
 
     @torch.no_grad()

@@ -336,6 +336,47 @@ def _qk_norm_rope_bwd_torch(heads, raw, n_q, table, w_q, w_k, eps, positions, se
 
 
 # ---------------------------------------------------------------------------------------------------
+# embedding backward
+# ---------------------------------------------------------------------------------------------------
+def embedding_bwd_(dy, ids, out):
+    """``out[v] += sum of dy[t] over the tokens t with ids[t] == v``, **in place** on ``out [V, H]``; returns ``out``.
+    ``dy`` is ``[..., H]`` with one row per id.  Deterministic: each id's rows are summed in fp32 in token order, added to
+    the out row and rounded to ``out``'s dtype once.  Rows whose id does not occur are not read or written, so ``out``
+    may already hold another contribution (a tied LM head's dW).
+
+    CUDA bf16 / fp16 / fp32 operands with ``H % 8 == 0`` and 16-byte aligned buffers run ``transformer.cu``'s
+    ``embedding_bwd_kernel`` (ids sorted on the device, no host sync); anything else runs :func:`_embedding_bwd_torch`."""
+    H = out.shape[-1]
+    dy2 = dy.reshape(-1, H)
+    ids1 = ids.reshape(-1)
+    floats = (torch.bfloat16, torch.float16, torch.float32)
+    if dy2.is_cuda and out.is_cuda and out.is_contiguous() and dy2.dtype in floats and out.dtype in floats:
+        dy2 = dy2.contiguous()
+        sid, order = torch.sort(ids1.long(), stable=True)
+        lib = N.cuda()
+        part = torch.empty(lib.dsb_embedding_bwd_part_rows(N.c_i64(ids1.numel())), H, dtype=torch.float32,
+                           device=out.device)
+        rc = lib.dsb_embedding_bwd(_p(dy2), _p(sid), _p(order), _p(part), _p(out), N.c_i64(ids1.numel()), H, N.dt(dy2),
+                                   N.dt(out), N.stream())
+        if rc != -2:
+            N.check(rc, "embedding_bwd")
+            return out
+    return _embedding_bwd_torch(dy2, ids1, out)
+
+
+def _embedding_bwd_torch(dy2, ids1, out):
+    """The torch form of :func:`embedding_bwd_` with the same semantics: an fp32 ``index_add_`` over the rows in sorted
+    (stable, so token) order, one rounding per touched row."""
+    sid, order = torch.sort(ids1.long(), stable=True)
+    uniq, seg = torch.unique_consecutive(sid, return_inverse=True)
+    acc = torch.zeros(uniq.numel(), out.shape[-1], dtype=torch.float32, device=out.device)
+    acc.index_add_(0, seg.to(out.device), dy2[order].float().to(out.device))
+    uniq = uniq.to(out.device)
+    out[uniq] = (out[uniq].float() + acc).to(out.dtype)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------
 # gated activation (SwiGLU & friends)
 # ---------------------------------------------------------------------------------------------------
 def gated_act_fwd_raw(gu, act=ACT_SILU, out=None):

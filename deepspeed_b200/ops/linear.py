@@ -8,6 +8,8 @@
 * :func:`chunked_linear_xent` -- LM head + softmax cross-entropy over token chunks; logits gradient is
   produced in place by the fused kernel, ``dh`` and ``dW`` are accumulated per chunk, so the
   ``[tokens, vocab]`` logits tensor is never materialised (role: reference ``FPDT_LogitsLoss``).
+* :func:`embedding` -- the input embedding of a model with a tied LM head: its backward adds into the flat gradient
+  view the head's dW already sits in, with the deterministic native embedding backward, and marks the weight ready.
 """
 import functools
 
@@ -573,7 +575,7 @@ def fp8_ragged_swiglu_mlp(x, offsets, w13, w2, recipe="tensorwise"):
 class _ChunkedLinearXent(torch.autograd.Function):
 
     @staticmethod
-    def forward(ctx, h, weight, labels, chunk, ignore_index, assumed_scale):
+    def forward(ctx, h, weight, labels, chunk, ignore_index, assumed_scale, defer_ready):
         from deepspeed_b200.ops import gemm
         T, H = h.shape
         n_valid = xent_valid(labels, weight.shape[0], ignore_index).sum().clamp(min=1).to(torch.float32)
@@ -612,6 +614,7 @@ class _ChunkedLinearXent(torch.autograd.Function):
         ctx.dh = dh
         ctx.dw_tmp = dw_tmp
         ctx.direct = direct
+        ctx.defer_ready = defer_ready
         return total / n_valid
 
     @staticmethod
@@ -630,7 +633,7 @@ class _ChunkedLinearXent(torch.autograd.Function):
                 from deepspeed_b200.ops.kernels import flat_ops
                 flat = ctx.dw_tmp.view(-1)
                 flat_ops.scale_cast(flat, flat, scale=1.0, d_scale=r.reshape(1))
-                zo.mark_grad_ready(w)
+                _mark_or_note(zo, w, ctx.defer_ready)
             elif zo is not None:
                 gv = zo.grad_view_for(w)
                 if zo.grad_is_fresh(w):
@@ -638,16 +641,27 @@ class _ChunkedLinearXent(torch.autograd.Function):
                         ctx.dw_tmp.float() * r)
                 else:
                     gv.add_((ctx.dw_tmp.float() * r).to(gv.dtype))
-                zo.mark_grad_ready(w)
+                _mark_or_note(zo, w, ctx.defer_ready)
             else:
                 dw = ctx.dw_tmp * r.to(ctx.dw_tmp.dtype)
         ctx.dh = None
         ctx.dw_tmp = None
-        return dh, dw, None, None, None, None
+        return dh, dw, None, None, None, None, None
 
 
-def chunked_linear_xent(h, weight, labels, chunk=2048, ignore_index=-100, assumed_scale=1.0):
-    """Mean cross entropy of ``softmax(h W^T)`` vs ``labels`` without materialising the logits."""
+def _mark_or_note(zo, w, defer_ready):
+    """``w``'s gradient view holds this node's contribution: mark ``w`` ready, or with ``defer_ready`` only note the
+    write, so that a later producer of the same weight accumulates and marks it."""
+    if defer_ready:
+        zo.note_grad_written(w)
+    else:
+        zo.mark_grad_ready(w)
+
+
+def chunked_linear_xent(h, weight, labels, chunk=2048, ignore_index=-100, assumed_scale=1.0, defer_ready=False):
+    """Mean cross entropy of ``softmax(h W^T)`` vs ``labels`` without materialising the logits.  ``defer_ready``: the
+    weight has another producer whose backward runs later (a tied input embedding, see :func:`embedding`), which marks
+    it ready; this node's dW is left in the ZeRO gradient view for it to accumulate onto."""
     if not torch.is_grad_enabled():
         total = torch.zeros((), dtype=torch.float32, device=h.device)
         n = xent_valid(labels, weight.shape[0], ignore_index).sum().clamp(min=1)
@@ -657,4 +671,40 @@ def chunked_linear_xent(h, weight, labels, chunk=2048, ignore_index=-100, assume
             rows, _ = softmax_xent_fwd_bwd(logits, labels[s:e].contiguous(), 1.0, None, ignore_index, False)
             total = total + rows.sum()
         return total / n
-    return _ChunkedLinearXent.apply(h, weight, labels, chunk, ignore_index, float(assumed_scale) or 1.0)
+    return _ChunkedLinearXent.apply(h, weight, labels, chunk, ignore_index, float(assumed_scale) or 1.0, defer_ready)
+
+
+class _EmbeddingFn(torch.autograd.Function):
+    """``weight[ids]`` whose backward adds the weight gradient straight into the ZeRO flat gradient view with the
+    deterministic embedding backward (:func:`transformer_ops.embedding_bwd_`): only the rows of ids that occur are
+    touched, so a tied LM head's dW may already sit in the view (stored there on a fresh view, which is zeroed first),
+    and the weight is marked ready once both have landed.  Without an owner the gradient is a zero ``[V, H]`` tensor
+    accumulated into and returned to autograd.  Backward reads no weight."""
+
+    @staticmethod
+    def forward(ctx, ids, weight):
+        ctx.save_for_backward(ids)
+        ctx.weight_ref = weight
+        return F.embedding(ids, weight)
+
+    @staticmethod
+    def backward(ctx, dy):
+        from deepspeed_b200.ops.kernels.transformer_ops import embedding_bwd_
+        (ids, ) = ctx.saved_tensors
+        w = ctx.weight_ref
+        zo = _zo_of(w)
+        if zo is None:
+            return None, embedding_bwd_(dy, ids, torch.zeros(w.shape, dtype=w.dtype, device=dy.device))
+        gv = zo.grad_view_for(w)
+        if zo.grad_is_fresh(w):
+            gv.zero_()
+        embedding_bwd_(dy, ids, gv)
+        zo.mark_grad_ready(w)
+        return None, None
+
+
+def embedding(ids, weight):
+    """``F.embedding(ids, weight)`` whose weight gradient goes through :class:`_EmbeddingFn`."""
+    if not torch.is_grad_enabled() or not weight.requires_grad:
+        return F.embedding(ids, weight)
+    return _EmbeddingFn.apply(ids, weight)

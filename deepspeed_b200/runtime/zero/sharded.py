@@ -161,12 +161,14 @@ class _UnitRT:
         self.dense_grads = False  # set by model integrations that write every gradient view
         self.temp_refs = 0  # GatheredParameters / external users holding the unit
         self.home = None  # buffer used by this iteration's forward gather (backward MUST reuse it)
+        self.borrow_home = None  # ... and by the forward gather for a module sharing the unit's weight
         self.running = 0  # forward passes of the unit's module currently executing (re-entrancy counter)
         self.unsynced = None  # local gradient parked by backward passes under engine.no_sync()
         self.fwd_calls = 0  # grad-enabled forward invocations of the module since the last backward finished
         self.bwd_calls = 0  # ... and how many of them have been back-propagated
         self.consumed = False  # a module hook actually used the gathered copy (vs. a speculative prefetch)
         self.skip_bwd_fetch = False  # module's backward does not read its weights (embedding, fused LM head)
+        self.own_grad_slot: Optional[_Slot] = None  # units with borrowers: a gradient buffer outside the pool
 
 
 class ZeroShardedOptimizer(ZeROOptimizer):
@@ -348,6 +350,7 @@ class ZeroShardedOptimizer(ZeROOptimizer):
         self.stats = flat_ops.GradStats(self.device if not self.offload_optimizer else "cpu")
         self._dev_stats = flat_ops.GradStats(self.device) if self.offload_optimizer else self.stats
         self._trace: List[int] = []
+        self._borrow_pos = set()  # positions in _trace that are borrows (fetches for a module sharing the unit's weight)
         self._trace_done = False
         self._order_pos: Dict[int, int] = {}
         self._in_backward = False
@@ -489,6 +492,12 @@ class ZeroShardedOptimizer(ZeROOptimizer):
             self.param_pool = []
             self.lp_arena = None  # shards are views of full_arena
         self.grad_pool = [_Slot(self._symm_or_empty(self.max_full, self.comm_dtype)) for _ in range(2)]
+        for rt in self.rts:
+            if rt.u.borrowers:
+                # a tied LM head writes its dW into the shared weight's gradient view in forward and the embedding's
+                # backward adds to it at the very end: held through the whole backward, the view gets a buffer of its
+                # own rather than one of the two the other units take turns on
+                rt.own_grad_slot = _Slot(self._symm_or_empty(rt.u.full_numel, self.comm_dtype))
         self._rs_tmp = [self._empty(max(u.shard_numel for u in self.units), self.comm_dtype) for _ in range(2)] \
             if self.shard_world > 1 else []
 
@@ -642,6 +651,9 @@ class ZeroShardedOptimizer(ZeROOptimizer):
                 self._tag_param(rt, s)
                 if p.requires_grad:
                     self._hook_handles.append(p.register_post_accumulate_grad_hook(self._make_grad_hook(rt, s)))
+            if self.transient and not rt.u.persistent:
+                for _, b in rt.u.borrowers:
+                    self._hook_borrower(rt, b)
             m = rt.u.module
             if m is None or not self.transient or rt.u.persistent:
                 continue
@@ -652,6 +664,34 @@ class ZeroShardedOptimizer(ZeROOptimizer):
                 self._hook_handles.append(m.register_full_backward_pre_hook(self._make_pre_bwd(rt)))
                 if bool(getattr(self.zc, "b200_multi_forward", True)):
                     self._hook_handles.append(m.register_full_backward_hook(self._make_post_bwd(rt)))
+
+    def _hook_borrower(self, rt, m):
+        """ZeRO-3 hooks on a module outside unit ``rt`` that uses one of its parameters (a tied LM head): gather the unit
+        for the module's forward and release it after; the same around its backward unless the module is
+        ``ds_skip_backward_fetch`` (its backward reads no weight).  The forward fetch is recorded in the trace as a borrow,
+        so once the order is known the unit is prefetched ahead of the borrower like any other unit."""
+
+        def pre_fwd(module, args):
+            self.fetch_unit(rt, forward=not self._in_backward, borrow=True)
+            rt.running += 1
+
+        def post_fwd(module, args, output):
+            rt.running = max(0, rt.running - 1)
+            if not self._in_backward and rt.running == 0:
+                self.release_unit(rt)
+
+        def pre_bwd(module, grad_output):
+            self._in_backward = True
+            self.fetch_unit(rt, forward=False, borrow=True)
+
+        def post_bwd(module, grad_input, grad_output):
+            self.release_unit(rt)
+
+        self._hook_handles.append(m.register_forward_pre_hook(pre_fwd))
+        self._hook_handles.append(m.register_forward_hook(post_fwd))
+        if not getattr(m, "ds_skip_backward_fetch", False):
+            self._hook_handles.append(m.register_full_backward_pre_hook(pre_bwd))
+            self._hook_handles.append(m.register_full_backward_hook(post_bwd))
 
     def _tag_param(self, rt, s):
         """Reference-style per-parameter introspection attributes (``partition_parameters.py:1111``): ``ds_id``,
@@ -727,7 +767,8 @@ class ZeroShardedOptimizer(ZeROOptimizer):
 
     def _last_forward_unit(self):
         if self._trace_done and self._trace:
-            return self._trace[-1]
+            return next((u for i, u in reversed(list(enumerate(self._trace))) if i not in self._borrow_pos),
+                        self.units[-1].index)
         return self.units[-1].index
 
     def _make_grad_hook(self, rt, slot):
@@ -758,7 +799,7 @@ class ZeroShardedOptimizer(ZeROOptimizer):
         if rt.grad_full is not None:
             return
         # round-robin over the pool; wait until the previous reduce that used the slot is done
-        slot = self.grad_pool[rt.u.index % len(self.grad_pool)]
+        slot = rt.own_grad_slot or self.grad_pool[rt.u.index % len(self.grad_pool)]
         if slot.owner is not None and slot.owner is not rt and slot.owner.grad_full is not None:
             # previous owner still accumulating (out-of-order graph): fall back to a private buffer
             slot = _Slot(torch.empty(self.max_full, dtype=self.comm_dtype, device=self.device))
@@ -792,6 +833,13 @@ class ZeroShardedOptimizer(ZeROOptimizer):
     def grad_is_fresh(self, p: nn.Parameter) -> bool:
         return not getattr(self.slot_of_param[id(p)], "_written", False)
 
+    def note_grad_written(self, p: nn.Parameter):
+        """Public: ``p``'s gradient view holds a contribution of this micro step, but ``p`` has another producer still
+        to come (a tied LM head before the embedding's backward): the next producer accumulates instead of storing,
+        and its :meth:`mark_grad_ready` is the one readiness event."""
+        self._in_backward = True
+        self.slot_of_param[id(p)]._written = True
+
     def mark_grad_ready(self, p: nn.Parameter):
         self._in_backward = True
         s = self.slot_of_param[id(p)]
@@ -810,17 +858,20 @@ class ZeroShardedOptimizer(ZeROOptimizer):
         return self._order_pos.get(rt.u.index, rt.u.index)
 
     @instrument_w_nvtx
-    def fetch_unit(self, rt: _UnitRT, forward=True, prefetch=True):
-        """Make ``rt``'s parameters available on the compute stream; kick off prefetches."""
+    def fetch_unit(self, rt: _UnitRT, forward=True, prefetch=True, borrow=False):
+        """Make ``rt``'s parameters available on the compute stream; kick off prefetches.  ``borrow``: for a module
+        outside the unit that shares one of its parameters (see :meth:`_hook_borrower`)."""
         if not self.transient or rt.u.persistent:
             return
         if forward and not self._trace_done:
+            if borrow:
+                self._borrow_pos.add(len(self._trace))
             self._trace.append(rt.u.index)
         prof = self.param_profiler
         if rt.state == NOT_GATHERED:
             if prof is not None:
                 prof.count("fetch_miss", rt.u.full_numel)   # not prefetched: the gather is issued on demand
-            self._launch_gather(rt)
+            self._launch_gather(rt, borrow=borrow)
         elif prof is not None:
             prof.count("fetch_hit", rt.u.full_numel)
         if rt.state == INFLIGHT:
@@ -829,9 +880,9 @@ class ZeroShardedOptimizer(ZeROOptimizer):
             rt.state = GATHERED
         rt.consumed = True
         if prefetch and self.prefetch_depth > 0:
-            for nxt in self._upcoming(rt, forward):
+            for nxt, nxt_borrow in self._upcoming(rt, forward, borrow):
                 if nxt.state == NOT_GATHERED and not nxt.u.persistent and (forward or not nxt.skip_bwd_fetch):
-                    self._launch_gather(nxt)
+                    self._launch_gather(nxt, borrow=nxt_borrow)
 
     # ---- exposed-communication accounting (bench / profiling aid) -----------------------------------
     def measure_exposed(self, on=True):
@@ -867,25 +918,36 @@ class ZeroShardedOptimizer(ZeROOptimizer):
         self._exposed = []
         return out
 
-    def _upcoming(self, rt, forward):
-        order = self._trace if (self._trace_done and self._trace) else [u.index for u in self.units]
-        try:
-            pos = order.index(rt.u.index) if forward else len(order) - 1 - order[::-1].index(rt.u.index)
-        except ValueError:
+    def _upcoming(self, rt, forward, borrow=False):
+        """-> [(unit, is a borrow)] the next ``prefetch_depth`` entries of the unit order after this fetch."""
+        traced = self._trace_done and self._trace
+        order = self._trace if traced else [u.index for u in self.units]
+        borrows = self._borrow_pos if traced else ()
+        # a unit appears once as itself and once per borrow: the position of this fetch's kind
+        at = [i for i, u in enumerate(order) if u == rt.u.index and (i in borrows) == borrow]
+        if not at:
             return []
+        pos = at[0] if forward else at[-1]
         out = []
         step = 1 if forward else -1
         for k in range(1, self.prefetch_depth + 1):
             q = pos + step * k
             if 0 <= q < len(order):
-                out.append(self.rts[order[q]])
+                out.append((self.rts[order[q]], q in borrows))
         return out
 
-    def _launch_gather(self, rt: _UnitRT):
+    def _launch_gather(self, rt: _UnitRT, borrow=False):
+        """``borrow``: a gather for a module sharing the unit's weight, which runs after the unit's own module and
+        typically after every other unit (a tied LM head).  It has a home of its own (``rt.borrow_home``), first the pool
+        buffer that follows the last unit's: the unit's own home may be held by a unit still live at that point."""
         u = rt.u
         # Autograd may hold *views* of the gathered weights saved during forward, so the backward
         # re-gather must land in the very same memory: ``rt.home`` remembers the forward buffer.
-        slot = rt.home if rt.home is not None else self.param_pool[u.index % len(self.param_pool)]
+        home = rt.borrow_home if borrow else rt.home
+        if home is not None:
+            slot = home
+        else:
+            slot = self.param_pool[(len(self.units) if borrow else u.index) % len(self.param_pool)]
         occ = slot.owner
         if occ is not None and occ is not rt and occ.state != NOT_GATHERED and not occ.consumed \
                 and occ.temp_refs == 0:
@@ -899,13 +961,15 @@ class ZeroShardedOptimizer(ZeROOptimizer):
             # release it (it keeps its home: its own backward gathers it back into the same memory)
             self.release_unit(occ)
         if occ is not None and occ is not rt and occ.state != NOT_GATHERED:
-            if rt.home is not None:
+            if home is not None:
                 raise RuntimeError(
                     f"ZeRO-3 unit '{u.name}' must be re-gathered into the buffer it used in forward, but that "
                     f"buffer still holds live unit '{occ.u.name}'.  Increase zero_optimization.b200_unit_prefetch "
                     f"(pool size) or mark the enclosing module as a z3 leaf module.")
             slot = _Slot(self._symm_or_empty(self.max_full, self.model_dtype))  # irregular graph: private buffer
-        if self._in_backward is False or rt.home is None:
+        if borrow and (self._in_backward is False or rt.borrow_home is None):
+            rt.borrow_home = slot
+        elif not borrow and (self._in_backward is False or rt.home is None):
             rt.home = slot
         stream = self.ag_stream
         cur = torch.cuda.current_stream() if self.on_cuda else None
@@ -1356,18 +1420,21 @@ class ZeroShardedOptimizer(ZeROOptimizer):
             for rt in self.rts:
                 if not rt.u.persistent and rt.state != NOT_GATHERED and rt.grad_full is None:
                     self.release_unit(rt)
-                rt.home = None
+                rt.home = rt.borrow_home = None
                 rt.fwd_calls = rt.bwd_calls = 0
         self._in_backward = False
         if not self._trace_done and self._trace:
             self._trace_done = True
-            # keep first occurrence order
-            seen, order = set(), []
-            for i in self._trace:
-                if i not in seen:
-                    seen.add(i)
+            # keep first occurrence order, of a unit and of each unit's borrows
+            seen, order, borrows = set(), [], set()
+            for pos, i in enumerate(self._trace):
+                key = (i, pos in self._borrow_pos)
+                if key not in seen:
+                    seen.add(key)
+                    if key[1]:
+                        borrows.add(len(order))
                     order.append(i)
-            self._trace = order
+            self._trace, self._borrow_pos = order, borrows
             if self.shard_world > 1:
                 # every rank must walk the units in the same order or the prefetched collectives would mismatch
                 # (reference coordinator.py:237 assert_ints_same_as_other_ranks)
@@ -1991,7 +2058,7 @@ class ZeroShardedOptimizer(ZeROOptimizer):
 
     def reset_step(self):
         """Forget the recorded unit order (the module graph changed): it is re-traced on the next iteration."""
-        self._trace, self._trace_done = [], False
+        self._trace, self._trace_done, self._borrow_pos = [], False, set()
 
     def clear_lp_grads(self):
         self.zero_grad()

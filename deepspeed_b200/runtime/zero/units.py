@@ -49,6 +49,8 @@ class Unit:
     shard_numel: int = 0
     arena_offset: int = 0  # offset of this unit's shard inside the rank-local shard arena
     persistent: bool = False
+    # modules outside the unit's subtree that hold one of its parameters directly (a tied LM head): (name, module)
+    borrowers: List[Tuple[str, nn.Module]] = field(default_factory=list)
 
     @property
     def raw_numel(self):
@@ -102,7 +104,8 @@ def build_units(model: nn.Module,
                 trainable_only: bool = False,
                 param_filter=None) -> List[Unit]:
     """Build the unit plan for ``model``.  Shared (tied) parameters are assigned to the first unit
-    that references them.  Units larger than ``max_unit_numel`` are not split (a unit is the
+    that references them; every other module holding one directly is recorded as a borrower of that
+    unit (:attr:`Unit.borrowers`).  Units larger than ``max_unit_numel`` are not split (a unit is the
     module-hook granularity) but the value is used by ZeRO-1/2 to form reduce buckets."""
     param_to_group = param_to_group or {}
     roots = default_unit_modules(model, leaf_classes)
@@ -142,7 +145,19 @@ def build_units(model: nn.Module,
     for u in units:
         u.arena_offset = arena
         arena += u.shard_numel
+    _find_borrowers(model, units, roots)
     return units
+
+
+def _find_borrowers(model: nn.Module, units: List[Unit], roots) -> None:
+    root_of = dict(roots)  # a ":own" unit holds its root module's own parameters: that module is its subtree
+    subtree = {u.index: {id(m) for m in ([root_of[u.name]] if u.module is None else u.module.modules())} for u in units}
+    owner = {id(s.param): u for u in units for s in u.slots}
+    for name, m in model.named_modules():
+        for p in m.parameters(recurse=False):
+            u = owner.get(id(p))
+            if u is not None and id(m) not in subtree[u.index] and all(b is not m for _, b in u.borrowers):
+                u.borrowers.append((name, m))
 
 
 def _ds_numel(p):
