@@ -28,9 +28,38 @@ __device__ __forceinline__ uint32_t hash_u32(uint32_t x)
 // uniform in [0,1)
 __device__ __forceinline__ float rand01(uint32_t seed, uint32_t idx) { return (hash_u32(seed ^ (idx * 0x9e3779b9u)) >> 8) * (1.0f / 16777216.0f); }
 
+// floor(t + r) for r in [0, 1), exactly: the fp32 sum itself can round up to the next integer (0.5 - 2^-25 + 0.5 is 1)
+__device__ __forceinline__ float floor_add(float t, float r)
+{
+    const float q = floorf(t);
+    return (t - q) >= 1.f - r ? q + 1.f : q;
+}
+
 struct Range {
     float lo, hi;
 };
+
+// Non-finite groups: the range reductions propagate NaN (fmaxf would drop it), so a group holding a NaN or an inf
+// has a non-finite range, gets a NaN scale, and every element of it dequantizes to NaN.  So does an asymmetric group
+// whose range hi - lo overflows fp32: no finite scale spans it.  Its codes are whatever the NaN quotient clamps to;
+// only the scale carries the information.
+__device__ __forceinline__ float nan_max(float a, float b) { return (a > b || a != a) ? a : b; }
+struct NanMaxOp {
+    __device__ __forceinline__ float operator()(float a, float b) const { return nan_max(a, b); }
+    __host__ __device__ static constexpr float identity() { return -3.402823466e+38f; }
+};
+
+// Scale of a group whose range is `span` (amax, or hi - lo) spread over `levels` steps.  NaN when the range is not
+// finite; at least the smallest fp32 subnormal, so that a tiny group keeps a non-zero scale.
+__device__ __forceinline__ float group_scale(float span, float levels)
+{
+    if (!isfinite(span)) return __int_as_float(0x7fc00000);
+    return span > 0.f ? fmaxf(span / levels, 1.401298464e-45f) : 1.f;
+}
+
+// x / scale through the fp32 reciprocal `inv`; when 1/scale overflows (scale below 2^-128) divide instead, so that
+// a zero still encodes to zero.
+__device__ __forceinline__ float to_grid(float x, float scale, float inv) { return isfinite(inv) ? x * inv : x / scale; }
 
 // Block-wide min/max of one group (elements [base, base+n)); leaves the unpacked group in `cache`.
 template <typename T>
@@ -47,14 +76,14 @@ __device__ __forceinline__ Range group_range(const T* __restrict__ x, int n, flo
             Elem<T>::unpack(ld_stream(x + v * kPer), cache[k]);
 #pragma unroll
             for (int e = 0; e < kPer; ++e) {
-                lo = fminf(lo, cache[k][e]);
-                hi = fmaxf(hi, cache[k][e]);
+                lo = -nan_max(-lo, -cache[k][e]);
+                hi = nan_max(hi, cache[k][e]);
             }
         }
     }
     // (n is required to be a multiple of kPer and <= kMaxCache * blockDim * kPer by the host wrapper)
-    hi = block_reduce<MaxOp>(hi, scratch);
-    lo = -block_reduce<MaxOp>(-lo, scratch);
+    hi = block_reduce<NanMaxOp>(hi, scratch);
+    lo = -block_reduce<NanMaxOp>(-lo, scratch);
     return Range{lo, hi};
 }
 
@@ -76,9 +105,9 @@ quantize_kernel(const T* __restrict__ x, int8_t* __restrict__ q, float* __restri
     float scale, offset = 0.f;
     if (SYM) {
         const float amax = fmaxf(fabsf(r.lo), fabsf(r.hi));
-        scale = amax > 0.f ? amax / (qmax + 1.f) : 1.f;  // amax -> 2^(b-1); +side saturates
+        scale = group_scale(amax, qmax + 1.f);  // amax -> 2^(b-1); +side saturates
     } else {
-        scale = (r.hi - r.lo) > 0.f ? (r.hi - r.lo) / (qmax_asym + 1.f) : 1.f;
+        scale = group_scale(r.hi - r.lo, qmax_asym + 1.f);
         offset = r.lo;
     }
     const float inv = 1.f / scale;
@@ -100,9 +129,9 @@ quantize_kernel(const T* __restrict__ x, int8_t* __restrict__ q, float* __restri
             int qi[kPer];
 #pragma unroll
             for (int e = 0; e < kPer; ++e) {
-                float f = (cache[k][e] - offset) * inv;
+                float f = to_grid(cache[k][e] - offset, scale, inv);
                 if (stochastic) {
-                    f = floorf(f + rand01(seed, static_cast<uint32_t>(g * group_size + v * kPer + e)));
+                    f = floor_add(f, rand01(seed, static_cast<uint32_t>(g * group_size + v * kPer + e)));
                 } else {
                     f = rintf(f);
                 }
@@ -149,14 +178,15 @@ loco_quantize_kernel(const T* __restrict__ x, float* __restrict__ err, int8_t* _
             for (int e = 0; e < kPer; ++e) {
                 old[k][e] = eg[v * kPer + e];
                 comp[k][e] += old[k][e];
-                amax = fmaxf(amax, fabsf(comp[k][e]));
+                amax = nan_max(amax, fabsf(comp[k][e]));
             }
         }
     }
-    amax = block_reduce<MaxOp>(amax, scratch);
+    amax = block_reduce<NanMaxOp>(amax, scratch);
     constexpr float qmax = static_cast<float>((1 << (BITS - 1)) - 1);
-    const float scale = amax > 0.f ? amax / (qmax + 1.f) : 1.f;  // amax -> 2^(b-1); +side saturates
+    const float scale = group_scale(amax, qmax + 1.f);  // amax -> 2^(b-1); +side saturates
     const float inv = 1.f / scale;
+    const bool finite = isfinite(scale);  // a non-finite group leaves its error slice as it was: that step is skipped
     if (threadIdx.x == 0) params[g] = scale;
     int8_t* qg = q + static_cast<int64_t>(g) * out_group_stride_bytes;
 #pragma unroll
@@ -166,10 +196,10 @@ loco_quantize_kernel(const T* __restrict__ x, float* __restrict__ err, int8_t* _
             int qi[kPer];
 #pragma unroll
             for (int e = 0; e < kPer; ++e) {
-                float f = fminf(fmaxf(rintf(comp[k][e] * inv), -qmax - 1.f), qmax);
+                float f = fminf(fmaxf(rintf(to_grid(comp[k][e], scale, inv)), -qmax - 1.f), qmax);
                 qi[e] = static_cast<int>(f);
-                const float new_err = comp[k][e] - f * scale;
-                eg[v * kPer + e] = reset ? 0.f : beta * old[k][e] + (1.f - beta) * new_err;
+                const float new_err = __fmaf_rn(-f, scale, comp[k][e]);
+                if (finite) eg[v * kPer + e] = reset ? 0.f : __fmaf_rn(beta, old[k][e], __fmul_rn(1.f - beta, new_err));
             }
             if (BITS == 8) {
 #pragma unroll
@@ -193,7 +223,7 @@ __device__ __forceinline__ float dequant_one(const int8_t* qg, int i, int bits, 
         v = (i & 1) ? (byte >> 4) : (byte & 0xf);
         if (sym && (v & 8)) v -= 16;
     }
-    return static_cast<float>(v) * scale + offset;
+    return __fmaf_rn(static_cast<float>(v), scale, offset);
 }
 
 template <typename T>
@@ -234,25 +264,25 @@ dequant_reduce_kernel(const int8_t* __restrict__ qin, const float* __restrict__ 
             const float off = SYM ? 0.f : pin[2 * gi + 1];
             s += dequant_one(qin + gi * bpg, i, BITS, SYM, scale, off);
         }
-        if (err) s += err_beta * err[static_cast<int64_t>(g) * group_size + i];
+        if (err) s = __fmaf_rn(err_beta, err[static_cast<int64_t>(g) * group_size + i], s);
         acc[i] = s;
     }
     __syncthreads();
     float lo = 3.402823466e+38f, hi = -3.402823466e+38f;
     for (int i = threadIdx.x; i < group_size; i += blockDim.x) {
-        lo = fminf(lo, acc[i]);
-        hi = fmaxf(hi, acc[i]);
+        lo = -nan_max(-lo, -acc[i]);
+        hi = nan_max(hi, acc[i]);
     }
-    hi = block_reduce<MaxOp>(hi, scratch);
-    lo = -block_reduce<MaxOp>(-lo, scratch);
+    hi = block_reduce<NanMaxOp>(hi, scratch);
+    lo = -block_reduce<NanMaxOp>(-lo, scratch);
     constexpr float qmax = static_cast<float>((1 << (BITS - 1)) - 1);
     constexpr float qmax_asym = static_cast<float>((1 << BITS) - 1);
     float scale, offset = 0.f;
     if (SYM) {
         const float amax = fmaxf(fabsf(lo), fabsf(hi));
-        scale = amax > 0.f ? amax / (qmax + 1.f) : 1.f;  // amax -> 2^(b-1); +side saturates
+        scale = group_scale(amax, qmax + 1.f);  // amax -> 2^(b-1); +side saturates
     } else {
-        scale = (hi - lo) > 0.f ? (hi - lo) / (qmax_asym + 1.f) : 1.f;
+        scale = group_scale(hi - lo, qmax_asym + 1.f);
         offset = lo;
     }
     if (threadIdx.x == 0) {
@@ -269,10 +299,11 @@ dequant_reduce_kernel(const int8_t* __restrict__ qin, const float* __restrict__ 
     for (int i = threadIdx.x * step; i < group_size; i += blockDim.x * step) {
         int qi[2];
         for (int e = 0; e < step; ++e) {
-            float f = rintf((acc[i + e] - offset) * inv);
+            float f = rintf(to_grid(acc[i + e] - offset, scale, inv));
             f = SYM ? fminf(fmaxf(f, -qmax - 1.f), qmax) : fminf(fmaxf(f, 0.f), qmax_asym);
             qi[e] = static_cast<int>(f);
-            if (err) err[static_cast<int64_t>(g) * group_size + i + e] = acc[i + e] - (f * scale + offset);
+            if (err && isfinite(scale))  // a non-finite group leaves its error slice as it was
+                err[static_cast<int64_t>(g) * group_size + i + e] = acc[i + e] - __fmaf_rn(f, scale, offset);
         }
         if (BITS == 8)
             qg[i] = static_cast<int8_t>(SYM ? qi[0] : qi[0] - 128);
@@ -297,11 +328,11 @@ fake_quant_kernel(T* __restrict__ x, int group_size, int bits, int sym, int stoc
     float scale, offset = 0.f, lo_q, hi_q;
     if (sym) {
         const float amax = fmaxf(fabsf(r.lo), fabsf(r.hi));
-        scale = amax > 0.f ? amax / (qmax + 1.f) : 1.f;  // amax -> 2^(b-1); +side saturates
+        scale = group_scale(amax, qmax + 1.f);  // amax -> 2^(b-1); +side saturates
         lo_q = -qmax - 1.f;
         hi_q = qmax;
     } else {
-        scale = (r.hi - r.lo) > 0.f ? (r.hi - r.lo) / (levels + 1.f) : 1.f;
+        scale = group_scale(r.hi - r.lo, levels + 1.f);
         offset = r.lo;
         lo_q = 0.f;
         hi_q = levels;
@@ -315,10 +346,10 @@ fake_quant_kernel(T* __restrict__ x, int group_size, int bits, int sym, int stoc
             float o[kPer];
 #pragma unroll
             for (int e = 0; e < kPer; ++e) {
-                float f = (cache[k][e] - offset) * inv;
-                f = stochastic ? floorf(f + rand01(seed, static_cast<uint32_t>(g * group_size + v * kPer + e))) : rintf(f);
+                float f = to_grid(cache[k][e] - offset, scale, inv);
+                f = stochastic ? floor_add(f, rand01(seed, static_cast<uint32_t>(g * group_size + v * kPer + e))) : rintf(f);
                 f = fminf(fmaxf(f, lo_q), hi_q);
-                o[e] = f * scale + offset;
+                o[e] = __fmaf_rn(f, scale, offset);
             }
             st_plain(xg + v * kPer, Elem<T>::pack(o));
         }
@@ -342,13 +373,13 @@ __device__ __forceinline__ uint32_t minifloat_encode(float x, int E, int M, floa
     uint32_t code;
     const float min_normal = ldexpf(1.f, 1 - bias);
     if (a < min_normal) {
-        const float q = floorf(a * ldexpf(1.f, M - (1 - bias)) + rnd);  // units of the subnormal step
+        const float q = floor_add(a * ldexpf(1.f, M - (1 - bias)), rnd);  // units of the subnormal step
         code = static_cast<uint32_t>(q);                                 // == 1<<M rolls into the first normal
     } else {
         int e;
         const float fr = frexpf(a, &e);  // a = fr * 2^e, fr in [0.5,1)
         e -= 1;                          // a = (2*fr) * 2^e with 2*fr in [1,2)
-        float m = floorf((2.f * fr - 1.f) * static_cast<float>(1 << M) + rnd);
+        float m = floor_add((2.f * fr - 1.f) * static_cast<float>(1 << M), rnd);
         if (m >= static_cast<float>(1 << M)) {
             m = 0.f;
             e += 1;
@@ -383,21 +414,6 @@ __device__ __forceinline__ float fp_format_max(int bits, int M)
     return minifloat_max(bits - 1 - M, M);
 }
 
-__device__ __forceinline__ uint32_t fp_encode(float x, int bits, int M, float rnd)
-{
-    if (bits == 8) {
-        if (rnd != 0.5f) {  // stochastic: dither by one target ulp before the RN hardware convert
-            const float ax = fabsf(x);
-            int e;
-            frexpf(ax > 0.f ? ax : 1e-30f, &e);
-            const float ulp = ldexpf(1.f, (e - 1) - M);
-            x += (rnd - 0.5f) * ulp;
-        }
-        return static_cast<uint32_t>(__nv_cvt_float_to_fp8(x, __NV_SATFINITE, M == 3 ? __NV_E4M3 : __NV_E5M2));
-    }
-    return minifloat_encode(x, bits - 1 - M, M, rnd);
-}
-
 __device__ __forceinline__ float fp_decode(uint32_t code, int bits, int M)
 {
     if (bits == 8) {
@@ -405,6 +421,29 @@ __device__ __forceinline__ float fp_decode(uint32_t code, int bits, int M)
         return __half2float(*reinterpret_cast<const __half*>(&h));
     }
     return minifloat_decode(code, bits - 1 - M, M);
+}
+
+__device__ __forceinline__ uint32_t fp_encode(float x, int bits, int M, float rnd)
+{
+    if (bits == 8) {
+        const __nv_fp8_interpretation_t fmt = M == 3 ? __NV_E4M3 : __NV_E5M2;
+        if (rnd != 0.5f && x == x) {
+            // stochastic: floor(|x| / ulp + rnd) * ulp, with ulp the grid spacing at |x| (the subnormal step below
+            // the smallest normal).  The hardware only rounds to nearest, so convert |x| + rnd * ulp and step one
+            // code down when that rounded up.
+            const float ax = fabsf(x);
+            const int emin = M == 3 ? -6 : -14;  // exponent of the smallest normal
+            int e;
+            frexpf(ax, &e);  // ax in [2^(e-1), 2^e)
+            const float ulp = ldexpf(1.f, (ax < ldexpf(1.f, emin) ? emin : e - 1) - M);
+            const float y = ax + rnd * ulp;
+            uint32_t c = __nv_cvt_float_to_fp8(y, __NV_SATFINITE, fmt);
+            if (fp_decode(c, 8, M) > y) c -= 1;
+            return x < 0.f ? (c | 0x80u) : c;
+        }
+        return static_cast<uint32_t>(__nv_cvt_float_to_fp8(x, __NV_SATFINITE, fmt));
+    }
+    return minifloat_encode(x, bits - 1 - M, M, rnd);
 }
 
 // Packed code storage: codes of `bits` width are written little-endian into a byte stream per group.
@@ -443,10 +482,9 @@ fp_quantize_kernel(const T* __restrict__ x, uint8_t* __restrict__ q, float* __re
     if (g >= groups) return;
     const T* xg = x + g * group_size;
     float amax = 0.f;
-    for (int i = lane; i < group_size; i += 32) amax = fmaxf(amax, fabsf(Elem<T>::to_f(xg[i])));
-    amax = warp_reduce<MaxOp>(amax);
-    const float fmax = fp_format_max(bits, M);
-    const float scale = amax > 0.f ? amax / fmax : 1.f;
+    for (int i = lane; i < group_size; i += 32) amax = nan_max(amax, fabsf(Elem<T>::to_f(xg[i])));
+    amax = warp_reduce<NanMaxOp>(amax);
+    const float scale = group_scale(amax, fp_format_max(bits, M));
     const float inv = 1.f / scale;
     if (lane == 0) scales[g] = scale;
     const int64_t bytes_per_group = (static_cast<int64_t>(group_size) * bits + 7) / 8;
@@ -457,7 +495,7 @@ fp_quantize_kernel(const T* __restrict__ x, uint8_t* __restrict__ q, float* __re
         uint32_t codes[4];
         for (int e = 0; e < per; ++e) {
             const int i = i0 + e;
-            const float v = i < group_size ? Elem<T>::to_f(xg[i]) * inv : 0.f;
+            const float v = i < group_size ? to_grid(Elem<T>::to_f(xg[i]), scale, inv) : 0.f;
             const float rnd = stochastic ? rand01(seed, static_cast<uint32_t>(g * group_size + i)) : 0.5f;
             codes[e] = fp_encode(v, bits, M, rnd);
         }
@@ -591,6 +629,7 @@ DSB_EXPORT int dsb_dequantize(const void* q, const float* params, void* out, int
                               int sym, int out_dtype, cudaStream_t stream)
 {
     if (groups <= 0) return 0;
+    if ((bits != 4 && bits != 8) || group_size % 2) return -2;
     const int64_t total = groups * group_size;
     const int grid = flat_grid(total, kThreads, 16);
     DISPATCH_QT(out_dtype, T, {
@@ -598,6 +637,18 @@ DSB_EXPORT int dsb_dequantize(const void* q, const float* params, void* out, int
     })
     DSB_CHECK_LAUNCH();
     return 0;
+}
+
+template <int BITS, bool SYM>
+static void launch_dequant_reduce(const void* qin, const float* pin, void* qout, float* pout, int peers, int out_groups,
+                                  int group_size, float* err, float err_beta, size_t smem, cudaStream_t stream)
+{
+    // the kernel's static scratch comes on top of the dynamic accumulators: past the default 48 KB in all for the
+    // largest groups, so opt in to 48 KB of dynamic shared memory
+    if (smem > 46 * 1024)
+        cudaFuncSetAttribute(dequant_reduce_kernel<BITS, SYM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024);
+    dequant_reduce_kernel<BITS, SYM><<<out_groups, kThreads, smem, stream>>>((const int8_t*)qin, pin, (int8_t*)qout, pout,
+                                                                            peers, out_groups, group_size, err, err_beta);
 }
 
 DSB_EXPORT int dsb_dequant_reduce(const void* qin, const float* pin, void* qout, float* pout, int peers, int out_groups,
@@ -608,17 +659,13 @@ DSB_EXPORT int dsb_dequant_reduce(const void* qin, const float* pin, void* qout,
     const size_t smem = static_cast<size_t>(group_size) * sizeof(float);
     if (smem > 48 * 1024) return -2;
     if (bits == 8 && sym)
-        dequant_reduce_kernel<8, true><<<out_groups, kThreads, smem, stream>>>((const int8_t*)qin, pin, (int8_t*)qout, pout,
-                                                                                 peers, out_groups, group_size, err, err_beta);
+        launch_dequant_reduce<8, true>(qin, pin, qout, pout, peers, out_groups, group_size, err, err_beta, smem, stream);
     else if (bits == 8)
-        dequant_reduce_kernel<8, false><<<out_groups, kThreads, smem, stream>>>((const int8_t*)qin, pin, (int8_t*)qout, pout,
-                                                                                  peers, out_groups, group_size, err, err_beta);
+        launch_dequant_reduce<8, false>(qin, pin, qout, pout, peers, out_groups, group_size, err, err_beta, smem, stream);
     else if (sym)
-        dequant_reduce_kernel<4, true><<<out_groups, kThreads, smem, stream>>>((const int8_t*)qin, pin, (int8_t*)qout, pout,
-                                                                                 peers, out_groups, group_size, err, err_beta);
+        launch_dequant_reduce<4, true>(qin, pin, qout, pout, peers, out_groups, group_size, err, err_beta, smem, stream);
     else
-        dequant_reduce_kernel<4, false><<<out_groups, kThreads, smem, stream>>>((const int8_t*)qin, pin, (int8_t*)qout, pout,
-                                                                                  peers, out_groups, group_size, err, err_beta);
+        launch_dequant_reduce<4, false>(qin, pin, qout, pout, peers, out_groups, group_size, err, err_beta, smem, stream);
     DSB_CHECK_LAUNCH();
     return 0;
 }
@@ -636,11 +683,16 @@ DSB_EXPORT int dsb_fake_quantize(void* x, int64_t groups, int group_size, int bi
 }
 
 // bits in {4, 6, 8, 12}; mantissa bits M: FP8 E4M3 -> 3, E5M2 -> 2, FP6 -> 2, FP4 -> 1, FP12 -> 7
+static inline bool fp_format_ok(int bits, int M)
+{
+    return (bits == 8 && (M == 3 || M == 2)) || (bits == 6 && M == 2) || (bits == 4 && M == 1) || (bits == 12 && M == 7);
+}
+
 DSB_EXPORT int dsb_fp_quantize(const void* x, void* q, float* scales, int64_t groups, int group_size, int bits, int M,
                                int dtype, int stochastic, uint32_t seed, cudaStream_t stream)
 {
     if (groups <= 0) return 0;
-    if ((bits != 4 && bits != 6 && bits != 8 && bits != 12) || group_size % 4) return -2;
+    if (!fp_format_ok(bits, M) || group_size % 4) return -2;
     const int grid = static_cast<int>((groups + (kThreads / 32) - 1) / (kThreads / 32));
     DISPATCH_QT(dtype, T, {
         fp_quantize_kernel<T><<<grid, kThreads, 0, stream>>>((const T*)x, (uint8_t*)q, scales, groups, group_size, bits, M,
@@ -654,6 +706,7 @@ DSB_EXPORT int dsb_fp_dequantize(const void* q, const float* scales, void* out, 
                                  int bits, int M, int out_dtype, const int* rows, int groups_per_row, cudaStream_t stream)
 {
     if (out_groups <= 0) return 0;
+    if (!fp_format_ok(bits, M) || group_size % 4) return -2;
     const int grid = flat_grid(out_groups * group_size, kThreads, 16);
     DISPATCH_QT(out_dtype, T, {
         fp_dequantize_kernel<T><<<grid, kThreads, 0, stream>>>((const uint8_t*)q, scales, (T*)out, out_groups, group_size,

@@ -8,6 +8,7 @@ import ctypes
 import torch
 
 from deepspeed_b200.ops import native as N
+from deepspeed_b200.ops.quantizer.quantizer import _to_grid
 
 _MANTISSA = {8: 3, 6: 2, 4: 1, 12: 7}
 
@@ -36,7 +37,8 @@ def _host_codec(v, bits, m):
     sub_step = 2.0**(1 - bias - m)
     ex = torch.floor(torch.log2(a.clamp(min=1e-30)))
     step = torch.where(a < min_normal, torch.full_like(a, sub_step), 2.0**(ex - m))
-    q = torch.floor(a / step + 0.5) * step
+    t = a / step
+    q = (torch.floor(t) + (t - torch.floor(t) >= 0.5)) * step  # ties away; t + 0.5 could round up from below a tie
     return torch.sign(v) * q.clamp(max=_fmt_max(bits, m))
 
 
@@ -82,9 +84,12 @@ class FP_Quantize(Quantizer):
         else:
             g = x.float().reshape(groups, gs)
             amax = g.abs().amax(1, keepdim=True)
-            scales = torch.where(amax > 0, amax / _fmt_max(q_bits, q_mantisa_bits), torch.ones_like(amax)).reshape(groups)
+            # the kernel's scale: NaN for a group holding a NaN or an inf, at least the smallest fp32 subnormal
+            scales = torch.where(amax > 0, (amax / _fmt_max(q_bits, q_mantisa_bits)).clamp(min=2.0**-149),
+                                 torch.ones_like(amax))
+            scales = torch.where(torch.isfinite(amax), scales, float("nan")).reshape(groups)
             # host tier keeps decoded values (1 float per code) -- layout is an implementation detail
-            q = _host_codec(g / scales[:, None], q_bits, q_mantisa_bits).reshape(-1)
+            q = _host_codec(_to_grid(g, scales[:, None]), q_bits, q_mantisa_bits).reshape(-1)
         self.scales = scales
         if return_meta_tensor:
             return q, scales

@@ -18,24 +18,62 @@ def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else ctypes.c_void_p(0)
 
 
-def _host_quant(x, groups, bits, sym, stochastic=False):
-    g = x.reshape(groups, -1).float()
+def _fma32(a, b, c):
+    """fp32 ``a * b + c`` rounded once, like the kernels' ``__fmaf_rn``.  The float64 product of two fp32 values is
+    exact, but the float64 sum may round; rounding that sum to fp32 again is only wrong when it lands exactly on an fp32
+    midpoint, and then the sum's exact error (TwoSum) says which neighbour the exact value is nearer to."""
+    p = a.double() * b.double()
+    c = c.double()
+    s = p + c
+    bb = s - p
+    err = (p - (s - bb)) + (c - bb)
+    r = s.float()
+    d = s - r.double()
+    up, dn = torch.nextafter(r, torch.full_like(r, float("inf"))), torch.nextafter(r, torch.full_like(r, -float("inf")))
+    r = torch.where((err > 0) & (d > 0) & (d == (up.double() - r.double()) / 2), up, r)
+    return torch.where((err < 0) & (d < 0) & (-d == (r.double() - dn.double()) / 2), dn, r)
+
+
+def _to_grid(x, scale):
+    """``x / scale`` as the kernels compute it: times the fp32 reciprocal, or divided when that overflows."""
+    inv = 1.0 / scale
+    return torch.where(torch.isfinite(inv), x * inv, x / scale)
+
+
+def _host_codes(g, bits, sym, stochastic=False):
+    """Codes (as floats) of the groups in the rows of fp32 ``g``, with the kernels' arithmetic: the scale is the
+    group's range over ``2^bits`` steps (at least the smallest fp32 subnormal), ``x * (1/scale)`` through the fp32
+    reciprocal (a division when that overflows), round half to even, clamp.  A group whose range is not finite (it
+    holds a NaN or an inf, or its asymmetric range overflows) gets a NaN scale and the lowest code everywhere, so all of
+    it dequantizes to NaN.  Returns ``(v, scale, offset)``."""
+    nan = torch.full_like(g[:, :1], float("nan"))
     if sym:
-        qmax = 2**(bits - 1) - 1
-        amax = g.abs().amax(dim=1, keepdim=True)
-        scale = torch.where(amax > 0, amax / (qmax + 1), torch.ones_like(amax))  # reference: q_range / (2 * absmax)
-        v = g / scale
-        v = torch.floor(v + torch.rand_like(v)) if stochastic else torch.round(v)
-        q = v.clamp(-qmax - 1, qmax).to(torch.int32)
-        params = scale.reshape(groups)
+        span, offset = g.abs().amax(dim=1, keepdim=True), torch.zeros_like(nan)
+        lo_q, hi_q, steps = -2**(bits - 1), 2**(bits - 1) - 1, 2**(bits - 1)  # amax -> 2^(b-1); +side saturates
     else:
-        levels = 2**bits - 1
-        lo, hi = g.amin(dim=1, keepdim=True), g.amax(dim=1, keepdim=True)
-        scale = torch.where(hi > lo, (hi - lo) / (levels + 1), torch.ones_like(hi))  # reference: q_range / (max - min)
-        v = (g - lo) / scale
-        v = torch.floor(v + torch.rand_like(v)) if stochastic else torch.round(v)
-        q = v.clamp(0, levels).to(torch.int32)
-        params = torch.cat([scale, lo], dim=1)
+        offset = g.amin(dim=1, keepdim=True)
+        span = g.amax(dim=1, keepdim=True) - offset
+        lo_q, hi_q, steps = 0, 2**bits - 1, 2**bits
+    bad = ~torch.isfinite(span)
+    scale = torch.where(bad, nan, torch.where(span > 0, (span / steps).clamp(min=2.0**-149), torch.ones_like(span)))
+    v = _to_grid(g - offset, scale)
+    if stochastic:  # floor(v + r), exactly
+        fl = torch.floor(v)
+        v = fl + (v - fl >= 1.0 - torch.rand_like(v))
+    else:
+        v = torch.round(v)
+    v = torch.where(bad, torch.full_like(v, lo_q), v.clamp(lo_q, hi_q))
+    return v, scale, offset
+
+
+def _host_quant(x, groups, bits, sym, stochastic=False):
+    return _host_pack(*_host_codes(x.reshape(groups, -1).float(), bits, sym, stochastic), bits, sym)
+
+
+def _host_pack(v, scale, offset, bits, sym):
+    groups = v.shape[0]
+    q = v.to(torch.int32)
+    params = scale.reshape(groups) if sym else torch.cat([scale, offset], dim=1)
     if bits == 8:
         out = (q if sym else q - 128).to(torch.int8)
     else:
@@ -57,7 +95,7 @@ def _host_dequant(q, params, groups, bits, sym, dtype):
     if sym:
         return (v.float() * params.reshape(groups, 1)).to(dtype)
     p = params.reshape(groups, 2)
-    return (v.float() * p[:, :1] + p[:, 1:]).to(dtype)
+    return _fma32(v.float(), p[:, :1], p[:, 1:]).to(dtype)
 
 
 def aligned_group_size(n, target=2048):
@@ -104,13 +142,17 @@ def loco_quantize(x, err, groups, num_bits=4, beta=0.8, reset=False):
     assert n % groups == 0 and err.numel() == n and err.dtype == torch.float32 and err.is_contiguous()
     gs = n // groups
     if not x.is_cuda:
-        comp = x.reshape(-1).float() + err.reshape(-1)
-        q, params = _host_quant(comp, groups, num_bits, True)
-        deq = _host_dequant(q, params, groups, num_bits, True, torch.float32).reshape(-1)
+        comp = x.reshape(groups, -1).float() + err.reshape(groups, -1)
+        v, scale, offset = _host_codes(comp, num_bits, True)
+        q, params = _host_pack(v, scale, offset, num_bits, True)
+        ok = torch.isfinite(scale)  # a non-finite group leaves its error slice as it was
+        e = err.view(groups, -1)
         if reset:
-            err.zero_()
+            new = torch.zeros_like(e)
         else:
-            err.reshape(-1).mul_(beta).add_(comp - deq, alpha=1.0 - beta)
+            f = torch.tensor(beta, dtype=torch.float32)
+            new = _fma32(f, e, (1.0 - f) * _fma32(-v, scale, comp))
+        e.copy_(torch.where(ok, new, e))
         return q.reshape(-1), params
     q = torch.empty(n if num_bits == 8 else n // 2, dtype=torch.int8, device=x.device)
     params = torch.empty(groups, dtype=torch.float32, device=x.device)
@@ -161,12 +203,17 @@ def quantized_reduction(q, params, in_groups, out_groups, num_bits=8, q_type=Sym
     n_in = q.numel() * (1 if num_bits == 8 else 2)
     gs = n_in // in_groups
     if not q.is_cuda:
-        full = _host_dequant(q, params, in_groups, num_bits, sym, torch.float32).reshape(peers, out_groups, gs).sum(0)
+        deq = _host_dequant(q, params, in_groups, num_bits, sym, torch.float32).reshape(peers, out_groups, gs)
+        full = torch.zeros(out_groups, gs)
+        for p in range(peers):  # the kernel's order of summation
+            full = full + deq[p]
         if err is not None:
-            full = full + err_beta * err.reshape(out_groups, gs)
+            e = err.view(out_groups, gs)
+            full = _fma32(torch.tensor(err_beta, dtype=torch.float32), e, full)
         oq, op = _host_quant(full, out_groups, num_bits, sym)
         if err is not None:
-            err.copy_((full - _host_dequant(oq, op, out_groups, num_bits, sym, torch.float32)).reshape(err.shape))
+            ok = torch.isfinite(op.reshape(out_groups, -1)[:, :1])  # a non-finite group leaves its error slice as it was
+            e.copy_(torch.where(ok, full - _host_dequant(oq, op, out_groups, num_bits, sym, torch.float32), e))
         return oq.reshape(-1), op
     oq = torch.empty(out_groups * gs // (1 if num_bits == 8 else 2), dtype=torch.int8, device=q.device)
     op = torch.empty(out_groups if sym else out_groups * 2, dtype=torch.float32, device=q.device)
@@ -187,22 +234,8 @@ def fake_quantize(x, groups, num_bits, q_type=Symmetric, stochastic=False, seed=
     sym = q_type == Symmetric
     gs = x.numel() // groups
     if not x.is_cuda:
-        g = x.reshape(groups, gs).float()
-        if sym:
-            qmax = 2**(num_bits - 1) - 1
-            amax = g.abs().amax(1, keepdim=True)
-            sc = torch.where(amax > 0, amax / (qmax + 1), torch.ones_like(amax))
-            v = g / sc
-            v = torch.floor(v + torch.rand_like(v)) if stochastic else torch.round(v)
-            y = v.clamp(-qmax - 1, qmax) * sc
-        else:
-            lv = 2**num_bits - 1
-            lo, hi = g.amin(1, keepdim=True), g.amax(1, keepdim=True)
-            sc = torch.where(hi > lo, (hi - lo) / (lv + 1), torch.ones_like(hi))
-            v = (g - lo) / sc
-            v = torch.floor(v + torch.rand_like(v)) if stochastic else torch.round(v)
-            y = v.clamp(0, lv) * sc + lo
-        x.copy_(y.reshape(x.shape).to(x.dtype))
+        v, sc, lo = _host_codes(x.reshape(groups, gs).float(), num_bits, sym, stochastic)
+        x.copy_(_fma32(v, sc, lo).reshape(x.shape).to(x.dtype))
         return x
     rc = N.cuda().dsb_fake_quantize(_p(x), ctypes.c_int64(groups), gs, num_bits, int(sym), N.dt(x), int(stochastic),
                                     ctypes.c_uint32(seed & 0xffffffff), N.stream())

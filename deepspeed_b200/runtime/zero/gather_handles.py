@@ -32,31 +32,37 @@ class QuantizationInfo:
 
 class CUDAQuantizer:
     """Symmetric int8 group codec backed by the native quantiser op.  Group count is chosen so that groups are a
-    multiple of 8 elements, ≤16k elements, and as close to ``target_group_size`` as divisibility allows (cached per
-    tensor size)."""
+    multiple of 8 elements, no larger than the kernel takes for the dtype (8192 16-bit or 4096 fp32 elements), and as
+    close to ``target_group_size`` as divisibility allows (cached per tensor size and dtype)."""
     async_flag = True
     target_group_size = 8000
     group_size_cache = {}
 
-    def _groups_for(self, n):
-        g = self.group_size_cache.get(n)
+    @staticmethod
+    def max_group_size(dtype):
+        """Largest group the quantize kernel accepts: one CTA keeps 4 16-byte vectors per thread in registers."""
+        return 4096 if dtype == torch.float32 else 8192
+
+    def _groups_for(self, n, dtype=torch.bfloat16):
+        key = (n, self.max_group_size(dtype))
+        g = self.group_size_cache.get(key)
         if g is not None:
             return g
         assert n % 8 == 0, f"quantised weights need a multiple of 8 elements, got {n}"
         units = n // 8  # groups must divide ``units``
-        lo = max(1, math.ceil(n / 16000 + 1e-9))
+        lo = max(1, math.ceil(n / key[1]))
         want = max(lo, math.ceil(n / self.target_group_size))
         cands = [d for d in _divisors(units) if d >= lo]
         assert cands and cands[0] < n, f"adaptive grouping cannot find a group size for a tensor of {n} elements"
         # largest group (fewest groups) that still respects the 8k target; else the smallest legal count
         below = [d for d in cands if d >= want]
         g = below[0] if below else cands[-1]
-        self.group_size_cache[n] = g
+        self.group_size_cache[key] = g
         return g
 
     def quantize(self, param, groups=None):
         from deepspeed_b200.ops.quantizer import quantizer as Q
-        groups = groups or self._groups_for(param.numel())
+        groups = groups or self._groups_for(param.numel(), param.dtype)
         return Q.quantize(param.contiguous().view(-1), groups, 8, Q.Symmetric)
 
     def dequantize(self, quantized_param, scale, dtype=torch.bfloat16):

@@ -1,4 +1,4 @@
-"""sm_90a kernels of misc.cu / quant.cu / moe_ragged.cu vs their host (plain PyTorch fp32) definitions."""
+"""sm_90a kernels of misc.cu / moe_ragged.cu vs their host (plain PyTorch fp32) definitions (quant.cu: test_quant_exact_gpu.py)."""
 import pytest
 import torch
 
@@ -125,25 +125,3 @@ def test_onebit_pack_unpack_kernels_match_torch_path():
     torch.testing.assert_close(got, ref, atol=1e-6, rtol=1e-5)
     # single-rank backend round trip through the kernels
     be = C.CompressedBackend(group=None) if torch.distributed.is_initialized() else None
-
-
-@pytest.mark.parametrize("bits", [4, 8])
-@pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
-def test_loco_quantize_kernel_matches_host_definition(bits, dtype):
-    """Fused LoCo kernel (compensate + quantise + error update in one pass) vs the host formulation of the same op."""
-    from deepspeed_b200.ops.quantizer import quantizer as Q
-    torch.manual_seed(0)
-    groups, gs = 37, 2048
-    x = (torch.randn(groups * gs, device="cuda") * 3).to(dtype)
-    err = torch.randn(groups * gs, device="cuda") * 0.05
-    err_h, x_h = err.cpu().clone(), x.cpu().clone()
-    q, p = Q.loco_quantize(x, err, groups, num_bits=bits, beta=0.8)
-    qh, ph = Q.loco_quantize(x_h, err_h, groups, num_bits=bits, beta=0.8)
-    torch.testing.assert_close(p.cpu(), ph, rtol=1e-6, atol=1e-7)
-    mism = (q.cpu() != qh).float().mean().item()
-    assert mism < 1e-3, mism  # ties at .5 may round differently after the fp32 divide
-    close = (err.cpu() - err_h).abs() < 1e-5
-    assert close.float().mean().item() > 0.999
-    # reset clears the feedback buffer
-    Q.loco_quantize(x, err, groups, num_bits=bits, beta=0.8, reset=True)
-    assert err.abs().max().item() == 0.0

@@ -44,7 +44,7 @@ def assert_within(out, ref, bound, what):
 def assert_bits_equal(out, ref, what):
     """``out`` and ``ref`` (same dtype) hold the same bit patterns, NaN payloads and signed zeros included."""
     assert out.dtype == ref.dtype and out.shape == ref.shape, (what, out.dtype, ref.dtype, out.shape, ref.shape)
-    view = {2: torch.int16, 4: torch.int32, 8: torch.int64}[out.element_size()]
+    view = {1: torch.int8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[out.element_size()]
     bad = out.contiguous().view(view) != ref.contiguous().view(view)
     if bool(bad.any()):
         k = int(bad.reshape(-1).nonzero()[0])
@@ -813,3 +813,272 @@ def clip_coeff_reference(sumsq, inv_loss_scale, max_norm):
 def round_bf16_truncate(x):
     """fp32 -> bf16 by dropping the low 16 bits (round toward zero): the wrong cast a bound check must reject."""
     return (x.float().contiguous().view(torch.int32) & -65536).view(torch.float32).bfloat16()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# group quantization (csrc/cuda/quant.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+# Exact emulations of the kernels' fp32 arithmetic, in numpy float32 (IEEE, subnormals kept, like the kernels built
+# without fast-math): a group's scale is ``span / 2^k`` (at least the smallest fp32 subnormal, 1 for an empty range,
+# NaN when the group holds a NaN or an inf), codes are ``rint(x * (1/scale))`` through the fp32 reciprocal (a division
+# when that overflows), clamped; dequantization is ``fmaf(code, scale, offset)``.  The minifloat formats are defined
+# independently: each grid is enumerated from its codes and values are rounded to the nearest grid point in float64.
+import numpy as np  # noqa: E402
+
+F32_TINY = np.float32(2.0**-149)  # smallest fp32 subnormal
+
+
+def _np32(x):
+    return x.detach().cpu().float().numpy() if torch.is_tensor(x) else np.asarray(x, dtype=np.float32)
+
+
+def fmaf(a, b, c):
+    """fp32 ``a * b + c`` rounded once (``__fmaf_rn``).  The float64 product of two fp32 values is exact; the float64
+    sum is corrected with its exact rounding error (TwoSum) where it lands on an fp32 rounding midpoint."""
+    a, b, c = (np.asarray(t, dtype=np.float32).astype(np.float64) for t in (a, b, c))
+    p = a * b
+    s = p + c
+    bb = s - p
+    err = (p - (s - bb)) + (c - bb)
+    with np.errstate(invalid="ignore", over="ignore"):
+        r = s.astype(np.float32)
+        d = s - r.astype(np.float64)
+        up = np.nextafter(r, np.float32(np.inf))
+        dn = np.nextafter(r, np.float32(-np.inf))
+        half_up = (up.astype(np.float64) - r) / 2
+        half_dn = (r.astype(np.float64) - dn.astype(np.float64)) / 2
+        fix_up = (err > 0) & (d > 0) & (d == half_up)
+        fix_dn = (err < 0) & (d < 0) & (-d == half_dn)
+    return np.where(fix_up, up, np.where(fix_dn, dn, r)).astype(np.float32)
+
+
+def to_grid(x, scale):
+    """``x / scale`` as the kernels compute it: ``x * (1/scale)`` in fp32, or the division when ``1/scale`` overflows."""
+    x, scale = np.asarray(x, np.float32), np.asarray(scale, np.float32)
+    with np.errstate(divide="ignore", over="ignore", invalid="ignore"):
+        inv = np.float32(1) / scale
+        return np.where(np.isfinite(inv), x * inv, x / scale).astype(np.float32)
+
+
+def group_scale(span, finite, steps):
+    """Scale of a group whose range is ``span`` (fp32) over ``steps`` quantization steps."""
+    span = np.asarray(span, np.float32)
+    with np.errstate(invalid="ignore", over="ignore"):
+        sc = np.where(span > 0, np.maximum(span / np.float32(steps), F32_TINY), np.float32(1)).astype(np.float32)
+    return np.where(finite, sc, np.float32(np.nan)).astype(np.float32)
+
+
+def int_quant_reference(x, groups, bits, sym, rint=np.rint):
+    """Emulation of ``quantize_kernel`` / ``fake_quant_kernel``: ``(codes int64 [groups, gs], scale, offset)`` with
+    codes in ``[-2^(b-1), 2^(b-1)-1]`` (symmetric) or ``[0, 2^b - 1]`` (asymmetric, before the int8 bias of -128)."""
+    g = _np32(x).reshape(groups, -1)
+    with np.errstate(invalid="ignore", over="ignore"):
+        if sym:
+            lo_q, hi_q, steps = -2**(bits - 1), 2**(bits - 1) - 1, 2**(bits - 1)
+            span = np.abs(g).max(axis=1)
+            offset = np.zeros(groups, np.float32)
+        else:
+            lo_q, hi_q, steps = 0, 2**bits - 1, 2**bits
+            offset = g.min(axis=1)
+            span = (g.max(axis=1) - offset).astype(np.float32)
+        finite = np.isfinite(span)  # a NaN or an inf in the group, or an asymmetric range beyond fp32
+        scale = group_scale(span, finite, steps)
+        v = rint(to_grid(g - offset[:, None], scale[:, None]))
+        v = np.where(finite[:, None], np.clip(v, lo_q, hi_q), lo_q)  # a non-finite group: its NaN quotient clamps low
+    return v.astype(np.int64), scale, offset
+
+
+def int_dequant_reference(codes, scale, offset=None):
+    """fp32 ``fmaf(code, scale, offset)`` per element, like ``dequant_one``."""
+    off = np.zeros_like(scale) if offset is None else offset
+    return fmaf(codes.astype(np.float32), scale[:, None], off[:, None])
+
+
+def pack_int(codes, bits, sym):
+    """Byte layout of ``quantize``'s codes: int8 (asymmetric biased by -128), or 4-bit nibbles, low nibble first."""
+    c = codes.reshape(codes.shape[0], -1)
+    if bits == 8:
+        return (c if sym else c - 128).astype(np.int8)
+    n = c & 0xF
+    return (n[:, 0::2] | (n[:, 1::2] << 4)).astype(np.uint8).view(np.int8)
+
+
+# ---- minifloats ----
+FP_FORMATS = {"e4m3": (8, 3), "e5m2": (8, 2), "e3m2": (6, 2), "e2m1": (4, 1), "e4m7": (12, 7)}
+
+
+def fp_grid(fmt):
+    """``(values float64, codes int64)`` of every finite non-negative value of ``fmt``, ascending, by enumerating the
+    codes: the hardware FP8 formats through torch's float8 dtypes, the software formats (no inf / NaN codes) from the
+    sign / exponent / mantissa fields."""
+    bits, m = FP_FORMATS[fmt]
+    if bits == 8:
+        dt = torch.float8_e4m3fn if m == 3 else torch.float8_e5m2
+        vals = torch.arange(128, dtype=torch.uint8).view(dt).double().numpy()
+        codes = np.arange(128)
+        ok = np.isfinite(vals)
+        return vals[ok], codes[ok]
+    e = bits - 1 - m
+    bias = 2**(e - 1) - 1
+    codes = np.arange(2**(bits - 1))
+    ef, mf = codes >> m, codes & (2**m - 1)
+    vals = np.where(ef == 0, mf * 2.0**(1 - bias - m), (1 + mf * 2.0**-m) * 2.0**(ef.astype(np.float64) - bias))
+    return vals, codes
+
+
+def fp_round(v, fmt, ties_even=None):
+    """Codes of fp32 values ``v`` (already divided by the scale) rounded to the nearest ``fmt`` value, saturating at
+    the format's maximum: ties to even for FP8 (the hardware conversion), away from zero for the software formats
+    (``ties_even`` overrides that).
+    The sign bit is the sign of ``v`` (FP8) or ``v < 0`` (software formats, whose encoder never writes -0 for a zero);
+    a NaN gives the FP8 NaN code or the maximum."""
+    bits, m = FP_FORMATS[fmt]
+    vals, codes = fp_grid(fmt)
+    v = np.asarray(v, np.float32).astype(np.float64)
+    a = np.abs(v)
+    nan = np.isnan(a)
+    a = np.where(nan, vals[-1], np.minimum(a, vals[-1]))
+    lo = np.clip(np.searchsorted(vals, a, side="right") - 1, 0, len(vals) - 1)
+    hi = np.minimum(lo + 1, len(vals) - 1)
+    dlo, dhi = a - vals[lo], vals[hi] - a
+    if ties_even is None:
+        ties_even = bits == 8
+    tie_hi = (codes[hi] & 1) == 0 if ties_even else np.ones_like(dlo, dtype=bool)
+    c = np.where((dhi < dlo) | ((dhi == dlo) & tie_hi & (hi != lo)), codes[hi], codes[lo])
+    neg = np.signbit(v) if bits == 8 else (v < 0)
+    c = np.where(neg, c | (1 << (bits - 1)), c)
+    if bits == 8:
+        c = np.where(nan, 0x7F, c)
+    return c.astype(np.int64)
+
+
+def fp_decode(codes, fmt):
+    """float64 value of every code (NaN for the FP8 NaN codes)."""
+    bits, m = FP_FORMATS[fmt]
+    if bits == 8:
+        dt = torch.float8_e4m3fn if m == 3 else torch.float8_e5m2
+        return torch.from_numpy(np.asarray(codes, np.uint8)).view(dt).double().numpy()
+    vals, _ = fp_grid(fmt)
+    codes = np.asarray(codes)
+    mag = vals[codes & (2**(bits - 1) - 1)]
+    return np.where(codes >> (bits - 1), -mag, mag)
+
+
+def fp_max(fmt):
+    return fp_grid(fmt)[0][-1]
+
+
+def fp_quant_reference(x, groups, fmt):
+    """Emulation of ``fp_quantize_kernel`` (round to nearest): ``(codes int64 [groups, gs], scale fp32 [groups])``."""
+    g = _np32(x).reshape(groups, -1)
+    with np.errstate(invalid="ignore"):
+        amax = np.abs(g).max(axis=1)
+        scale = group_scale(amax, np.isfinite(amax), np.float32(fp_max(fmt)))
+    return fp_round(to_grid(g, scale[:, None]), fmt), scale
+
+
+def fp_dequant_reference(codes, scale, fmt):
+    """fp32 ``decode(code) * scale`` per element."""
+    return (fp_decode(codes, fmt).astype(np.float32) * np.asarray(scale, np.float32)[:, None]).astype(np.float32)
+
+
+def pack_bits(codes, bits):
+    """Codes of ``bits`` width written little-endian into one byte stream per group (rows), padded to whole bytes."""
+    c = np.asarray(codes, np.int64).reshape(codes.shape[0], -1)
+    rows, n = c.shape
+    bitarr = ((c[:, :, None] >> np.arange(bits)) & 1).reshape(rows, n * bits)
+    pad = (-bitarr.shape[1]) % 8
+    bitarr = np.concatenate([bitarr, np.zeros((rows, pad), np.int64)], axis=1)
+    return (bitarr.reshape(rows, -1, 8) << np.arange(8)).sum(axis=2).astype(np.uint8)
+
+
+def quant_cases(groups, gs, dtype, bits, sym, gen, tiny=True):
+    """``groups`` groups of ``gs`` values in ``dtype``, the first ones the edges where codecs go wrong, the rest random
+    with group magnitudes across 2^-20 .. 2^20 (2^-10 .. 2^10 in fp16):
+    0. every value on an exact ``x / scale = k + 1/2`` tie, with +-amax (symmetric) or lo / hi (asymmetric) present;
+    1. a constant group (hi == lo); 2. an all-zero group; 3. a negative-only group;
+    4. a tiny group (amax about 1e-38, so ``1/scale`` overflows to inf; zeros among it) unless ``tiny`` is false;
+    5. a group with a huge (finite) range."""
+    x = torch.randn(groups, gs, generator=gen, dtype=torch.float64)
+    e = 10 if dtype == torch.float16 else 20
+    x *= torch.exp2(torch.randint(-e, e + 1, (groups, 1), generator=gen).double())
+    huge = x[min(5, groups - 1)] / x[min(5, groups - 1)].abs().max() * (6e4 if dtype == torch.float16 else 1e36)
+    s = 2.0**-3
+    half = 2**(bits - 1)
+    if sym:
+        k = torch.randint(-half, half - 1, (gs, ), generator=gen).double()
+        ties = (k + 0.5) * s
+        ties[0], ties[-1] = half * s, -half * s
+    else:
+        k = torch.randint(0, 2 * half - 1, (gs, ), generator=gen).double()
+        ties = (k - half + 0.5) * s
+        ties[0], ties[-1] = -half * s, half * s
+    rows = [ties, torch.full((gs, ), -0.3), torch.zeros(gs), -x[min(3, groups - 1)].abs() - 1.0]
+    if tiny:
+        t = x[min(4, groups - 1)] / x[min(4, groups - 1)].abs().max() * 1e-38
+        t[::3] = 0.0
+        rows.append(t)
+    rows.append(huge)
+    for i, r in enumerate(rows[:groups]):
+        x[i] = r
+    # + 0 turns the -0s of underflowed values into +0: which of two equal zeros a min reduction keeps is unspecified
+    return (x.to(dtype) + 0.0).reshape(-1)
+
+
+def loco_reference(x, err, groups, bits, beta, reset):
+    """Emulation of ``loco_quantize_kernel``: ``comp = x + err``; codes of ``comp``; the error slice becomes
+    ``fmaf(beta, err, (1 - beta) * fmaf(-code, scale, comp))`` (0 on reset), and stays as it was in a non-finite
+    group.  Returns ``(codes, scale, new err [groups, gs])``."""
+    e = _np32(err).reshape(groups, -1)
+    comp = (_np32(x).reshape(groups, -1) + e).astype(np.float32)
+    codes, scale, _ = int_quant_reference(comp, groups, bits, True)
+    b = np.float32(beta)
+    if reset:
+        upd = np.zeros_like(comp)
+    else:
+        upd = fmaf(b, e, ((np.float32(1) - b) * fmaf(-codes.astype(np.float32), scale[:, None], comp)).astype(np.float32))
+    return codes, scale, np.where(np.isfinite(scale)[:, None], upd, e).astype(np.float32)
+
+
+def reduce_reference(codes, scale, offset, peers, bits, sym, err=None, err_beta=0.0):
+    """Emulation of ``dequant_reduce_kernel`` over input groups ``[peers * out_groups]``: the dequantized chunks summed
+    in peer order in fp32, ``fmaf(err_beta, err, sum)``, requantized; the error slice becomes
+    ``sum - fmaf(code, scale, offset)`` unless the group is non-finite.  Returns ``(codes, scale, offset, new err)``."""
+    deq = int_dequant_reference(codes, scale, offset)
+    out_groups = deq.shape[0] // peers
+    deq = deq.reshape(peers, out_groups, -1)
+    acc = np.zeros(deq.shape[1:], np.float32)
+    for k in range(peers):
+        acc = (acc + deq[k]).astype(np.float32)
+    if err is not None:
+        acc = fmaf(np.float32(err_beta), _np32(err).reshape(acc.shape), acc)
+    c2, s2, o2 = int_quant_reference(acc, out_groups, bits, sym)
+    new = None
+    if err is not None:
+        new = (acc - int_dequant_reference(c2, s2, o2)).astype(np.float32)
+        new = np.where(np.isfinite(s2)[:, None], new, _np32(err).reshape(acc.shape))
+    return c2, s2, o2, new
+
+
+def fp_cases(fmt, groups, gs, gen):
+    """Group 0 holds, in units of the scale (its amax is the format maximum, so the scale is 1), every grid value,
+    every midpoint (ties), values one fp32 ulp either side of them (the subnormal band and each mantissa rollover into
+    the next binade included); group 1 is all zeros, group 2 tiny (amax 1e-38, zeros among it), the rest random
+    across 2^-24 .. 2^4 of their amax."""
+    vals, _ = fp_grid(fmt)
+    mids = ((vals[:-1] + vals[1:]) / 2).astype(np.float32)
+    special = np.concatenate([vals.astype(np.float32), mids, np.nextafter(mids, np.float32(0)),
+                              np.nextafter(mids, np.float32(np.inf))])
+    special = np.concatenate([special, -special])
+    x = torch.randn(groups, gs, generator=gen, dtype=torch.float64)
+    x *= torch.exp2(torch.randint(-24, 5, (groups, gs), generator=gen).double())
+    sp = torch.from_numpy(special).double()
+    take = sp[torch.randint(0, sp.numel(), (gs, ), generator=gen)]
+    take[:min(gs, sp.numel())] = sp[torch.randperm(sp.numel(), generator=gen)[:gs]]
+    take[0] = vals[-1]
+    x[0] = take
+    x[1] = 0.0
+    if groups > 2:
+        x[2] = x[2] / x[2].abs().max() * 1e-38
+        x[2, ::3] = 0.0
+    return x.float().reshape(-1)
