@@ -311,20 +311,17 @@ paged_decode_mma_kernel(const T* __restrict__ q, const T* __restrict__ cache, T*
     const T* kbase = cache + static_cast<int64_t>(kvh) * D;
     const T* vbase = kbase + static_cast<int64_t>(hkv) * D;
 
-    // query fragments (scaled), zero rows for g >= rep
+    // query fragments as stored, zero rows for g >= rep.  The softmax scale is applied to the fp32 scores after the MMA:
+    // q * scale rounded back to bf16 / fp16 would add a relative error of up to 2^-9 / 2^-12 to every logit.
     Vec16 qv[NC];
 #pragma unroll
     for (int i = 0; i < NC; ++i) {
-        float f[8];
         if (g < rep) {
-            Elem<T>::unpack(ld_plain(q + static_cast<int64_t>(t) * q_stride + static_cast<int64_t>(kvh * rep + g) * D + 32 * i + 8 * tq), f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] *= scale;
+            qv[i] = ld_plain(q + static_cast<int64_t>(t) * q_stride + static_cast<int64_t>(kvh * rep + g) * D + 32 * i + 8 * tq);
         } else {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = 0.f;
+            for (int w = 0; w < 4; ++w) qv[i].w[w] = 0u;
         }
-        qv[i] = Elem<T>::pack(f);
     }
     float o[NO][2];
 #pragma unroll
@@ -366,8 +363,8 @@ paged_decode_mma_kernel(const T* __restrict__ q, const T* __restrict__ cache, T*
                 MmaT<T>::mma(s[nt][0], s[nt][1], z0, z1, qv[i].w[2], qv[i].w[3], kx[nt][i].w[2], kx[nt][i].w[3]);
             }
             const int key = kb + 8 * nt + 2 * tq;
-            if (key >= k1) s[nt][0] = -INFINITY;
-            if (key + 1 >= k1) s[nt][1] = -INFINITY;
+            s[nt][0] = key < k1 ? s[nt][0] * scale : -INFINITY;
+            s[nt][1] = key + 1 < k1 ? s[nt][1] * scale : -INFINITY;
         }
         // ---- online softmax for row g (values spread over the 4 t-lanes)
         float mx = fmaxf(fmaxf(s[0][0], s[0][1]), fmaxf(s[1][0], s[1][1]));

@@ -53,6 +53,19 @@ top_k_gating_kernel(const T* __restrict__ logits, int32_t* __restrict__ expert_i
             if (e < E) probs_out[static_cast<int64_t>(warp) * E + e] = v[j] * inv;
         }
     }
+    // A NaN or +inf logit, or a row without a finite logit, makes the sum NaN (it is >= 1 otherwise) and leaves nothing to
+    // rank: the row routes to experts 0..K-1 with NaN weights, so the NaN reaches the layer output and every id and
+    // count index stays in range.  `sum` is the same in every lane, so the whole warp takes this branch.
+    if (sum != sum) {
+        if (lane == 0) {
+            for (int k = 0; k < K; ++k) {
+                expert_ids[static_cast<int64_t>(warp) * K + k] = k;
+                weights[static_cast<int64_t>(warp) * K + k] = __int_as_float(0x7fffffff);
+                atomicAdd(counts + k, 1);
+            }
+        }
+        return;
+    }
     float wsum = 0.f;
     float wk[kMaxTopK];
     int ek[kMaxTopK];
@@ -300,8 +313,9 @@ kv_rotary_append_kernel(T* __restrict__ qkv, T* __restrict__ cache, const float*
         T* base = row + static_cast<int64_t>(h) * d;
         const float a = Elem<T>::to_f(base[j]), b = Elem<T>::to_f(base[j + half]);
         const float c = cos_t[static_cast<int64_t>(pos) * half + j], s = sin_t[static_cast<int64_t>(pos) * half + j];
-        base[j] = Elem<T>::from_f(a * c - b * s);
-        base[j + half] = Elem<T>::from_f(b * c + a * s);
+        // explicit fmas: the rounding is fixed by the source, not by the compiler's contraction choices
+        base[j] = Elem<T>::from_f(fmaf(a, c, -(b * s)));
+        base[j + half] = Elem<T>::from_f(fmaf(b, c, a * s));
     }
     __syncthreads();
     // append k, v

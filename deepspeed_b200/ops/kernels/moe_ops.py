@@ -17,7 +17,8 @@ def _p(t):
 
 def top_k_gating(logits, k, normalize=True):
     """Fused softmax + top-k (inference path, no autograd).  Returns ids [T,k] int32, weights [T,k] fp32,
-    counts [E] int32."""
+    counts [E] int32.  Ties go to the lowest expert index.  A row whose softmax is not finite (a NaN or +inf logit, or no
+    finite logit) routes to experts 0..k-1 with NaN weights."""
     T, E = logits.shape
     if logits.is_cuda:
         ids = torch.empty(T, k, dtype=torch.int32, device=logits.device)
@@ -28,9 +29,16 @@ def top_k_gating(logits, k, normalize=True):
         N.check(rc, "top_k_gating")
         return ids, w, counts
     probs = torch.softmax(logits.float(), dim=-1)
-    w, ids = probs.topk(k, dim=-1)
+    w, ids = torch.sort(probs, dim=-1, descending=True, stable=True)  # stable: ties to the lowest index
+    w, ids = w[:, :k].contiguous(), ids[:, :k].contiguous()
     if normalize:
         w = w / w.sum(-1, keepdim=True)
+    # a NaN or +inf logit, or a row without a finite logit, leaves nothing to rank (the kernel's contract): experts
+    # 0..k-1 with NaN weights
+    bad = torch.isnan(probs).any(-1)
+    if bool(bad.any()):
+        ids[bad] = torch.arange(k, dtype=ids.dtype)
+        w[bad] = float("nan")
     counts = torch.bincount(ids.reshape(-1), minlength=E).to(torch.int32)
     return ids.to(torch.int32), w, counts
 

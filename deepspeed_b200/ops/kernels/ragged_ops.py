@@ -12,6 +12,7 @@ import os
 import torch
 
 from deepspeed_b200.ops import native as N
+from deepspeed_b200.ops.quantizer.quantizer import _fma32
 
 
 _ws = {}
@@ -27,9 +28,32 @@ def _decode_ws(device, n_acc, n_ml):
     return ent
 
 
-def _decode_eligible(qkv, hq, hkv, d):
-    return (qkv.dtype in (torch.bfloat16, torch.float16) and d in (64, 128, 256) and hq % hkv == 0
-            and hq // hkv in (1, 2, 4, 8) and qkv.shape[1] % 8 == 0)
+def _decode_eligible(dtype, hq, hkv, d, q_stride):
+    return (dtype in (torch.bfloat16, torch.float16) and d in (64, 128, 256) and hq % hkv == 0
+            and hq // hkv in (1, 2, 4, 8) and q_stride % 8 == 0)
+
+
+def paged_attention_path(dtype, hq, hkv, d, q_stride):
+    """The CUDA kernel ``paged_attention`` runs for this problem: ``"mma"`` (tensor-core split-KV decode, d 64 / 128),
+    ``"cuda_core"`` (split-KV decode, d 256 or with ``DSB200_PAGED_DECODE_MMA=0``) or ``"generic"`` (one CTA per query
+    head: fp32, other head dims or head ratios, or ``DSB200_PAGED_V1=1``)."""
+    if not _decode_eligible(dtype, hq, hkv, d, q_stride) or os.environ.get("DSB200_PAGED_V1", "0") == "1":
+        return "generic"
+    mma = not os.environ.get("DSB200_PAGED_DECODE_MMA", "1").startswith("0")
+    return "mma" if mma and d in (64, 128) else "cuda_core"
+
+
+def decode_splits(tokens, hkv, max_ctx):
+    """KV splits of the decode kernels: enough that (tokens x kv_heads x splits) covers the 132 SMs a few times over, at
+    most 32, and at least 256 cache positions per split.  It depends only on static shapes (graph-capturable: no
+    device->host read of the positions)."""
+    # the tensor-core kernel runs 2 CTAs per SM: one full wave (296 CTAs) is enough, every extra KV split costs a
+    # partial-result round trip (measured: 118 us at 296 vs 130 us at 592 for 64 seqs x 2048 ctx)
+    target = int(os.environ.get("DSB200_PAGED_CTA_TARGET", "296" if os.environ.get("DSB200_PAGED_DECODE_MMA", "1") != "0" else "592"))
+    nsplit = 1
+    while tokens * hkv * nsplit < target and nsplit < 32 and max_ctx // (nsplit * 2) >= 256:
+        nsplit *= 2
+    return nsplit
 
 
 def _p(t):
@@ -76,8 +100,9 @@ def kv_rotary_append(qkv, cache, cos, sin, seq_of, pos_of, block_table, hq, hkv,
         s = sin[pos_of.long()][:, None, :].to(torch.float32)
         rot = v[:, :hq + hkv].float()
         a, b = rot[..., :half].clone(), rot[..., half:rot_dim].clone()
-        v[:, :hq + hkv, :half] = (a * c - b * s).to(qkv.dtype)
-        v[:, :hq + hkv, half:rot_dim] = (b * c + a * s).to(qkv.dtype)
+        # the kernel's fmaf(a, c, -(b * s)) and fmaf(b, c, a * s), rounded the same way
+        v[:, :hq + hkv, :half] = _fma32(a, c, -(b * s)).to(qkv.dtype)
+        v[:, :hq + hkv, half:rot_dim] = _fma32(b, c, a * s).to(qkv.dtype)
     blk = block_table[seq_of.long(), (pos_of // block_size).long()].long()
     slot = (pos_of % block_size).long()
     cache[blk, slot] = v[:, hq:].reshape(T, 2, hkv, d)
@@ -91,17 +116,8 @@ def paged_attention(qkv, cache, seq_of, pos_of, block_table, hq, hkv, d, block_s
     max_blocks = block_table.shape[1]
     if qkv.is_cuda:
         out = torch.empty(T, hq * d, dtype=qkv.dtype, device=qkv.device)
-        if _decode_eligible(qkv, hq, hkv, d) and os.environ.get("DSB200_PAGED_V1", "0") != "1":
-            # split the KV range so (tokens x kv_heads x splits) covers the 132 SMs a few times over; the split count
-            # depends only on static shapes (graph-capturable: no device->host read of the positions)
-            max_ctx = max_blocks * block_size
-            nsplit = 1
-            ctas = T * hkv
-            # the tensor-core kernel runs 2 CTAs per SM: one full wave (296 CTAs) is enough, every extra KV split costs a
-            # partial-result round trip (measured: 118 us at 296 vs 130 us at 592 for 64 seqs x 2048 ctx)
-            target = int(os.environ.get("DSB200_PAGED_CTA_TARGET", "296" if os.environ.get("DSB200_PAGED_DECODE_MMA", "1") != "0" else "592"))
-            while ctas * nsplit < target and nsplit < 32 and max_ctx // (nsplit * 2) >= 256:
-                nsplit *= 2
+        if paged_attention_path(qkv.dtype, hq, hkv, d, qkv.shape[1]) != "generic":
+            nsplit = decode_splits(T, hkv, max_blocks * block_size)
             ws_acc, ws_ml = _decode_ws(qkv.device, T * hq * nsplit * d, T * hq * nsplit * 2) if nsplit > 1 else (None, None)
             rc = N.cuda().dsb_paged_decode(_p(qkv), _p(cache), _p(out), _p(ws_acc), _p(ws_ml), _p(seq_of), _p(pos_of),
                                            _p(block_table), T, hq, hkv, d, qkv.shape[1], block_size, max_blocks,

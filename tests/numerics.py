@@ -1082,3 +1082,223 @@ def fp_cases(fmt, groups, gs, gen):
         x[2] = x[2] / x[2].abs().max() * 1e-38
         x[2, ::3] = 0.0
     return x.float().reshape(-1)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ragged inference: paged attention, MoE gating, weight-only quantized GEMMs (csrc/cuda/attention.cu, moe_ragged.cu,
+# wq_gemm.cu, wq_tc_gemm.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+U_OUT = {torch.bfloat16: 2.0**-8, torch.float16: 2.0**-11, torch.float32: U}  # unit roundoff of each storage type
+
+
+def paged_rows(cache, block_table, seq, n, block_size):
+    """``(k, v)`` ``[n, hkv, d]`` in the stored dtype: the first ``n`` cached positions of sequence ``seq``, read through
+    its block table (position j lives in block ``block_table[seq, j // block_size]``, slot ``j % block_size``)."""
+    j = torch.arange(n, device=cache.device)
+    blk = block_table[seq].to(cache.device).long()[j // block_size]
+    kv = cache[blk, j % block_size]  # [n, 2, hkv, d]
+    return kv[:, 0], kv[:, 1]
+
+
+def paged_problem(ctx, hq, hkv, d, block_size, dtype, gen, peak=20.0, max_blocks=None, chunk=None):
+    """``(qkv, cache, seq_of, pos_of, block_table)`` on ``gen``'s device: a packed qkv batch and a paged cache.  Sequence i
+    has ``ctx[i]`` cached positions and one decode token at the last one (with ``chunk[i] = c`` its last c positions are
+    query tokens of one prefill chunk, each with its own causal limit).  The blocks are a random permutation of a pool
+    with spare blocks, so block tables are permuted and non-contiguous; table entries past a sequence point at real
+    blocks but are never read.  q and k are scaled so the largest ``|q.k| / sqrt(d)`` of a token is about ``peak``
+    (the max over ~1e3 keys of N(0, a^4) scores is ~3.5 a^2); values are N(0, 1)."""
+    dev = gen.device
+    need = [-(-c // block_size) for c in ctx]
+    pool = sum(need) + 3
+    perm = torch.randperm(pool, generator=gen, device=dev).to(torch.int32)
+    bt = torch.zeros(len(ctx), max(need) if max_blocks is None else max_blocks, dtype=torch.int32, device=dev)
+    o = 0
+    for i, n in enumerate(need):
+        bt[i, :n] = perm[o:o + n]
+        bt[i, n:] = perm[(o + n) % pool]
+        o += n
+    a = math.sqrt(peak / 3.5)
+    cache = torch.randn(pool, block_size, 2, hkv, d, generator=gen, device=dev) * a
+    cache[:, :, 1] /= a
+    seq_of, pos_of = [], []
+    for i, c in enumerate(ctx):
+        for p in range(c - (1 if chunk is None else chunk[i]), c):
+            seq_of.append(i)
+            pos_of.append(p)
+    qkv = torch.randn(len(seq_of), (hq + 2 * hkv) * d, generator=gen, device=dev) * a
+    i32 = dict(dtype=torch.int32, device=dev)
+    return qkv.to(dtype), cache.to(dtype), torch.tensor(seq_of, **i32), torch.tensor(pos_of, **i32), bt
+
+
+def paged_attention_bounds(q, cache, seq_of, pos_of, block_table, block_size, scale, dtype, nsplit=1, mma=False):
+    """``(ref, bound)`` float64 ``[T, hq, d]``: decode attention over the paged cache and a per-element bound on the
+    paged-attention kernels' output.  ``q [T, hq, d]`` holds the stored query rows; token t sees the cached keys
+    ``[0, pos_of[t]]`` of sequence ``seq_of[t]``; query head h reads kv head ``h // (hq / hkv)``.  ``scale`` is used as
+    the fp32 value the kernels receive.  ``nsplit``: KV splits merged at the end; ``mma``: the tensor-core kernel, which
+    rounds P to ``dtype`` before ``P V``.
+
+    Per (token, head), with ``x = scale q.k`` over the n visible keys and ``n_s = ceil(n / 4) + nsplit + 8`` bounding the
+    sequential fp32 updates any one accumulator sees (each of 4 warps walks a quarter of a split's keys, then the warps and
+    the splits are merged):
+
+    1. The score sums d exact products in fp32 (the tensor core may truncate): :func:`gemm_accum_error`.  The CUDA-core
+       kernels round ``q * scale`` to fp32 first and the tensor-core kernel rounds ``s * scale`` once: ``2 U scale |q||k|``
+       and ``U |x|`` cover either.
+    2. ``p = __expf(x - m)`` for a running max m: ex2.approx errs by 2 ulp (``4U``); the subtraction, the product with
+       ``log2 e`` and that constant's rounding each move the argument by ``U |x - m|``: ``3U (x_max - x + 2 e_max)``.
+       Results below ``2**-126`` flush to zero.
+    3. The running max is common to every p and cancels in ``o / l``, but each rescale ``alpha = __expf(m_old - m_new)``
+       and the warp and split merges weigh the keys seen before it: ``4U`` and ``3U |dm|`` per factor, the increments of
+       the max adding up to the row's span, and the rounding of ``acc * alpha`` and ``l * alpha``: ``(6 n_s + 30) U +
+       9U span`` as a relative error of p.
+    4. ``o`` and ``l`` sum at most ``n_s + 16`` terms each in fp32 (16 keys per MMA inside the tensor core): ``2 (n_s + 16)
+       U`` of ``sum p |v|`` and ``(n_s + 16) U`` of ``sum p``.
+    5. The tensor-core kernel rounds p to ``dtype`` for ``P V`` while ``l`` sums the fp32 p: ``u_dtype p |v|``.
+    6. ``o / l`` (or ``o * (1 / l)``) rounds at most three times, then once more to ``dtype`` (one :func:`ulp`)."""
+    T, hq, d = q.shape
+    hkv = cache.shape[3]
+    rep = hq // hkv
+    c = float(np.float32(scale))
+    dev = q.device
+    ref = torch.zeros(T, hq, d, dtype=torch.float64, device=dev)
+    bnd = torch.zeros_like(ref)
+    u_p = U_OUT[dtype] if mma else 0.0
+    for t in range(T):
+        n = int(pos_of[t]) + 1
+        k, v = paged_rows(cache, block_table, int(seq_of[t]), n, block_size)
+        n_s = -(-n // 4) + nsplit + 8
+        for g in range(hkv):
+            K, V = k[:, g].to(dev).double(), v[:, g].to(dev).double()
+            Q = q[t, g * rep:(g + 1) * rep].double()  # [rep, d]
+            s = Q @ K.t()
+            x = c * s
+            e_x = c * (gemm_accum_error(Q.abs() @ K.abs().t(), d) + 2 * U * (Q.abs() @ K.abs().t())) + U * x.abs()
+            xmax = x.max(-1, keepdim=True).values
+            emax = e_x.max(-1, keepdim=True).values
+            span = xmax - x.min(-1, keepdim=True).values + 2 * emax
+            dist = xmax - x + 2 * emax
+            lnrel = e_x + 3 * U * dist + (6 * n_s + 30) * U + 9 * U * span
+            P = torch.softmax(x, -1)
+            O = P @ V
+            Pe = P * torch.expm1(lnrel) + 2.0**-125
+            Pw = P + Pe
+            aV = V.abs()
+            num = Pe @ aV + (u_p + 2 * (n_s + 16) * U) * (Pw @ aV)
+            rho = Pe.sum(-1, keepdim=True) + (n_s + 16) * U * Pw.sum(-1, keepdim=True)
+            e_pre = (num + O.abs() * rho) / (1 - rho)
+            e_o = e_pre + _rel(3) * (O.abs() + e_pre)
+            ref[t, g * rep:(g + 1) * rep] = O
+            bnd[t, g * rep:(g + 1) * rep] = ulp(O.abs() + e_o, dtype) + e_o
+    return ref, bnd
+
+
+def gating_reference(logits, K, normalize):
+    """``(P, bound, order)``: float64 softmax of ``logits [T, E]``, a bound on the kernel's fp32 probabilities and the
+    stable descending order of P (ties to the lowest index).
+
+    The kernel forms ``v = __expf(x - max)`` (the subtraction rounds, ``__expf`` errs by ``4U`` plus ``2U |x - max|``
+    through its argument), sums the E values in fp32 and multiplies by ``1 / sum`` (two roundings): ``3U |x - max| +
+    (E + 8) U`` as a relative error of each probability, plus the ``2**-126`` below which ``__expf`` flushes."""
+    x = logits.double()
+    P = torch.softmax(x, -1)
+    y = (x - x.max(-1, keepdim=True).values).abs()
+    y = torch.where(torch.isfinite(y), y, 0.0)  # a -inf logit: p = 0 exactly
+    bound = P * torch.expm1(3 * U * y + (logits.shape[1] + 8) * U) + 2.0**-126
+    order = torch.sort(P, dim=-1, descending=True, stable=True).indices
+    return P, bound, order
+
+
+def check_gating(ids, w, counts, logits, K, normalize, what="gating"):
+    """The exact selection oracle for top-k gating.  For each row and rank r, the chosen expert ``i = ids[r]``:
+
+    * is in range and not chosen at an earlier rank;
+    * beats every expert e not chosen by rank r within the bounds: ``P[e] - b[e] <= P[i] + b[i]``;
+    * on an exact float64 tie ``P[e] == P[i]`` (equal logits: the kernel computes the same fp32 value), is the lower index.
+
+    Weights lie within the bound of ``P[i]`` (renormalized over the chosen K when ``normalize``: K fp32 adds and a
+    division on top), and ``counts`` is exactly the histogram of ``ids``."""
+    P, b, _ = gating_reference(logits, K, normalize)
+    T, E = P.shape
+    ids = ids.long().cpu()
+    P, b = P.cpu(), b.cpu()
+    assert bool(((ids >= 0) & (ids < E)).all()), f"{what}: id out of range"
+    taken = torch.zeros(T, E, dtype=torch.bool)
+    rows = torch.arange(T)
+    for r in range(K):
+        i = ids[:, r]
+        assert not bool(taken[rows, i].any()), f"{what}: an expert chosen twice (rank {r})"
+        pi, bi = P[rows, i], b[rows, i]
+        free = ~taken
+        free[rows, i] = False
+        beaten = free & ((P - b) > (pi + bi)[:, None])
+        tie = free & (P == pi[:, None]) & (torch.arange(E)[None, :] < i[:, None])
+        bad = beaten | tie
+        if bool(bad.any()):
+            t = int(bad.any(-1).nonzero()[0])
+            raise AssertionError(f"{what}: row {t} rank {r} chose {int(i[t])} (p={float(pi[t])!r}) over "
+                                 f"{bad[t].nonzero().flatten().tolist()[:8]}")
+        taken[rows, i] = True
+    Wsel = P.gather(1, ids)
+    Bsel = b.gather(1, ids)
+    if normalize:
+        S = Wsel.sum(-1, keepdim=True)
+        rel = (Bsel.sum(-1, keepdim=True) / S) + Bsel / Wsel.clamp_min(1e-300)
+        ref = Wsel / S
+        bound = ref * (torch.expm1(rel + (K + 2) * U)) + 2.0**-126
+    else:
+        ref, bound = Wsel, Bsel + U * Wsel
+    assert_within(w.cpu().double(), ref, bound, f"{what}: weights")
+    want = torch.bincount(ids.reshape(-1), minlength=E).to(torch.int32)
+    assert torch.equal(counts.cpu(), want), f"{what}: counts"
+
+
+def wq_codes(mode, N, K, gen, spread=True):
+    """Random weight codes ``[N, K]`` of a weight-only format and their float64 values: int8 in [-127, 127], int4 in
+    [-8, 7], every e4m3 code but NaN, every e3m2 code."""
+    if mode == "int8":
+        c = torch.randint(-127, 128, (N, K), generator=gen)
+        return c, c.double()
+    if mode == "int4":
+        c = torch.randint(-8, 8, (N, K), generator=gen)
+        return c, c.double()
+    fmt = "e4m3" if mode == "fp8" else "e3m2"
+    top = 256 if mode == "fp8" else 64
+    c = torch.randint(0, top, (N, K), generator=gen)
+    if mode == "fp8":
+        c = torch.where((c & 0x7F) == 0x7F, c - 1, c)  # no NaN codes
+    return c, torch.from_numpy(fp_decode(c.numpy(), fmt))
+
+
+def wq_pack(codes, mode):
+    """Byte layout the kernels read: int8 one byte per code, int4 two's-complement nibbles (low first), e4m3 one byte,
+    e3m2 a little-endian 6-bit stream (8 codes in 6 bytes); rows of ``K`` codes."""
+    N, K = codes.shape
+    c = codes.numpy().astype(np.int64)
+    if mode in ("int8", "fp8"):
+        return torch.from_numpy((c & 0xFF).astype(np.uint8).view(np.int8).copy())
+    if mode == "int4":
+        n = c & 0xF
+        return torch.from_numpy((n[:, 0::2] | (n[:, 1::2] << 4)).astype(np.uint8).view(np.int8).copy())
+    return torch.from_numpy(pack_bits(c.reshape(N, K), 6).view(np.int8).copy())
+
+
+def wq_bounds(x, wdq, bias, dtype, tile, k_steps, w_round=0.0):
+    """``(ref, bound)`` float64 ``[M, N]`` of ``x @ wdq^T + bias`` (``wdq`` the exact float64 dequantized weight) for the
+    weight-only GEMMs.  Products of the stored activations and the integer / minifloat codes are exact in fp32.
+
+    * ``tile`` products are summed in fp32 (the tensor core may truncate) before the group scale touches the sum: the
+      mma.sync GEMV accumulates each 64 (int8, fp8) or 128 (int4) element chunk into its own tile, ``2 tile U`` of
+      ``|x| |W|``;
+    * ``k_steps`` more fp32 roundings of the running sum: one ``fmaf(tile, scale, acc)`` per chunk, the 8-warp reduction
+      and the bias add for the GEMV, or the wgmma accumulation for the tensor-core GEMM;
+    * ``w_round``: the tensor-core GEMM rounds ``code * scale`` to fp32 and then to bf16 before the MMA (``2**-8 + U``
+      of every ``|W|``); the GEMV scales in fp32 instead and passes 0;
+    * the output's rounding to ``dtype``: one :func:`ulp`."""
+    ref = x.double() @ wdq.t()
+    if bias is not None:
+        ref = ref + bias.double()[None, :]
+    mag = x.double().abs() @ wdq.abs().t()
+    e = w_round * mag + (2 * tile + k_steps) * U * (1 + w_round) * mag
+    if bias is not None:
+        e = e + U * (ref.abs() + e)
+    return ref, ulp(ref.abs() + e, dtype) + e
